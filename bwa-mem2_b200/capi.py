@@ -373,7 +373,7 @@ class Context:
         return v.value
 
     def gather_probe(self, span_bytes: int = 0, mlp: int = 4, shape: int = 0) -> float:
-        """bm2_gather_probe: GB/s of random requests over the Occ table (shape 0: 64 B as 4 x 16 B, 1: 32 B as one 256-bit load, 2: 64 B as two)."""
+        """bm2_gather_probe: GB/s of random requests over the Occ table (shape 0: 64 B as 4 x 16 B, 1: 32 B as two 16-B loads of one sector, 2: 64 B as two such sectors)."""
         v = C.c_double()
         lib().bm2_gather_probe.argtypes = [C.c_void_p, C.c_ulonglong, C.c_int, C.c_int, C.POINTER(C.c_double)]
         self._check(lib().bm2_gather_probe(self._ctx, int(span_bytes), int(mlp), int(shape), C.byref(v)), "bm2_gather_probe")

@@ -1,4 +1,4 @@
-// bm2_common.cuh — shared declarations of the B200 seed-and-extend library (sm_100a only).
+// bm2_common.cuh — shared declarations of the H100 seed-and-extend library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>

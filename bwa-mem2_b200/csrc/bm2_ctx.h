@@ -25,7 +25,7 @@ struct DevIndex {                 // FM-index + reference resident in HBM (repli
 };
 
 struct bm2_ctx {
-    int device = 0, n_sm = 148;
+    int device = 0, n_sm = 132;
     cudaStream_t stream = nullptr, own_stream = nullptr, side_stream = nullptr;
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     bm2_mem_opt_t opt;

@@ -1,4 +1,4 @@
-// bsw.cu — banded affine-gap seed-extension (BSW) kernels for sm_100a.
+// bsw.cu — banded affine-gap seed-extension (BSW) kernels for sm_90a.
 //
 // Replaces BandedPairWiseSW::{getScores8,getScores16,scalarBandedSWAWrapper}
 // (reference src/bandedSWA.cpp:1970, :2664, :242).  Semantics = ksw_extend2 / scalarBandedSWA
@@ -98,7 +98,7 @@ __global__ void bsw_class_off_kernel(const int32_t *class_cnt, int32_t *class_of
 // The extension DP of one job (one thread).  `St` abstracts the per-column state storage.
 // ---------------------------------------------------------------------------------------------
 // (Measured: splitting H and E into separate narrow arrays - 2 LDS + 2 STS per cell instead of pack/unpack ALU
-// ops - made the kernel 6 % slower, profiles/r1d notes; the packed word stays.)
+// ops - made the kernel slower in an A/B; the packed word stays.)
 // The kernel is bound by the integer-ALU pipe (LOP3/SHF/VIMNMX/SEL/PRMT); the FMA pipe (IMAD) idles.  Field
 // extraction and packing are therefore written as multiply-adds so that they issue on the FMA pipe:
 //   x >> s == umulhi(x, 2^(32-s)),  x & (2^s-1) == x - (x >> s) * 2^s,  (a << s) | b == a * 2^s + b  (b < 2^s).
@@ -717,16 +717,15 @@ int bsw_launch_with_scratch(bm2_ctx *ctx_for_error, cudaStream_t stream, const B
     cub::DeviceRadixSort::SortPairs(nullptr, cub_bytes, keys_in, keys_out, idx_in, idx_out, n);
 
     BM2_CUDA_OK(cudaMemsetAsync(class_cnt, 0, 512, stream));
-    // Two-jobs-per-thread kernel (bsw_pair.cuh): bit-exact, but measured SLOWER than the thread-per-job kernel on B200
-    // (115 vs 89 ms per 1 M reads: the lanes of a warp spend the pre/post column segments of their pairs apart,
-    // profiles/r1k_bsw_pair_3gbp.md), so it is off unless BM2_BSW_PAIR=1 asks for it (experiments, tests).
+    // Two-jobs-per-thread kernel (bsw_pair.cuh): bit-exact, but slower than the thread-per-job kernel in an A/B (the lanes of
+    // a warp spend the pre/post column segments of their pairs apart), so it is off unless BM2_BSW_PAIR=1 asks for it (experiments, tests).
     const char *pair_env = getenv("BM2_BSW_PAIR");
     const int pair_ok = (pair_env && pair_env[0] == '1' && p2_params_ok(prm)) ? 1 : 0;
     bsw_keys_kernel<<<(n + 255) / 256, 256, 0, stream>>>(d_jobs, n, prm.a, pair_ok, d_qbase, keys_in, idx_in, class_cnt);
     BM2_CUDA_OK(cub::DeviceRadixSort::SortPairs(cub_tmp, cub_bytes, keys_in, keys_out, idx_in, idx_out, n, 0, 32, stream));
     bsw_class_off_kernel<<<1, 32, 0, stream>>>(class_cnt, class_off);
 
-    int dev = 0, n_sm = 148;
+    int dev = 0, n_sm = 132;
     BM2_CUDA_OK(cudaGetDevice(&dev));
     BM2_CUDA_OK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
     if (dev < 0 || dev >= BSW_MAX_DEV) { bm2_set_error(ctx_for_error, "bsw: device ordinal out of range"); return 1; }
@@ -778,9 +777,9 @@ int bsw_launch_with_scratch(bm2_ctx *ctx_for_error, cudaStream_t stream, const B
             // threads per CTA: the size that keeps the most threads resident per SM (shared memory is what limits this kernel's
             // occupancy: 6 B per column pair and thread; 64- or 96-thread CTAs waste less of the 227 KB than 128-thread ones)
             // Band shrink of a row (first / last column with a non-zero state): 0 = scans over shared memory; 1 = the two columns at either edge
-            // from the words just written, then the scans: measured 2 % SLOWER than 0 (profiles/r2g_exp_knobs.log: the extra branches cost more
-            // than the loads they save); 2 (default) = only the ONE column at either edge from registers, then the scans: 42.0 against 42.4 ms
-            // (profiles/r2n_exp_knobs.log).  BM2_BSW_REGSHRINK selects (A/B); BM2_BSW_UNROLL8=1: the scans with the pair loop unrolled x8 (no gain).
+            // from the words just written, then the scans: slower than 0 in an A/B (the extra branches cost more
+            // than the loads they save); 2 (default) = only the ONE column at either edge from registers, then the scans (the fastest of the
+            // three in an A/B).  BM2_BSW_REGSHRINK selects (A/B); BM2_BSW_UNROLL8=1: the scans with the pair loop unrolled x8 (no gain).
             const char *rs_env = getenv("BM2_BSW_REGSHRINK");
             int reg_shrink = 3;
             if (rs_env && rs_env[0] == '0') reg_shrink = 0; else if (rs_env && rs_env[0] == '1') reg_shrink = 1;
@@ -788,7 +787,7 @@ int bsw_launch_with_scratch(bm2_ctx *ctx_for_error, cudaStream_t stream, const B
             const char *dyn_env = getenv("BM2_BSW_DYN");
             const int dyn = (dyn_env && dyn_env[0] == '0') ? 0 : 1;           // per-warp job counters: class_cnt[64 + c], zeroed with class_cnt above
             int nthr2 = 128, best_res = 0, best_cps = 1;
-            int t_lo = 128, t_hi = 128;           // measured (profiles/r2e_exp_knobs.log): 128-thread CTAs 50.1 ms, 96: 53.5, 64: 51.2, most-resident-threads choice 52.3
+            int t_lo = 128, t_hi = 128;           // 128-thread CTAs: faster than 96 / 64 and than the most-resident-threads choice in an A/B
             if (const char *e = getenv("BM2_BSW_NTHR")) { const int v = atoi(e); if (v == 64 || v == 96 || v == 128) t_lo = t_hi = v; }      // A/B measurements
             for (int t = t_hi; t >= t_lo; t -= 32) {
                 int cps = (int) (smem_budget / ((size_t) NP * 6 * t + 1024)); if (cps < 1) cps = 1; if (cps > max_ctas * (128 / t)) cps = max_ctas * (128 / t);

@@ -108,8 +108,8 @@ static int create_impl(bm2_ctx **out, int device, const bm2_index_desc *idx, con
     BM2_CUDA_OK(cudaSetDevice(device));
     cudaDeviceProp prop;
     BM2_CUDA_OK(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) {      // the library holds an sm_100a cubin only (arch-specific: no forward compatibility to sm_11x / sm_12x)
-        bm2_set_error(nullptr, "bm2_create: device is not sm_10x (library is built for sm_100a only)");
+    if (prop.major != 9 || prop.minor != 0) {      // the library holds an sm_90a cubin only (arch-specific: no forward compatibility)
+        bm2_set_error(nullptr, "bm2_create: device is not sm_90 (library is built for sm_90a only)");
         return 2;
     }
     bm2_ctx *ctx = new bm2_ctx();
@@ -384,11 +384,12 @@ extern "C" int bm2_gather64_gbs(bm2_ctx *ctx, unsigned long long span_bytes, dou
 }
 
 // ---- gather probe with selectable request shape and memory-level parallelism ---------------------------------------------
-// shape 0: 64 B per request as four 16-B loads of one thread (the shape of bm2_gather64_gbs); shape 1: 32 B per request as ONE
-// 256-bit load (LDG.E.256: the half-checkpoint of the device Occ layout, fm_device.cuh); shape 2: 64 B per request as two 256-bit
-// loads.  `mlp` independent requests per thread are in flight (1, 2, 4 or 8).  Reports GB/s of requested bytes.
+// shape 0: 64 B per request as four 16-B loads of one thread (the shape of bm2_gather64_gbs); shape 1: 32 B per request as one
+// sector read by two 128-bit loads (the half-checkpoint of the device Occ layout, fm_ld256 in fm_device.cuh); shape 2: 64 B per
+// request as two such sectors.  `mlp` independent requests per thread are in flight (1, 2, 4 or 8).  Reports GB/s of requested bytes.
 __device__ __forceinline__ void ld256(const void *p, unsigned long long &a, unsigned long long &b, unsigned long long &c, unsigned long long &d) {
-    asm volatile("ld.global.nc.L1::no_allocate.v4.u64 {%0,%1,%2,%3}, [%4];" : "=l"(a), "=l"(b), "=l"(c), "=l"(d) : "l"(p));
+    asm volatile("ld.global.nc.v2.u64 {%0,%1}, [%4];\n\t"
+                 "ld.global.nc.v2.u64 {%2,%3}, [%4+16];" : "=l"(a), "=l"(b), "=l"(c), "=l"(d) : "l"(p));
 }
 template <int MLP, int SHAPE>
 __global__ void __launch_bounds__(256) gather_probe_kernel(const char *__restrict__ tab, unsigned long long n_units, int iters, unsigned long long seed,

@@ -38,9 +38,8 @@ BM2_HD void cigar_push_d(uint32_t *cigar, int &n, int op, int len) {
 // fixed slot 2W).  Same arithmetic and the same backtrack bytes at the same indices as the loop over memory rows below, which it replaces when
 // the band fits: no loads on the dependent path at all (the memory version spent 91 cycles per issued instruction waiting for its rows).
 // Requires w <= W and qlen <= tlen + w (then the last row reaches column qlen and H[qlen] is its h1).
-// MEASURED SLOWER inside sam_kernel and cigar_kernel (profiles/r2j_*: 168 registers per thread, 2 x 34 slots of unrolled code per row; the SAM
-// stage's per-pair kernel 29.9 -> 43.7 ms, bm2_gen_cigar 4.13 -> 3.28 M alignments/s against the memory rows with hoisted loads below), so it is
-// compiled out unless BM2_CIGAR_REG_BAND=1 is defined (it passed the CIGAR / SAM parity tests on the GPU: profiles/r2j_tests.log).
+// slower inside sam_kernel and cigar_kernel in an A/B (168 registers per thread, 2 x 34 slots of unrolled code per row, against the memory
+// rows with hoisted loads below), so it is compiled out unless BM2_CIGAR_REG_BAND=1 is defined.
 #ifndef BM2_CIGAR_REG_BAND
 #define BM2_CIGAR_REG_BAND 0
 #endif
@@ -172,7 +171,7 @@ BM2_HD int global_align_d(int qlen, const uint8_t *qp, int qstride, int tlen, co
         // Four cells per trip with all their loads (H, E, query bases) issued before the first cell is computed: the loads of neighbouring
         // cells do not depend on each other (only h1 and f run along the row, in registers), so a thread keeps 12 loads in flight instead of
         // waiting for each in turn - the rows live in per-thread global memory and this loop was bound by their latency (round 2 profile of the
-        // SAM stage: 91 stall cycles per issued instruction, profiles/r2g_sam_kernel_staged.md).  Same arithmetic, same order.
+        // SAM stage).  Same arithmetic, same order.
         for (j = beg; j + 4 <= end; j += 4) {
             const int32_t m0 = H[j], m1 = H[j + 1], m2 = H[j + 2], m3 = H[j + 3];
             const int32_t e0 = E[j], e1 = E[j + 1], e2 = E[j + 2], e3 = E[j + 3];

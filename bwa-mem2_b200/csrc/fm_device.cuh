@@ -17,8 +17,8 @@
 // layout 0: the checkpoints as the index file holds them, {cp_count[4]; one_hot_bwt_str[4]} (CP_OCC, src/FMI_search.h:54-58).
 // layout 1 (device only, made in place at upload by occ_relayout_kernel, pipeline.cu): the same eight words ordered
 // {cnt0, cnt1, bits0, bits1 | cnt2, cnt3, bits2, bits3}: an interval extension by base a needs base a and ONE partner base, and the partner
-// is always in a's half ({0,1} or {2,3}, see fm_backward_ext), so one checkpoint costs ONE 32-byte sector fetched by ONE 256-bit load
-// (LDG.E.256) instead of both sectors of the 64-byte line through four 8-byte loads.
+// is always in a's half ({0,1} or {2,3}, see fm_backward_ext), so one checkpoint costs ONE 32-byte sector (two 128-bit loads, fm_ld256)
+// instead of both sectors of the 64-byte line through four 8-byte loads.
 struct FmIndexView {
     const bm2_cp_occ *cp_occ;
     const int8_t *sa_ms;
@@ -33,9 +33,12 @@ struct FmIndexView {
 };
 
 #if defined(__CUDA_ARCH__)
-// 32 bytes by one 256-bit load, read-only path, no L1 allocation (the checkpoints of a multi-GB table are never re-used from L1)
+// 32 bytes (one aligned sector) by two 128-bit loads on the read-only path: sm_90 has no 256-bit load.  Both halves are issued before
+// either is used and lie in the same sector, so the second can be served by the first one's L1 fill (not measured on its own; the
+// gather probe of bench.py, shapes 1 and 2, reports the request rate of this access).
 BM2_D void fm_ld256(const void *p, uint64_t &a, uint64_t &b, uint64_t &c, uint64_t &d) {
-    asm volatile("ld.global.nc.L1::no_allocate.v4.u64 {%0,%1,%2,%3}, [%4];" : "=l"(a), "=l"(b), "=l"(c), "=l"(d) : "l"(p));
+    asm volatile("ld.global.nc.v2.u64 {%0,%1}, [%4];\n\t"
+                 "ld.global.nc.v2.u64 {%2,%3}, [%4+16];" : "=l"(a), "=l"(b), "=l"(c), "=l"(d) : "l"(p));
 }
 #endif
 
@@ -214,8 +217,8 @@ BM2_HD void fm_smem_pass3(const FmIndexView &fm, const Q &q, int len, const Smem
 // interval whenever its size changes) followed by a backward phase (extend all remembered intervals to the left,
 // longest first, emitting SMEMs).  The start of the NEXT search of pass 1 depends on the forward phase only
 // (next_x), so all forward phases of a read form one chain and every backward phase is an independent task.
-// Running them as separate kernels keeps the lanes of a warp in the same loop (measured: the forward-only pass-3
-// kernel does 2.6x more extensions per second than the mixed automaton, profiles/r1d_smem_split_3gbp.md).
+// Running them as separate kernels keeps the lanes of a warp in the same loop (the forward-only pass-3 kernel does
+// several times more extensions per second than the mixed automaton did).
 
 // Forward phase(s).  single == false: pass 1, all searches of the read from x = 0 with min_intv 1
 // (getSMEMsAllPosOneThread, src/FMI_search.cpp:672-724); single == true: one search from (x0, min_intv), pass 2

@@ -5,8 +5,7 @@
 // second version of bm2_sam_pe, as bm2_extend_pairs is for the extension kernel.  The arithmetic is ksw_warp.cuh (32 lanes split the
 // query, two max-plus scans per row), checked on the host against the oracle and the reference's golden vectors.
 //
-// STATUS: parity-green on a B200 (tests/test_zzz_ksw_gpu.py; first run = the driver's GPU suite of round 1, GPUTEST_r01; static facts in
-// profiles/r1t_static_staged_rescue.md).  sam.cu's staged rescue launches the same arithmetic on a job table built on the device.
+// Parity: tests/test_zzz_ksw_gpu.py.  sam.cu's staged rescue launches the same arithmetic on a job table built on the device.
 #include "bm2_common.cuh"
 #include "bm2_ctx.h"
 #include "ksw_warp.cuh"

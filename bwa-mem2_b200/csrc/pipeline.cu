@@ -344,7 +344,7 @@ sa_kernel(FmIndexView fm, const bm2_smem *__restrict__ sm, const int64_t *__rest
         const int64_t step = x.s > max_occ ? x.s / max_occ : 1;
         sa[t] = fm_sa_of_row(fm, x.k + (t - slot_off[o]) * step, &lf);
     }
-    // one atomic per warp (12 M same-address atomics cost ~6 ms, profiles/r1d)
+    // one atomic per warp (millions of same-address atomics per step are not free)
     lf = __reduce_add_sync(0xffffffffu, lf);
     if ((threadIdx.x & 31) == 0 && lf) atomicAdd(&cnt->n_lf, (unsigned long long) lf);
 }
@@ -683,7 +683,7 @@ __device__ int ext_tail_read_warp(const ContigView &cv, const ExtParams &p, cons
 // I. one read per thread (grid-stride: the NW scratch `he` is per thread)
 template <int mode>             // separate instances: the warp-per-read code (more registers) must not cost the per-thread pass its occupancy (96)
 // (mode 1 at 4 CTAs per SM = 128 registers.  Compiled for 6 / 8 CTAs - 80 / 64 registers, 350-470 B of spills - it was no faster: 13.0 / 13.4 against
-// 12.6 ms, profiles/r2t_exp_knobs.log: more resident warps do not help this kernel.)
+// no faster in an A/B: more resident warps do not help this kernel.)
 __global__ void __launch_bounds__(128, mode ? 4 : 1)
 tail_kernel(ContigView cv, ExtParams ep, const uint8_t *__restrict__ ref, const uint8_t *__restrict__ codes, const int64_t *__restrict__ offs,
             const bm2_chain *__restrict__ chains, const bm2_seed *__restrict__ seeds, const int64_t *__restrict__ chain_off,
@@ -693,8 +693,8 @@ tail_kernel(ContigView cv, ExtParams ep, const uint8_t *__restrict__ ref, const 
     // Heavy reads (many regs: O(regs^2) post-filter, sorts, patch DP) would serialise with the 31 other reads of their
     // warp (ncu: 1.9 active lanes per instruction), so they get a WARP each (mode 1: reads in decreasing-work order; the
     // post-filter scan runs on all lanes, the rest on lane 0); light reads run one per thread (mode 0).
-    // (Round 2 measured the heavy reads in SHARED memory - records, sort keys and index array copied in and out by the warp: no faster at the
-    // same number of resident warps, 8.2 against 8.3 ms, and slower with fewer, 11.1 ms at 2 CTAs per SM, profiles/r2l_exp_knobs.log: the
+    // (The heavy reads in SHARED memory - records, sort keys and index array copied in and out by the warp - were no faster at the
+    // same number of resident warps, and slower with fewer: the
     // records of one read stay in L1 between lane 0's passes, so the sequential part is bound by its instructions, not by memory latency.)
     const int tid = blockIdx.x * blockDim.x + threadIdx.x, nthr = gridDim.x * blockDim.x;
     const int lane = threadIdx.x & 31;
@@ -824,7 +824,7 @@ int scan64(bm2_ctx *ctx, const int64_t *in, int64_t *out, int64_t n) {
 }
 
 // sorts (keys, vals) of n reads; result permutation in vals_out
-// Measured (profiles/r1b_chain_tail_r1b.md): grouping heavy reads into the same warps makes the thread-per-read
+// Measured: grouping heavy reads into the same warps makes the thread-per-read
 // chain/tail kernels 2-7x SLOWER (32 private n^2 scans per warp thrash L1/L2), so until those kernels are
 // warp-cooperative the reads keep their input order (the permutation is the identity).
 static const bool kSortReadsByWork = false;
@@ -921,9 +921,8 @@ int run_pipeline(bm2_ctx *ctx, const bm2_read_batch *rb, UpTo upto, BatchState &
     const int stripe = max_len + 2;
     // CTAs per SM the SMEM kernels' grids may occupy (BM2_SMEM_CTAS): fewer leave room for the extension kernels of
     // the other sub-batches in flight (memory-latency-bound search next to ALU-bound DP on the same SM)
-    // Measured (profiles/r1q_exp_smem_ctas.log, 1 M reads, 3 Gbp): unsplit batch 8 CTAs/SM: SMEM stage 47 ms against 55 ms with 10
-    // and 50 ms with 6 (the stage sits on the random-access roofline of HBM: more searches in flight only thrash L2 / the DRAM
-    // pages); four sub-batch lanes with 3-4 CTAs/SM each: 126.5-127.3 ms per step against 129.2-129.8 ms with 10.
+    // 8 CTAs/SM for the unsplit batch was faster than 6 or 10 in an A/B (the stage sits on the random-access roofline of HBM: more
+    // searches in flight only thrash L2 / the DRAM pages); four sub-batch lanes with 3-4 CTAs/SM each were faster than with 10.
     const int use_tokens = ctx->parent ? env_int("BM2_STAGE_TOKENS", 0, 0, 3) : 0;
     // (with the SMEM token only one lane is in the SMEM stage at a time: it gets the unsplit batch's 8 CTAs per SM)
     const int smem_ctas = env_int("BM2_SMEM_CTAS", (ctx->parent && !(use_tokens & 1)) ? 4 : 8, 1, 16);
@@ -946,7 +945,7 @@ int run_pipeline(bm2_ctx *ctx, const bm2_read_batch *rb, UpTo upto, BatchState &
     const size_t qsm = q_smem ? (size_t) ((max_len + 7) / 8) * 128 * 4 : 0;
     const int blocks_b = ctx->n_sm * smem_ctas;
     // BM2_STAGE_TOKENS: bit 0 = SMEM-stage token, bit 1 = extension-stage token (sub-batch lanes only).  Off by default:
-    // measured SLOWER (149-160 ms against 138 ms per 1 M-read step, profiles/r1o_exp_stage_tokens.log) - taking turns in
+    // slower in an A/B - taking turns in
     // a stage leaves the other lanes' host threads waiting at the token instead of queueing work.
     StageToken tok_smem((use_tokens & 1) ? &ctx->parent->tok_smem : nullptr);
     for (int attempt = 0; attempt < 3; ++attempt) {
@@ -1056,8 +1055,8 @@ int run_pipeline(bm2_ctx *ctx, const bm2_read_batch *rb, UpTo upto, BatchState &
     int32_t *wv_in = (int32_t *) ((char *) ctx->d[B_PERM].p + 2 * al((size_t) n * 4)), *d_perm = (int32_t *) ((char *) ctx->d[B_PERM].p + 3 * al((size_t) n * 4));
     work_keys_slots_kernel<<<(n + 255) / 256, 256, 0, st>>>(P<int64_t>(ctx, B_READ_SMEM_OFF), P<int64_t>(ctx, B_SLOT_OFF), n, wk_in, wv_in);
     if (sort_work(ctx, wk_in, wk_out, wv_in, d_perm, n, true)) return 1;             // decreasing number of seed slots
-    // light reads of the chain and tail kernels in work order instead of input order: measured no better (chain 13.4 against 12.8 ms, tail equal,
-    // profiles/r2m_exp_knobs.log: neighbouring reads share cache lines of the per-read arrays), so off unless BM2_LIGHT_SORTED=1
+    // light reads of the chain and tail kernels in work order instead of input order: no better in an A/B (neighbouring reads share
+    // cache lines of the per-read arrays), so off unless BM2_LIGHT_SORTED=1
     const int light_sorted = env_int("BM2_LIGHT_SORTED", 0, 0, 1);
     const int chain_heavy = env_int("BM2_CHAIN_HEAVY", 64, 1, 1 << 30);          // seed occurrences from which a read gets a warp
     const int chain_coop_min = env_int("BM2_CHAIN_COOP_MIN", 1024, 0, 1 << 30);      // seed occurrences from which a warp shares the chaining of a read
@@ -1291,8 +1290,8 @@ static int run_regs(bm2_ctx *ctx, const bm2_read_batch *rb, const uint8_t *d_cod
     struct Job { int first = 0, n = 0; std::vector<int64_t> offs; bm2_read_batch rb; BatchState bs; int rc = 0; };
     // (Round 2 also ran every lane over several smaller sub-batches in a row, each sub-batch's regs copied to the host on a copy stream under
     // the kernels of the following ones - the device -> host copies at the end of the step, 387 MB per 1 M reads, are the gap between the
-    // resident and the end-to-end number.  Bit-identical and SLOWER end to end: 111.3 ms with 2 x 4 sub-batches, 119.4 with 3 x 4, against
-    // 108.5 with 4, profiles/r2p_exp_knobs.log - eight 125 k-read sub-batches lose more in the kernels than the hidden copies give back.)
+    // resident and the end-to-end number.  Bit-identical and slower end to end in an A/B (2 x 4 and 3 x 4 sub-batches against 4): eight
+    // 125 k-read sub-batches lose more in the kernels than the hidden copies give back.)
     std::vector<Job> jobs((size_t) K);
     // cut points (multiples of 512 reads).  BM2_LANE_SKEW = s percent: lane k gets a share proportional to 100 + s * k instead of equal shares,
     // so that the lanes - which start together - leave the SMEM stage at different times (experiment: do unequal lanes overlap unlike stages better?)

@@ -8,10 +8,9 @@
 // and CIGAR pools - optimistic pools with a second wave for the pairs that overflow are the obvious next step).  The libm values the stage needs (log of small
 // integers, the insert-size term of mem_pair) are tabulated on the host with the host's libm, as the reference computes them.
 //
-// STATUS: parity-green on a B200 in all three rescue modes; timed in round 2 (profiles/r2a_bench_sam.json): the per-pair kernel is the
-// bottleneck (128 ms per 100 k pairs next to 32 ms for the window alignments of the staged mode).
+// Parity-tested in all three rescue modes (tests/test_zz_sam_gpu.py, tests/test_zzz_sam_staged_gpu.py); `bench.py --workload sam` times it.
 //
-// Staged rescue (the default since round 2; bm2_set_sam_staged / BM2_SAM_STAGED select 0 = per-pair, 1 = warp per window, 2 = thread per window): the local alignments of the rescue - the
+// Staged rescue (the default; bm2_set_sam_staged / BM2_SAM_STAGED select 0 = per-pair, 1 = warp per window, 2 = thread per window): the local alignments of the rescue - the
 // bulk of the stage's arithmetic - leave the per-pair thread.  sam_jobs_kernel lists, from the regions BEFORE any rescue, the windows the
 // rescue block of every pair can ask for (mate_jobs_pair_d); sam_ksw_jobs_kernel aligns them one window per warp (ksw_warp.cuh, the mate read
 // in place, reverse-complemented by addressing); the per-pair thread then looks its alignments up (MateKswTable) and computes one itself
@@ -111,7 +110,7 @@ sam_ksw_jobs_kernel(KswMat25 mat, int a_match, int min_seed_len, int o_del, int 
 }
 
 // stage 2, other formulation (staged mode 2): one window per THREAD over the same job table - the one-thread sweep of ksw_device.cuh (the arithmetic the
-// per-pair kernel runs, proven on the B200) with 32 windows of similar size per warp in lock step.  Per-thread scratch in global memory:
+// per-pair kernel runs) with 32 windows of similar size per warp in lock step.  Per-thread scratch in global memory:
 // [3 * (max_l + 16) ints H / E / best row][lcap ints scores][lcap ints rows][tcap bytes reversed target][max_l + 1 bytes reverse complement].
 __global__ void __launch_bounds__(128)
 sam_ksw_jobs_thread_kernel(KswMat25 mat, int a_match, int min_seed_len, int o_del, int e_del, int o_ins, int e_ins, const uint8_t *__restrict__ ref, int64_t ref_len,
@@ -298,8 +297,8 @@ int run_sam(bm2_ctx *ctx, const bm2_read_batch *reads, const bm2_alnreg_t *regs,
     ContigView cv; cv.l_pac = ctx->idx.l_pac; cv.n_seqs = ctx->idx.n_seqs; cv.ann_off = ctx->idx.ann_off; cv.ann_len = ctx->idx.ann_len; cv.ann_alt = ctx->idx.ann_alt;
     const int rescue = paired && !(o.flag & 0x20);
     int staged = ctx->sam_staged;
-    // default: staged, one window per warp - byte-identical records (tests/test_zzz_sam_staged_gpu.py) and 6x the per-pair mode on the 3 Gbp
-    // workload (profiles/r2a_bench_sam.json: 1.01 M against 0.17 M reads/s); BM2_SAM_STAGED / bm2_set_sam_staged select the other modes
+    // default: staged, one window per warp - byte-identical records (tests/test_zzz_sam_staged_gpu.py) and about 12x the per-pair mode on the 1 Gbp
+    // bench workload (H100); BM2_SAM_STAGED / bm2_set_sam_staged select the other modes
     if (staged < 0) { const char *e = getenv("BM2_SAM_STAGED"); staged = e ? atoi(e) : 1; if (staged < 0 || staged > 2) staged = 1; }
     if (!rescue) staged = 0;
     for (double &v : ctx->sam_ms) v = 0;
@@ -336,7 +335,13 @@ int run_sam(bm2_ctx *ctx, const bm2_read_batch *reads, const bm2_alnreg_t *regs,
         desc[(size_t) pr].caps = sam_pair_caps_d(sh, pes, o.max_matesw, rescue != 0, o.a, o.e_del);
         desc[(size_t) pr].pair = pr;
     }
-    const size_t budget = (size_t) 32 << 30;                // scratch + stripes of one wave (≈0.5 MB per pair of 151-bp reads with 8 regions each)
+    // scratch + stripes of one wave (≈0.5 MB per pair of 151-bp reads with 8 regions each): an eighth of the device memory that is free
+    // or already held by this context's wave buffers.  Up to four sibling contexts (bm2_mem -p 4) may each hold a wave at once, ensure()
+    // adds a quarter on top, and the seed-and-extend buffers of the next chunk need room beside them.
+    size_t dev_free = 0, dev_total = 0;
+    BM2_CUDA_OK(cudaMemGetInfo(&dev_free, &dev_total));
+    for (int b : { SB_ARENA, SB_RECS_W, SB_XA_W, SB_OPS_W, SB_MD_W }) dev_free += ctx->d[b].cap;
+    const size_t budget = std::min((size_t) 32 << 30, std::max((size_t) 1 << 30, dev_free / 8));
     size_t used[4] = { 0, 0, 0, 0 };                        // recs, xa, ops, md of the batch so far
     for (int w0 = 0; w0 < n_pairs_all;) {
         size_t arena = 0; int64_t nrec = 0, nxa = 0, nops = 0, nmd = 0; int w1 = w0;
@@ -422,9 +427,9 @@ int run_sam(bm2_ctx *ctx, const bm2_read_batch *reads, const bm2_alnreg_t *regs,
                 }
                 keyed[(size_t) k] = { gapped * 4096 + (int) (nreg > 4095 ? 4095 : nreg), (int32_t) k };
             }
-            // Measured (profiles/r2g_bench_sam*.json, 100 k pairs): the sorted order is SLOWER, 185 against 125 ms - the kernel is bound by the
+            // The sorted order was slower in an A/B - the kernel is bound by the
             // latency of its per-thread global-memory DP rows and backtrack bytes (91 stall cycles per issue on long scoreboard, 3 % of the issue
-            // slots, profiles/r2g_sam_kernel_staged.md), and neighbouring pairs share cache lines of regs / reads that the sort scatters.  Off
+            // slots), and neighbouring pairs share cache lines of regs / reads that the sort scatters.  Off
             // unless BM2_SAM_ORDER=1.
             const char *env = getenv("BM2_SAM_ORDER");
             if (env && env[0] == '1') std::stable_sort(keyed.begin(), keyed.end(), [](const std::pair<int, int32_t> &x, const std::pair<int, int32_t> &y) { return x.first < y.first; });

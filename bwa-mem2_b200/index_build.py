@@ -259,7 +259,12 @@ def make_big_reference(total_bp: int, seed: int = 1, n_contigs: int = 24, repeat
             seqs = torch.where(rc[:, None], (3 - seqs).flip(1), seqs)
             pos = torch.randint(0, total_bp - L - 1, (len(u),), device=device, generator=g)
             idx = pos[:, None] + torch.arange(L, device=device)[None, :]
-            G[idx.reshape(-1)] = seqs.reshape(-1)
+            # copies may overlap: an indexed write with repeated positions keeps an unspecified writer on the GPU, so keep the
+            # last copy in order explicitly (the same genome from the same seed on every run)
+            p, order = torch.sort(idx.reshape(-1), stable=True)
+            last = torch.ones_like(p, dtype=torch.bool)
+            last[:-1] = p[1:] != p[:-1]
+            G[p[last]] = seqs.reshape(-1)[order[last]]
     w = np.array([0.8 ** i for i in range(n_contigs)], dtype=np.float64)
     lens = np.maximum((w / w.sum() * total_bp).astype(np.int64), 1000)
     lens[0] += total_bp - lens.sum()

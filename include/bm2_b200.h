@@ -1,4 +1,4 @@
-/* bm2_b200.h — C ABI of libbm2b200.so: the B200-native seed-and-extend hot path of bwa-mem2.
+/* bm2_b200.h — C ABI of libbm2b200.so: the H100-native seed-and-extend hot path of bwa-mem2.
  *
  * Plain C, pointers and sizes only.  Every entry point names the reference interface it replaces
  * (file:line under bwa-mem2 @ 97978f95).  The reference has no FFI; the seam is the C++ function
@@ -107,7 +107,7 @@ const char *bm2_last_error(const bm2_ctx *ctx);   /* ctx may be NULL: last creat
 int  bm2_set_stream(bm2_ctx *ctx, void *cuda_stream);
 /* Seam 2 runs a batch as `k` sub-batches in flight (own CUDA streams and scratch, shared index): the SMEM stage is
  * bound by memory latency and the extension stage by the integer pipe, so sub-batches at different stages fill
- * each other's stalls (measured +17 % reads/s at k = 4 on B200).  A batch is only split when every sub-batch gets
+ * each other's stalls (more reads/s at k = 4 than unsplit).  A batch is only split when every sub-batch gets
  * at least `min_reads` reads; cuts are multiples of 512 reads so that results do not depend on k (the reference's
  * kt_for works in 512-read blocks, src/kthread.cpp:41-115).  Defaults: k = 4, min_reads = 16384; k = 1 turns it off.
  * The mem_collect_smem / mem_kernel1_core stage entries (bm2_collect_smems, bm2_seed_chain) always run unsplit. */
@@ -120,7 +120,7 @@ int  bm2_int_pipe_gops(bm2_ctx *ctx, double *gops_s32);
  * per interval extension) when no dependent address chain limits it.  Reported next to the HBM copy peak in bench.py. */
 int  bm2_gather64_gbs(bm2_ctx *ctx, unsigned long long span_bytes, double *gbs);
 /* The same probe with a selectable request shape and memory-level parallelism: shape 0 = 64 B as four 16-B loads of one thread,
- * 1 = 32 B as ONE 256-bit load (the half-checkpoint of the device Occ layout), 2 = 64 B as two 256-bit loads, 3 = 32 B by cp.async.bulk
+ * 1 = 32 B as two 16-B loads of one sector (the half-checkpoint of the device Occ layout), 2 = 64 B as two such sectors, 3 = 32 B by cp.async.bulk
  * into shared memory behind an mbarrier (the TMA path; at most 4 in flight per thread), 4 = shape 3 and shape 1 together (mlp of each); `mlp` (1, 2, 4, 8)
  * independent requests in flight per thread.  GB/s of requested bytes.  Decides whether the SMEM stage is bound by DRAM, by the
  * load/store unit's request rate or by latency (DESIGN.md section 4). */

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Offline study (CPU only): how many 64-byte index lines per read the SMEM stage pulls from DRAM, and what alternatives would save.
 Replays the accesses of the kernels' own search logic (fm_device.cuh compiled for the host, three passes) of N reads through an LRU cache
-that is scaled to the index (126 MB of L2 against the 6 GB Occ table of a 3 Gbp genome = 2.1 % of the table), for
+that is scaled to the index (50 MB of H100 L2 against the 6 GB Occ table of a 3 Gbp genome = 0.8 % of the table), for
   0  the current layout (64-byte checkpoint per 64 BWT rows),
   1  a half-size table (64-byte line per 128 rows: 2-bit packed BWT + counts),
   2  a k-mer table that answers the first k-1 extensions of every forward search with one fetch (k scaled with the genome),
@@ -26,7 +26,7 @@ def main():
     reads = np.load(reads_path)[:n]
     codes = np.ascontiguousarray(reads.reshape(-1)); offs = (np.arange(len(reads) + 1) * reads.shape[1]).astype(np.int64)
     table_bytes = (idx.desc.reference_seq_len // 64 + 1) * 64
-    cache_lines = int(126e6 / 6.0e9 * table_bytes / 64)
+    cache_lines = int(50e6 / 6.0e9 * table_bytes / 64)
     # k of the k-mer table: 12 at 6e9 BWT rows, one less per factor 4
     kk = max(6, int(round(12 - np.log(6.0e9 / idx.desc.reference_seq_len) / np.log(4))))
     out = np.zeros((4, 5, 3), np.float64)

@@ -130,6 +130,27 @@ REG_CMP_FIELDS = ("rb", "re", "qb", "qe", "rid", "score", "truesc", "sub", "alt_
                   "secondary", "secondary_all", "seedlen0", "frac_rep", "hash")
 
 
+def _regs_digest(off, cols):
+    import hashlib
+    h = hashlib.sha256(np.asarray(off, np.int64).tobytes())
+    for name, v in cols:
+        v = np.asarray(v)
+        h.update(name.encode() + np.ascontiguousarray(v.astype(np.float64 if v.dtype.kind == "f" else np.int64)).tobytes())
+    return h.hexdigest()
+
+
+def regs_digest(regs, off):
+    """SHA-256 of what regs_equal_to_dump compares, for REG_DT regs (ours): equal digests <=> regs_equal_to_dump(...) == []."""
+    return _regs_digest(off, [(f, regs[f]) for f in REG_CMP_FIELDS] + [("n_comp", (regs["n_comp_is_alt"] << 2) >> 2),
+                                                                        ("is_alt", (regs["n_comp_is_alt"] >> 30) & 3)])
+
+
+def dump_digest(dump_regs, dump_off):
+    """regs_digest of a reference regs dump (refdump.read_regs): the stored form of the reference's regs in tests/golden."""
+    return _regs_digest(dump_off, [(f, dump_regs[f]) for f in REG_CMP_FIELDS] + [("n_comp", dump_regs["n_comp"]),
+                                                                                  ("is_alt", dump_regs["is_alt"] & 3)])
+
+
 def regs_equal_to_dump(regs, off, dump_regs, dump_off):
     """Compare REG_DT regs (ours) with refdump.REG_DT regs (reference dump). Returns list of differing reads."""
     bad = []

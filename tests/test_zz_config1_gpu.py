@@ -1,4 +1,4 @@
-"""BASELINE.json configs[0] at its stated size through the GPU path: a 10 Mbp synthetic reference (several contigs, planted repeat families,
+"""Config 1 at its stated size through the GPU path: a 10 Mbp synthetic reference (several contigs, planted repeat families,
 N runs) indexed live by the unmodified reference's `bwa-mem2 index`, 10 000 synthetic 2x151 bp pairs, default mem_opt_t.  The pure reference
 run and the run whose worker_bwt + worker_aln are replaced by libbm2b200.so through the C ABI (ref_driver BM2_MODE=gpu) must print the same
 SAM - SAM diff = 0, as the config asks.  (tests/test_dropin_sam_gpu.py is the same check on the small committed golden set.)"""

@@ -1,7 +1,7 @@
 """GPU parity of seam 4 (bm2_sam_pe: mate rescue, pairing, MAPQ, CIGAR / NM / MD, SAM records, XA entries) through the C ABI: every
 SAM column and the NM MD AS XS XA pa tags of every line of the UNMODIFIED reference's output on C0 (tests/golden/c0.sam), and the
 oracle on flag variants and on the tandem-repeat reads (hundreds of regions per read).
-First run on a B200: profiles/r1s_zz_tests_gpu.log (8 passed).  The per-pair logic the kernel launches is also checked on the host
+The per-pair logic the kernel launches is also checked on the host
 (tests/test_oracle_sam_pe.py)."""
 import numpy as np
 import pytest

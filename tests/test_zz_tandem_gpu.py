@@ -1,7 +1,7 @@
 """GPU parity on reads inside short tandem repeats (tests/golden/tandem_*, see tests/test_chain_tree_cpu.py): hundreds of chains per
 read, chains with equal positions (the kernels keep the shape of the reference's chain B-tree, chain_tree_put_d), up to a thousand
 alignment regions per read, 16-bit extension jobs of 251-bp reads.  Through the C ABI, against the UNMODIFIED reference's regs
-(golden) and the oracle.  First run on a B200: profiles/r1s_zz_tests_gpu.log (2 passed); the same device logic is checked on the host by
+(golden) and the oracle.  The same device logic is checked on the host by
 tests/test_chain_tree_cpu.py."""
 import numpy as np
 import pytest

@@ -7,7 +7,7 @@ import pytest
 import ksw_util as ku
 import test_oracle_ksw as tk
 
-pytestmark = [pytest.mark.gpu]      # first B200 run: GPUTEST_r01 (passed); no xfail any more
+pytestmark = [pytest.mark.gpu]
 
 
 def test_golden_vectors_of_the_reference(pkg, golden_dir):

@@ -8,7 +8,7 @@ import pytest
 import test_oracle_sam_pe as tp
 from test_zz_sam_gpu import c0, _xa_strings          # noqa: F401  (fixture)
 
-pytestmark = [pytest.mark.gpu]      # first B200 run: GPUTEST_r01 (passed); no xfail any more
+pytestmark = [pytest.mark.gpu]
 
 
 def _run(capi, idx, opt, codes, offs, staged, pes=None):
