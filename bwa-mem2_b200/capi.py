@@ -404,10 +404,10 @@ class Context:
         return regs, off
 
     def counters(self):
-        v = (C.c_ulonglong * 5)()
+        v = (C.c_ulonglong * 7)()
         lib().bm2_last_counters.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
-        lib().bm2_last_counters(self._ctx, v, 5)
-        return dict(n_ext=v[0], n_lf=v[1], cells=v[2], retry_left=v[3], retry_right=v[4])
+        lib().bm2_last_counters(self._ctx, v, 7)
+        return dict(n_ext=v[0], n_lf=v[1], cells=v[2], retry_left=v[3], retry_right=v[4], jobs_skipped=v[5], reads_done_wave1=v[6])
 
     def stage_ms(self):
         names = C.POINTER(C.c_char_p)(); ms = C.POINTER(C.c_float)(); n = C.c_int()

@@ -41,6 +41,7 @@ struct bm2_ctx {
     std::vector<const char *> stage_names;
     std::vector<float> stage_ms;
     unsigned long long last_n_ext = 0, last_n_lf = 0, last_cells = 0, last_n_retry[2] = {0, 0};
+    unsigned long long last_jobs_skipped = 0, last_walk_done = 0;     // lazy extension: jobs never run, reads decided after the first wave
     // seam 2 sub-batches in flight (pipeline.cu run_regs): child contexts with their own streams, events and scratch;
     // they share this context's index (their idx_allocs stay empty)
     int n_lanes = 4, lane_min_reads = 16384;

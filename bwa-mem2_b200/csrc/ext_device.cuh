@@ -64,13 +64,22 @@ BM2_HD void seedcov_d(bm2_alnreg_t &a, const bm2_seed *seeds, int n) {
     }
 }
 
+// Per-reg extension state of the lazy extension (one byte per reg; see ext_walk_read_d):
+enum : uint8_t {
+    EXT_TODO = 0,       // not extended, not decided
+    EXT_DONE = 1,       // extended (or needs no extension: the seed spans the read)
+    EXT_SKIP = 2,       // not extended, and the walk proved the seed purged: never extended
+    EXT_NEED = 3        // to be extended by the next wave: the first seed of a chain, or the seed a walk stopped at
+};
+
 // Builds regs + jobs of one read.  chains/seeds: the read's finalized chains; regs, reg_chain,
 // reg_seed: the read's output stripe (one entry per seed, creation order); left/right jobs and their
 // reg ids (GLOBAL reg index = reg_base + local).  srt: scratch of >= max chain length uint64.
+// state (may be null): the regs' extension states for the lazy extension (EXT_NEED for the first seed of each chain).
 BM2_HD void ext_build_read_d(const ContigView &cv, const ExtParams &p, const bm2_chain *chains, int n_chain, const bm2_seed *seeds,
                              int l_query, int64_t read_code_off, int64_t chain_base, int64_t reg_base, bm2_alnreg_t *regs,
                              int32_t *reg_chain, int32_t *reg_seed, ExtJobRec *left, int32_t *left_reg, ExtJobRec *right,
-                             int32_t *right_reg, uint64_t *srt)
+                             int32_t *right_reg, uint64_t *srt, uint8_t *state = nullptr)
 {
     const int64_t l_pac = cv.l_pac;
     int n_reg = 0, nl = 0, nr = 0;
@@ -129,6 +138,7 @@ BM2_HD void ext_build_read_d(const ContigView &cv, const ExtParams &p, const bm2
                 seedcov_d(a, cs, n);
             }
             reg_copy(&regs[ai], &a); reg_chain[ai] = (int32_t) (chain_base + ci); reg_seed[ai] = si;
+            if (state) state[ai] = (!s.qbeg && s.qbeg + s.len == l_query) ? EXT_DONE : (k == n - 1 ? EXT_NEED : EXT_TODO);
             ++n_reg;
         }
     }
@@ -157,17 +167,65 @@ BM2_HD bool ext_fold_d(const ExtParams &p, bm2_alnreg_t &a, int is_right, int h0
 // The fields of a reg the post-filter scans, 32 B instead of the 112-B mem_alnreg_t (the scan is O(regs x seeds)).
 struct PfBox { int64_t rb, re; int32_t qb, qe, seedlen0, w; };
 
+BM2_HD PfBox pf_box_d(const bm2_alnreg_t &a) {
+    PfBox b; b.rb = a.rb; b.re = a.re; b.qb = a.qb; b.qe = a.qe; b.seedlen0 = a.seedlen0; b.w = a.w;
+    return b;
+}
+
+// The post-filter's test of seed s against the box of one earlier reg (src/bwamem.cpp:2964-2977): 0 = the reg is purged (not
+// counted), 1 = counted (v++), 2 = s lies on the reg's diagonal band (the scan stops).
+BM2_HD int pf_box_kind_d(const ExtParams &p, const bm2_seed &s, const PfBox &q, int l_query) {
+    if (q.qb == -1 && q.qe == -1) return 0;
+    if (s.rbeg < q.rb || s.rbeg + s.len > q.re || s.qbeg < q.qb || s.qbeg + s.len > q.qe) return 1;
+    if (s.len - q.seedlen0 > .1 * l_query) return 1;
+    int64_t rd; int qd, w, max_gap;
+    qd = s.qbeg - q.qb; rd = s.rbeg - q.rb;
+    max_gap = cal_max_gap_d(p, qd < rd ? qd : (int) rd);
+    w = max_gap < q.w ? max_gap : q.w;
+    if (qd - rd < w && rd - qd < w) return 2;
+    qd = q.qe - (s.qbeg + s.len); rd = q.re - (s.rbeg + s.len);
+    max_gap = cal_max_gap_d(p, qd < rd ? qd : (int) rd);
+    w = max_gap < q.w ? max_gap : q.w;
+    if (qd - rd < w && rd - qd < w) return 2;
+    return 1;
+}
+
+// The second half of the decision (src/bwamem.cpp:2978-2986), for a seed that lies inside an earlier reg: it is kept only when a
+// long seed of the same chain visited before it (srt2[k+1..n), purged ones -1) overlaps it on another diagonal.
+BM2_HD bool pf_chain_overlap_d(const bm2_seed *cs, int n, const int32_t *srt2, int k, const bm2_seed &s) {
+    for (int vv = k + 1; vv < n; ++vv) {
+        if (srt2[vv] < 0) continue;
+        const bm2_seed &t = cs[srt2[vv]];
+        if (t.len < s.len * .95) continue;
+        if (s.qbeg <= t.qbeg && s.qbeg + s.len - t.qbeg >= s.len >> 2 && t.qbeg - s.qbeg != t.rbeg - s.rbeg) return true;
+        if (t.qbeg <= s.qbeg && t.qbeg + t.len - s.qbeg >= s.len >> 2 && s.qbeg - t.qbeg != s.rbeg - t.rbeg) return true;
+    }
+    return false;
+}
+
+// Post-filter decision of seed srt2[k] of chain cs[0..n) (src/bwamem.cpp:2957-2986): true = purged.  box[0..): the boxes of the read's
+// regs in creation order, purged ones with qb = qe = -1; lim: the number of regs kept so far.  The scan stops after lim counted boxes,
+// so it reads only the boxes of regs created before this seed's own.
+BM2_HD bool pf_seed_purged_d(const ExtParams &p, const bm2_seed *cs, int n, const int32_t *srt2, int k, int l_query, const PfBox *box,
+                             int n_reg, int lim)
+{
+    const bm2_seed s = cs[srt2[k]];
+    int v = 0;
+    for (int i = 0; i < n_reg && v < lim; ++i) {
+        const int kind = pf_box_kind_d(p, s, box[i], l_query);
+        if (kind == 2) break;
+        v += kind;
+    }
+    return v < lim && !pf_chain_overlap_d(cs, n, srt2, k, s);
+}
+
 // Post-filter of one read (src/bwamem.cpp:2895-2989).  regs[0..n_reg) in creation order;
 // reg_seed[i] = seed index (within its chain) of reg i; srt2: int scratch of >= max chain length;
 // box: scratch of n_reg entries.
 BM2_HD void ext_postfilter_read_d(const ExtParams &p, const bm2_chain *chains, int n_chain, const bm2_seed *seeds, int l_query,
                                   bm2_alnreg_t *regs, int n_reg, const int32_t *reg_seed, int32_t *srt2, PfBox *box)
 {
-    for (int i = 0; i < n_reg; ++i) {
-        const bm2_alnreg_t &a = regs[i];
-        PfBox b; b.rb = a.rb; b.re = a.re; b.qb = a.qb; b.qe = a.qe; b.seedlen0 = a.seedlen0; b.w = a.w;
-        box[i] = b;
-    }
+    for (int i = 0; i < n_reg; ++i) box[i] = pf_box_d(regs[i]);
     int lim = 0, base = 0;
     for (int ci = 0; ci < n_chain; ++ci) {
         const bm2_chain &c = chains[ci];
@@ -176,45 +234,67 @@ BM2_HD void ext_postfilter_read_d(const ExtParams &p, const bm2_chain *chains, i
         if (n == 0) continue;
         for (int k = n - 1; k >= 0; --k) srt2[k] = reg_seed[base + (n - 1 - k)];
         for (int k = n - 1; k >= 0; --k) {
-            const bm2_seed s = cs[srt2[k]];
-            int i, v = 0;
-            for (i = 0; i < n_reg && v < lim; ++i) {
-                const PfBox q = box[i];
-                if (q.qb == -1 && q.qe == -1) continue;
-                int64_t rd; int qd, w, max_gap;
-                if (s.rbeg < q.rb || s.rbeg + s.len > q.re || s.qbeg < q.qb || s.qbeg + s.len > q.qe) { v++; continue; }
-                if (s.len - q.seedlen0 > .1 * l_query) { v++; continue; }
-                qd = s.qbeg - q.qb; rd = s.rbeg - q.rb;
-                max_gap = cal_max_gap_d(p, qd < rd ? qd : (int) rd);
-                w = max_gap < q.w ? max_gap : q.w;
-                if (qd - rd < w && rd - qd < w) break;
-                qd = q.qe - (s.qbeg + s.len); rd = q.re - (s.rbeg + s.len);
-                max_gap = cal_max_gap_d(p, qd < rd ? qd : (int) rd);
-                w = max_gap < q.w ? max_gap : q.w;
-                if (qd - rd < w && rd - qd < w) break;
-                v++;
-            }
-            if (v < lim) {
-                int vv;
-                for (vv = k + 1; vv < n; ++vv) {
-                    if (srt2[vv] < 0) continue;
-                    const bm2_seed &t = cs[srt2[vv]];
-                    if (t.len < s.len * .95) continue;
-                    if (s.qbeg <= t.qbeg && s.qbeg + s.len - t.qbeg >= s.len >> 2 && t.qbeg - s.qbeg != t.rbeg - s.rbeg) break;
-                    if (t.qbeg <= s.qbeg && t.qbeg + t.len - s.qbeg >= s.len >> 2 && s.qbeg - t.qbeg != s.rbeg - t.rbeg) break;
-                }
-                if (vv == n) {
-                    const int ai = base + (n - 1 - k);
-                    regs[ai].qb = regs[ai].qe = -1;
-                    box[ai].qb = box[ai].qe = -1;
-                    srt2[k] = -1;
-                    continue;
-                }
+            if (pf_seed_purged_d(p, cs, n, srt2, k, l_query, box, n_reg, lim)) {
+                const int ai = base + (n - 1 - k);
+                regs[ai].qb = regs[ai].qe = -1;
+                box[ai].qb = box[ai].qe = -1;
+                srt2[k] = -1;
+                continue;
             }
             lim++;
         }
         base += n;
     }
+}
+
+// ---- lazy extension: extend only the seeds the post-filter keeps ----------------------------------------------------------------
+// Whether the post-filter purges a seed depends on the seeds and on the boxes of the EARLIER KEPT regs only (pf_seed_purged_d), so
+// a walk in the post-filter's order can decide every seed up to the first kept one whose reg has not been extended yet, and the
+// purged seeds before it need no extension at all.  The post-filter of the tail stays the decision that counts: it purges the
+// same seeds again, and every reg it keeps has been extended.
+
+// Where the walk of one read stands: chain ci, seed k of its post-filter order (-1: the chain's srt2 is not set up yet), the number
+// of kept regs before it, and the reg index of the chain's first reg.  ci == n_chain: the read is decided.
+struct PfCursor { int32_t ci, k, lim, base; };
+
+// Resumes the post-filter walk of one read at `cur` (start: {0, -1, 0, 0}).  Purged seeds are marked in srt2 (and, when not extended,
+// EXT_SKIP); the box of every decided reg is written for the later decisions.  Stops at the first kept seed whose reg is not extended,
+// marks it EXT_NEED and returns false; returns true when every seed of the read is decided.  regs / state / srt2 / box: the read's
+// stripes; srt2 and box must be kept between calls.
+BM2_HD bool ext_walk_read_d(const ExtParams &p, const bm2_chain *chains, int n_chain, const bm2_seed *seeds, int l_query,
+                            const bm2_alnreg_t *regs, int n_reg, const int32_t *reg_seed, uint8_t *state, int32_t *srt2, PfBox *box,
+                            PfCursor &cur)
+{
+    int ci = cur.ci, k = cur.k, lim = cur.lim, base = cur.base;
+    for (; ci < n_chain; ++ci, k = -1) {
+        const bm2_chain &c = chains[ci];
+        const bm2_seed *cs = seeds + c.seed_off;
+        const int n = c.n_seeds;
+        if (n == 0) continue;
+        if (k < 0) {
+            for (int kk = n - 1; kk >= 0; --kk) srt2[kk] = reg_seed[base + (n - 1 - kk)];
+            k = n - 1;
+        }
+        for (; k >= 0; --k) {
+            const int ai = base + (n - 1 - k);
+            if (pf_seed_purged_d(p, cs, n, srt2, k, l_query, box, n_reg, lim)) {
+                box[ai].qb = box[ai].qe = -1;
+                srt2[k] = -1;
+                if (state[ai] != EXT_DONE) state[ai] = EXT_SKIP;
+                continue;
+            }
+            if (state[ai] != EXT_DONE) {
+                state[ai] = EXT_NEED;
+                cur.ci = ci; cur.k = k; cur.lim = lim; cur.base = base;
+                return false;
+            }
+            box[ai] = pf_box_d(regs[ai]);
+            lim++;
+        }
+        base += n;
+    }
+    cur.ci = ci; cur.k = -1; cur.lim = lim; cur.base = base;
+    return true;
 }
 
 // score-only ksw_global2 (src/ksw.cpp:558-668) of query[0..qlen) vs target[0..tlen); sequences are

@@ -14,6 +14,7 @@
 //   F  ext_build_kernel    one read per thread: regs + left/right extension jobs
 //   G  BSW left  (bsw.cu) + fold + doubled-band retry
 //   H  BSW right (bsw.cu) + fold + doubled-band retry
+//      (G and H run in waves, with a post-filter walk in between that proves seeds purged before they are extended: lazy extension)
 //   I  tail_kernel         one read per thread: post-filter, dedup/patch, ALT marking
 //   J  gather of the final regs, D2H
 #include "bm2_common.cuh"
@@ -103,7 +104,7 @@ void bm2_free_index(bm2_ctx *ctx) {
 struct Counters {                 // device-side counters of one batch
     unsigned long long n_smem, n_ext, n_lf, n_retry, cells;
     unsigned long long n_pool, n_task, n_task1, n_rtask;     // SMEM stage: interval-list pool, search tasks, re-seed tasks
-    unsigned long long pad[3];
+    unsigned long long n_sel[2], n_walk_done;                // lazy extension: left / right jobs of the wave, reads decided by the first walk
 };
 
 struct SearchTask { int32_t read, x, min_intv, n; int64_t off; };     // one backward phase: list pool[off .. off+n)
@@ -432,6 +433,7 @@ __global__ void chain_compact_kernel(const int64_t *__restrict__ read_smem_off, 
 struct ExtBufs {
     bm2_alnreg_t *regs; int32_t *reg_chain, *reg_seed; uint64_t *srt;
     ExtJobRec *left, *right; int32_t *left_reg, *right_reg;
+    uint8_t *state;                  // per-reg extension state of the lazy extension (null: every job runs)
 };
 
 __global__ void __launch_bounds__(128)
@@ -447,7 +449,7 @@ ext_build_kernel(ContigView cv, ExtParams ep, const bm2_chain *__restrict__ chai
     const int64_t g0 = reg_off[r];
     ext_build_read_d(cv, ep, chains + c0, (int) (c1 - c0), seeds, (int) (offs[r + 1] - offs[r]), offs[r], c0, g0, b.regs + g0,
                      b.reg_chain + g0, b.reg_seed + g0, b.left + left_off[r], b.left_reg + left_off[r], b.right + right_off[r],
-                     b.right_reg + right_off[r], b.srt + g0);
+                     b.right_reg + right_off[r], b.srt + g0, b.state ? b.state + g0 : nullptr);
 }
 
 // G/H. fold one finished job into its reg; rejected jobs are appended to the retry list
@@ -479,6 +481,60 @@ __global__ void gather_jobs_kernel(const ExtJobRec *jobs, const int32_t *sel, in
     if (t < n) out[t] = jobs[sel[t]];
 }
 
+// ---- lazy extension (ext_walk_read_d, ext_device.cuh): the extension runs in waves ------------------------------------------------
+// The jobs of one wave: those whose reg is EXT_NEED or, in the last wave, any reg not extended yet (EXT_TODO), appended with their reg
+// ids to a compact list, one atomic per warp.  The order of the list does not matter: the extension kernels sort their jobs by size.
+__global__ void ext_select_kernel(const ExtJobRec *__restrict__ jobs, const int32_t *__restrict__ job_reg, int n,
+                                  const uint8_t *__restrict__ state, int last, ExtJobRec *out, int32_t *out_reg, unsigned long long *n_out)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x, lane = threadIdx.x & 31;
+    int g = 0;
+    bool take = false;
+    if (i < n) { g = job_reg[i]; const uint8_t s = state[g]; take = s == EXT_NEED || (last && s == EXT_TODO); }
+    const unsigned m = __ballot_sync(0xffffffffu, take);
+    if (!m) return;
+    const int leader = __ffs(m) - 1;
+    unsigned long long at = 0;
+    if (lane == leader) at = atomicAdd(n_out, (unsigned long long) __popc(m));
+    at = __shfl_sync(0xffffffffu, at, leader);
+    if (take) { const unsigned long long k = at + __popc(m & ((1u << lane) - 1u)); out[k] = jobs[i]; out_reg[k] = g; }
+}
+
+// after a wave: its regs are extended
+__global__ void ext_mark_done_kernel(uint8_t *state, int64_t n) {
+    const int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n && state[i] == EXT_NEED) state[i] = EXT_DONE;
+}
+
+// The post-filter walk, one read per thread, resumed from cur[r] (first: from the start).  Reads with more than `heavy` regs are not
+// walked (their O(regs^2) walk on one thread would hold up the grid): every job of theirs runs, in the last wave.
+__global__ void __launch_bounds__(128)
+ext_walk_kernel(ExtParams ep, const bm2_chain *__restrict__ chains, const bm2_seed *__restrict__ seeds, const int64_t *__restrict__ chain_off,
+                const int64_t *__restrict__ reg_off, const int64_t *__restrict__ offs, int n_reads, const bm2_alnreg_t *regs,
+                const int32_t *__restrict__ reg_seed, uint8_t *state, int32_t *srt2_all, PfBox *box_all, PfCursor *cur, int first, int heavy,
+                Counters *cnt)
+{
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    bool done = false;
+    if (r < n_reads) {
+        const int64_t c0 = chain_off[r], c1 = chain_off[r + 1], g0 = reg_off[r];
+        const int n_reg = (int) (reg_off[r + 1] - g0), n_chain = (int) (c1 - c0);
+        if (n_chain > 0 && n_reg <= heavy) {
+            PfCursor c;
+            if (first) { c.ci = 0; c.k = -1; c.lim = 0; c.base = 0; } else c = cur[r];
+            if (c.ci < n_chain) {
+                done = ext_walk_read_d(ep, chains + c0, n_chain, seeds, (int) (offs[r + 1] - offs[r]), regs + g0, n_reg, reg_seed + g0,
+                                       state + g0, srt2_all + g0, box_all + g0, c);
+                cur[r] = c;
+            }
+        }
+    }
+    if (first) {
+        const unsigned m = __ballot_sync(0xffffffffu, done);
+        if ((threadIdx.x & 31) == 0 && m) atomicAdd(&cnt->n_walk_done, (unsigned long long) __popc(m));
+    }
+}
+
 // Post-filter of one read by a whole warp (same result as ext_postfilter_read_d, src/bwamem.cpp:2895-2989): the scan of
 // the earlier alignments - O(regs) per seed, O(regs^2) per read - is split over the lanes, 32 boxes per step.  Each lane
 // classifies its box as skipped / counted (v++) / hit (break); the sequential loop `for (i = 0; i < n_reg && v < lim; ++i)`
@@ -487,11 +543,7 @@ __device__ void ext_postfilter_read_warp(const ExtParams &p, const bm2_chain *ch
                                          bm2_alnreg_t *regs, int n_reg, const int32_t *reg_seed, int32_t *srt2, PfBox *box)
 {
     const int lane = threadIdx.x & 31;
-    for (int i = lane; i < n_reg; i += 32) {
-        const bm2_alnreg_t &a = regs[i];
-        PfBox b; b.rb = a.rb; b.re = a.re; b.qb = a.qb; b.qe = a.qe; b.seedlen0 = a.seedlen0; b.w = a.w;
-        box[i] = b;
-    }
+    for (int i = lane; i < n_reg; i += 32) box[i] = pf_box_d(regs[i]);
     __syncwarp();
     int lim = 0, base = 0;
     for (int ci = 0; ci < n_chain; ++ci) {
@@ -514,28 +566,7 @@ __device__ void ext_postfilter_read_warp(const ExtParams &p, const bm2_chain *ch
 #pragma unroll
                 for (int g = 0; g < 4; ++g) {
                     const int i = i0 + 32 * g + lane;
-                    int kd = 0;                                 // 0 skipped, 1 counted, 2 hit
-                    if (i < n_reg) {
-                        const PfBox q = box[i];
-                        if (!(q.qb == -1 && q.qe == -1)) {
-                            kd = 1;
-                            if (!(s.rbeg < q.rb || s.rbeg + s.len > q.re || s.qbeg < q.qb || s.qbeg + s.len > q.qe) &&
-                                !(s.len - q.seedlen0 > .1 * l_query)) {
-                                int64_t rd; int qd, w, max_gap;
-                                qd = s.qbeg - q.qb; rd = s.rbeg - q.rb;
-                                max_gap = cal_max_gap_d(p, qd < rd ? qd : (int) rd);
-                                w = max_gap < q.w ? max_gap : q.w;
-                                if (qd - rd < w && rd - qd < w) kd = 2;
-                                else {
-                                    qd = q.qe - (s.qbeg + s.len); rd = q.re - (s.rbeg + s.len);
-                                    max_gap = cal_max_gap_d(p, qd < rd ? qd : (int) rd);
-                                    w = max_gap < q.w ? max_gap : q.w;
-                                    if (qd - rd < w && rd - qd < w) kd = 2;
-                                }
-                            }
-                        }
-                    }
-                    kind[g] = kd;
+                    kind[g] = i < n_reg ? pf_box_kind_d(p, s, box[i], l_query) : 0;      // 0 skipped, 1 counted, 2 hit
                 }
 #pragma unroll
                 for (int g = 0; g < 4; ++g) {
@@ -549,15 +580,7 @@ __device__ void ext_postfilter_read_warp(const ExtParams &p, const bm2_chain *ch
                 }
             }
             if (v < lim) {
-                int vv;
-                for (vv = k + 1; vv < n; ++vv) {
-                    if (srt2[vv] < 0) continue;
-                    const bm2_seed &t = cs[srt2[vv]];
-                    if (t.len < s.len * .95) continue;
-                    if (s.qbeg <= t.qbeg && s.qbeg + s.len - t.qbeg >= s.len >> 2 && t.qbeg - s.qbeg != t.rbeg - s.rbeg) break;
-                    if (t.qbeg <= s.qbeg && t.qbeg + t.len - s.qbeg >= s.len >> 2 && s.qbeg - t.qbeg != s.rbeg - t.rbeg) break;
-                }
-                if (vv == n) {
+                if (!pf_chain_overlap_d(cs, n, srt2, k, s)) {
                     __syncwarp();
                     if (lane == 0) {
                         const int ai = base + (n - 1 - k);
@@ -1100,10 +1123,18 @@ int run_pipeline(bm2_ctx *ctx, const bm2_read_batch *rb, UpTo upto, BatchState &
     // ---- F. regs + jobs -----------------------------------------------------------------------------------
     if (sg.mark("extbuild")) return 1;
     const size_t nr1 = (size_t) n_regs + 1, nl1 = (size_t) n_left + 1, nrt1 = (size_t) n_right + 1;
-    const size_t aux_bytes = al(nr1 * 4) * 3 + al(nr1 * 8) + al(nl1 * 4) * 2 + al(nrt1 * 4) * 2 + al(nr1 * sizeof(PfBox));
+    // Lazy extension (BM2_EXT_LAZY, default on): the jobs run in BM2_EXT_WAVES waves (default 2).  Wave 1 extends the first seed of every
+    // chain; a post-filter walk (ext_walk_kernel) then decides the seeds after it, up to the first kept seed not extended yet; further
+    // speculative waves extend the seeds the walks stopped at; the last wave extends every reg that is neither extended nor proved purged.
+    // The seeds proved purged are never extended.  BM2_EXT_LAZY=0: every job in one wave.
+    const int lazy = env_int("BM2_EXT_LAZY", 1, 0, 1);
+    const int waves = env_int("BM2_EXT_WAVES", 2, 2, 64);
+    const size_t aux_bytes = al(nr1 * 4) * 3 + al(nr1 * 8) + al(nl1 * 4) * 2 + al(nrt1 * 4) * 2 + al(nr1 * sizeof(PfBox)) +
+                             (lazy ? al(nr1) + al((size_t) n * sizeof(PfCursor)) + al(nl1 * 4) + al(nrt1 * 4) : 0);
     const size_t njmax = nl1 > nrt1 ? nl1 : nrt1;
     if (ctx->ensure(ctx->d[B_REGS], nr1 * sizeof(bm2_alnreg_t)) || ctx->ensure(ctx->d[B_REG_AUX], aux_bytes) ||
-        ctx->ensure(ctx->d[B_JOBS], al(nl1 * sizeof(ExtJobRec)) + al(nrt1 * sizeof(ExtJobRec)) + al(njmax * sizeof(ExtJobRec)) + al(njmax * sizeof(BswOut))) ||
+        ctx->ensure(ctx->d[B_JOBS], al(nl1 * sizeof(ExtJobRec)) + al(nrt1 * sizeof(ExtJobRec)) + al(njmax * sizeof(ExtJobRec)) + al(njmax * sizeof(BswOut)) +
+                                    (lazy ? al(nl1 * sizeof(ExtJobRec)) + al(nrt1 * sizeof(ExtJobRec)) : 0)) ||
         ctx->ensure(ctx->bsw_scratch, bsw_scratch_bytes((int) njmax))) return 1;
     char *ab = (char *) ctx->d[B_REG_AUX].p;
     int32_t *d_reg_chain = (int32_t *) ab; ab += al(nr1 * 4);
@@ -1115,13 +1146,22 @@ int run_pipeline(bm2_ctx *ctx, const bm2_read_batch *rb, UpTo upto, BatchState &
     int32_t *d_right_reg = (int32_t *) ab; ab += al(nrt1 * 4);
     int32_t *d_right_retry = (int32_t *) ab; ab += al(nrt1 * 4);
     PfBox *d_box = (PfBox *) ab; ab += al(nr1 * sizeof(PfBox));
+    uint8_t *d_state = nullptr; PfCursor *d_cursor = nullptr; int32_t *d_wleft_reg = nullptr, *d_wright_reg = nullptr;
+    if (lazy) {
+        d_state = (uint8_t *) ab; ab += al(nr1);
+        d_cursor = (PfCursor *) ab; ab += al((size_t) n * sizeof(PfCursor));
+        d_wleft_reg = (int32_t *) ab; ab += al(nl1 * 4);
+        d_wright_reg = (int32_t *) ab; ab += al(nrt1 * 4);
+    }
     char *jb = (char *) ctx->d[B_JOBS].p;
     ExtJobRec *d_left = (ExtJobRec *) jb; jb += al(nl1 * sizeof(ExtJobRec));
     ExtJobRec *d_right = (ExtJobRec *) jb; jb += al(nrt1 * sizeof(ExtJobRec));
     ExtJobRec *d_retry_jobs = (ExtJobRec *) jb; jb += al(njmax * sizeof(ExtJobRec));
-    BswOut *d_outs = (BswOut *) jb;
+    BswOut *d_outs = (BswOut *) jb; jb += al(njmax * sizeof(BswOut));
+    ExtJobRec *d_wleft = nullptr, *d_wright = nullptr;          // the jobs of one wave
+    if (lazy) { d_wleft = (ExtJobRec *) jb; jb += al(nl1 * sizeof(ExtJobRec)); d_wright = (ExtJobRec *) jb; }
     bm2_alnreg_t *d_regs = P<bm2_alnreg_t>(ctx, B_REGS);
-    ExtBufs eb = { d_regs, d_reg_chain, d_reg_seed, d_srt, d_left, d_right, d_left_reg, d_right_reg };
+    ExtBufs eb = { d_regs, d_reg_chain, d_reg_seed, d_srt, d_left, d_right, d_left_reg, d_right_reg, d_state };
     work_keys_off_kernel<<<(n + 255) / 256, 256, 0, st>>>(d_reg_off, n, wk_in, wv_in);       // work ~ regs of the read
     if (sort_work(ctx, wk_in, wk_out, wv_in, d_perm, n)) return 1;
     ext_build_kernel<<<(n + 127) / 128, 128, 0, st>>>(pv.cv, pv.ep, P<bm2_chain>(ctx, B_CHAINS), P<bm2_seed>(ctx, B_SEEDS), d_chain_off, d_reg_off,
@@ -1153,11 +1193,41 @@ int run_pipeline(bm2_ctx *ctx, const bm2_read_batch *rb, UpTo upto, BatchState &
                                                                             d_reg_chain, P<bm2_chain>(ctx, B_CHAINS), P<bm2_seed>(ctx, B_SEEDS), d_offs,
                                                                             retry, d_cnt);
         }
-        ctx->last_n_retry[is_right] = n_retry;
+        ctx->last_n_retry[is_right] += n_retry;
         return 0;
     };
-    if (phase("bsw_left", d_left, d_left_reg, d_left_retry, n_left, 0)) return 1;
-    if (phase("bsw_right", d_right, d_right_reg, d_right_retry, n_right, 1)) return 1;
+    ctx->last_n_retry[0] = ctx->last_n_retry[1] = 0;
+    ctx->last_jobs_skipped = 0;
+    if (!lazy) {
+        if (phase("bsw_left", d_left, d_left_reg, d_left_retry, n_left, 0)) return 1;
+        if (phase("bsw_right", d_right, d_right_reg, d_right_retry, n_right, 1)) return 1;
+    } else {
+        int64_t jobs_run = 0;
+        const int walk_heavy = env_int("BM2_EXT_WALK_HEAVY", 256, 0, 1 << 30);     // regs from which a read is not walked
+        for (int wave = 1; wave <= waves; ++wave) {
+            const int last = wave == waves;
+            if (sg.mark("ext_select")) return 1;
+            BM2_CUDA_OK(cudaMemsetAsync(d_cnt->n_sel, 0, sizeof(d_cnt->n_sel), st));
+            if (n_left > 0)
+                ext_select_kernel<<<(unsigned) ((n_left + 255) / 256), 256, 0, st>>>(d_left, d_left_reg, (int) n_left, d_state, last, d_wleft,
+                                                                                     d_wleft_reg, &d_cnt->n_sel[0]);
+            if (n_right > 0)
+                ext_select_kernel<<<(unsigned) ((n_right + 255) / 256), 256, 0, st>>>(d_right, d_right_reg, (int) n_right, d_state, last, d_wright,
+                                                                                      d_wright_reg, &d_cnt->n_sel[1]);
+            unsigned long long n_sel[2] = {0, 0};
+            BM2_CUDA_OK(cudaMemcpyAsync(n_sel, d_cnt->n_sel, sizeof(n_sel), cudaMemcpyDeviceToHost, st));
+            BM2_CUDA_OK(cudaStreamSynchronize(st));
+            if (phase("bsw_left", d_wleft, d_wleft_reg, d_left_retry, (int64_t) n_sel[0], 0)) return 1;
+            if (phase("bsw_right", d_wright, d_wright_reg, d_right_retry, (int64_t) n_sel[1], 1)) return 1;
+            jobs_run += (int64_t) (n_sel[0] + n_sel[1]);
+            if (last) break;
+            if (sg.mark("ext_walk")) return 1;
+            ext_mark_done_kernel<<<(unsigned) ((n_regs + 255) / 256), 256, 0, st>>>(d_state, n_regs);
+            ext_walk_kernel<<<(n + 127) / 128, 128, 0, st>>>(pv.ep, P<bm2_chain>(ctx, B_CHAINS), P<bm2_seed>(ctx, B_SEEDS), d_chain_off, d_reg_off, d_offs, n,
+                                                             d_regs, d_reg_seed, d_state, d_srt2, d_box, d_cursor, wave == 1, walk_heavy, d_cnt);
+        }
+        ctx->last_jobs_skipped = (unsigned long long) (n_left + n_right - jobs_run);
+    }
 
     // ---- I. post-filter + tail ----------------------------------------------------------------------------
     if (sg.mark("tail")) return 1;
@@ -1195,6 +1265,7 @@ int run_pipeline(bm2_ctx *ctx, const bm2_read_batch *rb, UpTo upto, BatchState &
     BM2_CUDA_OK(cudaMemcpyAsync(&h_cnt, d_cnt, sizeof(Counters), cudaMemcpyDeviceToHost, st));
     BM2_CUDA_OK(cudaStreamSynchronize(st));
     ctx->last_cells = h_cnt.cells;
+    ctx->last_walk_done = h_cnt.n_walk_done;
     const int64_t n_out = ((const int64_t *) ctx->h[H_OUT_OFF].p)[n];
     bs.n_out = n_out;
     if (copy_out && ctx->ensure_host(ctx->h[H_OUT_REGS], (size_t) (n_out + 1) * sizeof(bm2_alnreg_t))) return 1;
@@ -1212,12 +1283,17 @@ int finish_stage_times(bm2_ctx *ctx) {
     // the names vector may be longer than this run's marks when an earlier run went further
     size_t marks = 0;
     for (; marks < n; ++marks) if (strcmp(ctx->stage_names[marks], "end") == 0) { ++marks; break; }
-    for (size_t i = 0; i + 1 < marks; ++i) {
-        float ms = 0; BM2_CUDA_OK(cudaEventElapsedTime(&ms, ctx->events[i], ctx->events[i + 1]));
-        ctx->stage_ms.push_back(ms);
+    // a stage marked more than once (the extension stages, once per wave of the lazy extension) is reported once, its times summed
+    std::vector<const char *> names;
+    for (size_t i = 0; i < marks; ++i) {
+        float ms = 0;
+        if (i + 1 < marks) BM2_CUDA_OK(cudaEventElapsedTime(&ms, ctx->events[i], ctx->events[i + 1]));
+        size_t j = 0;
+        while (j < names.size() && strcmp(names[j], ctx->stage_names[i]) != 0) ++j;
+        if (j == names.size()) { names.push_back(ctx->stage_names[i]); ctx->stage_ms.push_back(0.f); }
+        ctx->stage_ms[j] += ms;
     }
-    ctx->stage_ms.push_back(0.f);
-    ctx->stage_names.resize(marks);
+    ctx->stage_names = names;
     return 0;
 }
 
@@ -1356,11 +1432,13 @@ static int run_regs(bm2_ctx *ctx, const bm2_read_batch *rb, const uint8_t *d_cod
     ctx->stage_names = ctx->lanes[0]->stage_names;
     ctx->stage_ms.assign(ctx->lanes[0]->stage_ms.size(), 0.f);
     ctx->last_n_ext = ctx->last_n_lf = ctx->last_cells = 0; ctx->last_n_retry[0] = ctx->last_n_retry[1] = 0;
+    ctx->last_jobs_skipped = ctx->last_walk_done = 0;
     for (int k = 0; k < K; ++k) {
         const bm2_ctx *l = ctx->lanes[k];
         for (size_t i = 0; i < ctx->stage_ms.size() && i < l->stage_ms.size(); ++i) ctx->stage_ms[i] += l->stage_ms[i];
         ctx->last_n_ext += l->last_n_ext; ctx->last_n_lf += l->last_n_lf; ctx->last_cells += l->last_cells;
         ctx->last_n_retry[0] += l->last_n_retry[0]; ctx->last_n_retry[1] += l->last_n_retry[1];
+        ctx->last_jobs_skipped += l->last_jobs_skipped; ctx->last_walk_done += l->last_walk_done;
     }
     out->n = n_out; out->regs = copy_out ? regs : nullptr; out->read_off = off;
     return 0;
@@ -1387,5 +1465,6 @@ extern "C" int bm2_last_stage_ms(const bm2_ctx *ctx, const char *const **names, 
 extern "C" int bm2_last_counters(const bm2_ctx *ctx, unsigned long long *v, int n) {
     if (!ctx || n < 5) return 1;
     v[0] = ctx->last_n_ext; v[1] = ctx->last_n_lf; v[2] = ctx->last_cells; v[3] = ctx->last_n_retry[0]; v[4] = ctx->last_n_retry[1];
+    if (n >= 7) { v[5] = ctx->last_jobs_skipped; v[6] = ctx->last_walk_done; }
     return 0;
 }

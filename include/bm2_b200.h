@@ -228,7 +228,9 @@ int bm2_seed_chain_extend_resident(bm2_ctx *ctx, const bm2_read_batch *reads, co
 int bm2_last_stage_ms(const bm2_ctx *ctx, const char *const **names, const float **ms, int *n);
 /* Work counters of the last seam-2 call: v[0] interval extensions (128 algorithmic bytes each),
  * v[1] LF steps of the SA walk (64 B each), v[2] banded DP cells, v[3]/v[4] left/right jobs re-run
- * with the doubled band.  n >= 5. */
+ * with the doubled band.  n >= 5.  With n >= 7 also v[5] extension jobs not run (their seeds proved
+ * purged by the post-filter before extension) and v[6] reads whose seeds were all decided after the
+ * first extension wave (both 0 with BM2_EXT_LAZY=0). */
 int bm2_last_counters(const bm2_ctx *ctx, unsigned long long *v, int n);
 
 /* ---------------------------------------------------------------------------------------------
