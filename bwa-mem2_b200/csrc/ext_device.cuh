@@ -190,6 +190,20 @@ BM2_HD int pf_box_kind_d(const ExtParams &p, const bm2_seed &s, const PfBox &q, 
     return 1;
 }
 
+// One step of 32 boxes of the scan in pf_seed_purged_d, resolved from the step's counted (kind 1) and hit (kind 2) masks, bit j = box j of
+// the step: advances v exactly as the sequential loop `for (i = 0; i < n_reg && v < lim; ++i)` does over those boxes and returns true
+// when that loop ends inside the step (a hit while v < lim, or v reaching lim).  Needs v < lim on entry.  The warp scans resolve their
+// ballots with it.
+BM2_HD bool pf_scan_step_d(uint32_t counted, uint32_t hit, int &v, int lim) {
+    if (hit) {
+        const int at = v + BM2_POPC32(counted & ((hit & (0u - hit)) - 1u));    // counted boxes before the first hit
+        if (at < lim) { v = at; return true; }
+    }
+    v += BM2_POPC32(counted);
+    if (v >= lim) { v = lim; return true; }
+    return false;
+}
+
 // The second half of the decision (src/bwamem.cpp:2978-2986), for a seed that lies inside an earlier reg: it is kept only when a
 // long seed of the same chain visited before it (srt2[k+1..n), purged ones -1) overlaps it on another diagonal.
 BM2_HD bool pf_chain_overlap_d(const bm2_seed *cs, int n, const int32_t *srt2, int k, const bm2_seed &s) {

@@ -12,8 +12,10 @@
 #endif
 
 #if defined(__CUDA_ARCH__)
+#define BM2_POPC32(x) __popc(x)
 #define BM2_POPC64(x) __popcll(x)
 #else
+#define BM2_POPC32(x) __builtin_popcount(x)
 #define BM2_POPC64(x) __builtin_popcountll(x)
 #endif
 
