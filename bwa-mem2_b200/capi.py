@@ -78,9 +78,25 @@ class FastqBatch(C.Structure):
                 ("quals", C.c_void_p), ("name_beg", C.c_void_p), ("name_len", C.c_void_p)]
 
 
-def sam_format(recs, xa, cigar, md, codes, offsets, contig_names, read_names=None, quals=None, n_threads=1, name_spans=None) -> bytes:
+class FastqSplit(C.Structure):
+    _fields_ = [("set", FastqBatch * 2), ("comment_beg", C.c_void_p * 2), ("comment_len", C.c_void_p * 2), ("read_index", C.c_void_p * 2)]
+
+
+class SamTextExtra(C.Structure):
+    _fields_ = [("rg_id", C.c_char_p), ("comment_beg", C.c_void_p), ("comment_len", C.c_void_p), ("contig_anno", C.c_void_p), ("ref_hdr", C.c_int32)]
+
+
+def _host(p, n, dt):
+    dt = np.dtype(dt)
+    return np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_uint8)), shape=(max(n, 1) * dt.itemsize,))[:n * dt.itemsize].view(dt).copy()
+
+
+def sam_format(recs, xa, cigar, md, codes, offsets, contig_names, read_names=None, quals=None, n_threads=1, name_spans=None,
+               rg_id=None, comments=None, contig_anno=None, ref_hdr=False) -> bytes:
     """bm2_sam_format: the SAM text of a batch from the records of bm2_sam_pe / bm2_sam_se (one line per record, QNAME to the last tag).
-    read_names: list of names, or name_spans = (buf1, buf2 or None, name_beg int64[], name_len int32[]) as bm2_fastq_encode returns them."""
+    read_names: list of names, or name_spans = (buf1, buf2 or None, name_beg int64[], name_len int32[]) as bm2_fastq_encode returns them.
+    With rg_id (-R), comments = (comment_beg int64[], comment_len int32[]) into the buffers of name_spans (-C) or contig_anno (list of str)
+    with ref_hdr (-V): bm2_sam_format_ex."""
     recs = np.ascontiguousarray(recs, SAM_REC_DT); xa = np.ascontiguousarray(xa, SAM_XA_DT)
     cigar = np.ascontiguousarray(cigar, np.uint32); md = np.ascontiguousarray(md, np.uint8)
     codes = np.ascontiguousarray(codes, np.uint8); offsets = np.ascontiguousarray(offsets, np.int64)
@@ -97,9 +113,21 @@ def sam_format(recs, xa, cigar, md, codes, offsets, contig_names, read_names=Non
         tin.name_buf[0] = b1; tin.name_buf[1] = b2
         tin.name_beg = nbeg.ctypes.data; tin.name_len = nlen.ctypes.data
     text = C.c_void_p(); n = C.c_int64()
-    f = lib().bm2_sam_format
-    f.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
-    rc = f(C.byref(tin), int(n_threads), C.byref(text), C.byref(n))
+    if rg_id is None and comments is None and contig_anno is None and not ref_hdr:
+        f = lib().bm2_sam_format
+        f.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+        rc = f(C.byref(tin), int(n_threads), C.byref(text), C.byref(n))
+    else:
+        x = SamTextExtra(rg_id.encode() if isinstance(rg_id, str) else rg_id, None, None, None, int(bool(ref_hdr)))
+        if comments is not None:
+            cb = np.ascontiguousarray(comments[0], np.int64); cl = np.ascontiguousarray(comments[1], np.int32)
+            x.comment_beg = cb.ctypes.data; x.comment_len = cl.ctypes.data
+        if contig_anno is not None:
+            ca = (C.c_char_p * len(contig_anno))(*[s.encode() if isinstance(s, str) else bytes(s) for s in contig_anno])
+            x.contig_anno = C.cast(ca, C.c_void_p)
+        f = lib().bm2_sam_format_ex
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+        rc = f(C.byref(tin), C.byref(x), int(n_threads), C.byref(text), C.byref(n))
     if rc:
         raise Bm2Error(f"bm2_sam_format failed ({rc})")
     out = C.string_at(text, n.value)
@@ -125,7 +153,7 @@ class RegResult(C.Structure):
     _fields_ = [("n", C.c_int64), ("regs", C.c_void_p), ("read_off", C.c_void_p)]
 
 
-EXPORTS = ["bm2_create_sibling", "bm2_fastq_encode", "bm2_sam_format", "bm2_free", "bm2_create_resident", "bm2_gather_probe", "bm2_set_sam_staged", "bm2_last_sam_stats", "bm2_gather64_gbs", "bm2_set_sub_batches", "bm2_seed_chain_extend_resident", "bm2_last_counters", "bm2_set_stream", "bm2_int_pipe_gops", "bm2_abi_version", "bm2_opt_init", "bm2_index_load", "bm2_index_free", "bm2_create", "bm2_destroy",
+EXPORTS = ["bm2_create_sibling", "bm2_fastq_encode", "bm2_fastq_comments", "bm2_fastq_smart_pair", "bm2_sam_format", "bm2_sam_format_ex", "bm2_free", "bm2_create_resident", "bm2_gather_probe", "bm2_set_sam_staged", "bm2_last_sam_stats", "bm2_gather64_gbs", "bm2_set_sub_batches", "bm2_seed_chain_extend_resident", "bm2_last_counters", "bm2_set_stream", "bm2_int_pipe_gops", "bm2_abi_version", "bm2_opt_init", "bm2_index_load", "bm2_index_free", "bm2_create", "bm2_destroy",
            "bm2_last_error", "bm2_extend_pairs", "bm2_extend_pairs_device", "bm2_collect_smems", "bm2_seed_chain",
            "bm2_seed_chain_extend", "bm2_last_stage_ms", "bm2_gen_cigar", "bm2_pestat", "bm2_sam_pe", "bm2_sam_se", "bm2_ksw_align2"]
 
@@ -337,6 +365,7 @@ class Context:
         f.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, C.c_char_p, C.c_int64, C.c_void_p]
         self._check(f(self._ctx, buf1, len(buf1), buf2, len(buf2) if buf2 is not None else 0, C.byref(b)), "bm2_fastq_encode")
         n = b.n_reads
+        self._fq_n = n
         offs = np.ctypeslib.as_array(C.cast(b.offsets, C.POINTER(C.c_int64)), shape=(n + 1,)).copy()
         tot = int(offs[-1])
         codes = np.ctypeslib.as_array(C.cast(b.codes, C.POINTER(C.c_uint8)), shape=(max(tot, 1),))[:tot].copy()
@@ -348,6 +377,32 @@ class Context:
         names = [bufs[r % stride][nb[r]:nb[r] + nl[r]] for r in range(n)] if want_names else None
         return dict(n_reads=n, codes=codes, offsets=offs, quals=quals, names=names, d_codes=b.d_codes, d_offsets=b.d_offsets,
                     name_spans=(buf1, buf2, nb, nl))
+
+    def fastq_comments(self):
+        """bm2_fastq_comments: (comment_beg int64[], comment_len int32[]) of the reads of the last fastq_encode, into their buffers."""
+        beg = C.c_void_p(); ln = C.c_void_p()
+        f = lib().bm2_fastq_comments
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        self._check(f(self._ctx, C.byref(beg), C.byref(ln)), "bm2_fastq_comments")
+        n = self._fq_n
+        return _host(beg, n, np.int64), _host(ln, n, np.int32)
+
+    def fastq_smart_pair(self):
+        """bm2_fastq_smart_pair: the last single-end fastq_encode batch split as bseq_classify does -> two dicts (single-end reads, pairs) with
+        n_reads, codes, offsets, quals, name_beg, name_len, comment_beg, comment_len, read_index, d_codes, d_offsets."""
+        sp = FastqSplit()
+        f = lib().bm2_fastq_smart_pair
+        f.argtypes = [C.c_void_p, C.c_void_p]
+        self._check(f(self._ctx, C.byref(sp)), "bm2_fastq_smart_pair")
+        out = []
+        for s in range(2):
+            b = sp.set[s]; n = b.n_reads
+            offs = _host(b.offsets, n + 1, np.int64); tot = int(offs[-1])
+            out.append(dict(n_reads=n, offsets=offs, codes=_host(b.codes, tot, np.uint8), quals=_host(b.quals, tot, np.uint8),
+                            name_beg=_host(b.name_beg, n, np.int64), name_len=_host(b.name_len, n, np.int32),
+                            comment_beg=_host(sp.comment_beg[s], n, np.int64), comment_len=_host(sp.comment_len[s], n, np.int32),
+                            read_index=_host(sp.read_index[s], n, np.int32), d_codes=b.d_codes, d_offsets=b.d_offsets))
+        return out
 
     def set_sam_staged(self, on: int):
         """bm2_set_sam_staged: 1 / 2 = the rescue's local alignments as a batch (one window per warp / per thread) before the per-pair kernel, 0 = inside it."""

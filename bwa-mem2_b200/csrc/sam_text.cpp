@@ -4,7 +4,7 @@
 // the arithmetic half (FLAG, POS, MAPQ, CIGAR, NM, MD, AS, XS, mate columns, XA entries) is done on the GPU by bm2_sam_pe / bm2_sam_se and
 // arrives as bm2_sam_rec / bm2_sam_xa; what is left is text - QNAME, the tab-separated columns, SEQ / QUAL trimmed by the record's hard
 // clips and reverse-complemented on the reverse strand (:1655-1680), the tag syntax NM MD MC AS XS SA pa XA in the reference's order
-// (:1683-1727).  Not written: the constant -C / -R / -V additions (no arithmetic; the caller appends them).
+// (:1683-1727), and with bm2_sam_format_ex the -R / -C / -V additions (RG, the FASTQ comment, XR: :1693, :1720-1728).
 // The reference formats inside worker_sam on all host threads (about 125 k reads/s per thread); this formatter is the same kind of code,
 // one pass per record with no allocation per line, so that the host keeps up with the GPU stages in front of it.
 #include "bm2_b200.h"
@@ -48,6 +48,7 @@ inline bool is_secondary(const bm2_sam_rec &r) { return (r.flag & 0x100) && r.su
 
 struct Job {
     const bm2_sam_text_in *in;
+    const bm2_sam_text_extra *x;           // may be NULL
     const int64_t *first_rec_of_read;      // n_reads + 1
     const int64_t *first_xa_of_read;       // n_reads + 1
     int64_t r0, r1;                        // read range
@@ -118,6 +119,7 @@ void format_read_range(Job &j) {
             if (r.n_mc > 0) { o.str("\tMC:Z:"); o.ops(ops + r.n_cigar, r.n_mc, "MIDSH"); }
             if (r.score >= 0) { o.str("\tAS:i:"); o.num(r.score); }
             if (r.sub >= 0) { o.str("\tXS:i:"); o.num(r.sub); }
+            if (j.x && j.x->rg_id && j.x->rg_id[0]) { o.str("\tRG:Z:"); o.str(j.x->rg_id); }
             if (!sec) {
                 bool any = false;
                 for (int64_t q = k0; q < k1; ++q) {
@@ -141,6 +143,16 @@ void format_read_range(Job &j) {
                     o.ch(','); o.num(e.nm); o.ch(';');
                 }
             }
+            if (j.x && j.x->comment_beg && j.x->comment_len && j.x->comment_len[rd] > 0 && in.name_buf[0]) {
+                const char *cb = (in.name_buf[1] && (rd & 1)) ? in.name_buf[1] : in.name_buf[0];
+                o.ch('\t'); o.bytes(cb + j.x->comment_beg[rd], (size_t) j.x->comment_len[rd]);
+            }
+            if (j.x && j.x->ref_hdr && j.x->contig_anno && r.rid >= 0 && j.x->contig_anno[r.rid] && j.x->contig_anno[r.rid][0]) {
+                o.str("\tXR:Z:");
+                const size_t at = o.n;
+                o.str(j.x->contig_anno[r.rid]);
+                for (size_t i = at; i < o.n; ++i) if (o.p[i] == '\t') o.p[i] = ' ';
+            }
             o.ch('\n');
         }
     }
@@ -148,7 +160,7 @@ void format_read_range(Job &j) {
 
 }  // namespace
 
-extern "C" int bm2_sam_format(const bm2_sam_text_in *in, int n_threads, char **text, int64_t *len) {
+extern "C" int bm2_sam_format_ex(const bm2_sam_text_in *in, const bm2_sam_text_extra *x, int n_threads, char **text, int64_t *len) {
     if (!in || !in->res || !in->reads || !in->contig_names || !text || !len) return 1;
     const bm2_sam_result &res = *in->res;
     const int64_t n_reads = in->reads->n_reads;
@@ -173,7 +185,7 @@ extern "C" int bm2_sam_format(const bm2_sam_text_in *in, int n_threads, char **t
     if ((int64_t) n_threads > n_reads) n_threads = n_reads > 0 ? (int) n_reads : 1;
     std::vector<Job> jobs((size_t) n_threads);
     for (int t = 0; t < n_threads; ++t) {
-        jobs[t].in = in; jobs[t].first_rec_of_read = first_rec.data(); jobs[t].first_xa_of_read = first_xa.data();
+        jobs[t].in = in; jobs[t].x = x; jobs[t].first_rec_of_read = first_rec.data(); jobs[t].first_xa_of_read = first_xa.data();
         jobs[t].r0 = n_reads * t / n_threads; jobs[t].r1 = n_reads * (t + 1) / n_threads;
     }
     {
@@ -199,5 +211,7 @@ extern "C" int bm2_sam_format(const bm2_sam_text_in *in, int n_threads, char **t
     *text = buf; *len = (int64_t) total;
     return 0;
 }
+
+extern "C" int bm2_sam_format(const bm2_sam_text_in *in, int n_threads, char **text, int64_t *len) { return bm2_sam_format_ex(in, nullptr, n_threads, text, len); }
 
 extern "C" void bm2_free(void *p) { free(p); }

@@ -345,6 +345,21 @@ typedef struct bm2_fastq_batch {
     const int64_t *name_beg; const int32_t *name_len;     /* HOST: QNAME of read r = its buffer [name_beg[r], + name_len[r])  */
 } bm2_fastq_batch;
 int  bm2_fastq_encode(bm2_ctx *ctx, const char *buf1, int64_t n1, const char *buf2, int64_t n2, bm2_fastq_batch *out);
+/* FASTQ comments of the reads of the context's last bm2_fastq_encode call, as kseq reads them (src/kseq.h:196): the rest of the header line after
+ * the blank that ends the name, one trailing '\r' dropped from a comment longer than one byte.  Comment of read r = its buffer [beg[r], + len[r]);
+ * len[r] == 0: none.  HOST arrays owned by the context (valid until its next bm2_fastq_* call).  This is what `bwa-mem2 mem -C` appends. */
+int  bm2_fastq_comments(bm2_ctx *ctx, const int64_t **beg, const int32_t **len);
+/* Smart pairing (`bwa-mem2 mem -p`, src/fastmap.cpp:249-296): splits the context's last single-end bm2_fastq_encode batch on the GPU as bseq_classify
+ * (src/bwa.cpp:226-242) does - read i pairs with read i-1 when their names (after trim_readno) are equal and read i-1 is not already paired with
+ * read i-2; every other read is single-end.  set[0]: the single-end reads, set[1]: the pairs (reads 2i, 2i+1 are mates), both in file order and
+ * laid out as a bm2_fastq_batch is, with device and host arrays; names and comments are spans of the encoded buffer.  read_index[s][j]: the read of the
+ * encoded batch that read j of set s is.  Arrays are owned by the context (valid until its next bm2_fastq_* call). */
+typedef struct bm2_fastq_split {
+    bm2_fastq_batch set[2];
+    const int64_t *comment_beg[2]; const int32_t *comment_len[2];
+    const int32_t *read_index[2];
+} bm2_fastq_split;
+int  bm2_fastq_smart_pair(bm2_ctx *ctx, bm2_fastq_split *out);
 
 /* ---- seam 5 (SURVEY 8f item 3, host I/O on the fast side): SAM text of a chunk --------------------------------------------------------
  * The formatting half of mem_aln2sam (src/bwamem.cpp:1592-1730): QNAME, the tab-separated columns, SEQ / QUAL trimmed by the record's
@@ -363,6 +378,18 @@ typedef struct bm2_sam_text_in {
     const int64_t *name_beg; const int32_t *name_len;
 } bm2_sam_text_in;
 int  bm2_sam_format(const bm2_sam_text_in *in, int n_threads, char **text, int64_t *len);
+/* The -R / -C / -V additions of mem_aln2sam (src/bwamem.cpp:1693, :1720-1728): RG:Z:<rg_id> after XS, the read's FASTQ comment after XA (a tab,
+ * then the comment as it is), and XR:Z:<contig annotation> last on mapped records when ref_hdr is set and the annotation is not empty (its tabs
+ * printed as spaces).  Comment of read r = the same buffer as its QNAME (bm2_sam_text_in::name_buf) [comment_beg[r], + comment_len[r]). */
+typedef struct bm2_sam_text_extra {
+    const char *rg_id;                            /* NULL or "": no RG tag                                                   */
+    const int64_t *comment_beg;                   /* NULL: no comments; comment_len[r] == 0: none for read r                 */
+    const int32_t *comment_len;
+    const char *const *contig_anno;               /* annotation by contig id (bntann1_t::anno, "" for none); NULL: none    */
+    int32_t ref_hdr;                              /* -V                                                                      */
+} bm2_sam_text_extra;
+/* bm2_sam_format with the additions; x == NULL is bm2_sam_format. */
+int  bm2_sam_format_ex(const bm2_sam_text_in *in, const bm2_sam_text_extra *x, int n_threads, char **text, int64_t *len);
 void bm2_free(void *p);
 
 /* Staged mate rescue inside bm2_sam_pe (same records, other kernels): the windows mem_matesw (src/bwamem_pair.cpp:150-283) can ask for are
