@@ -83,7 +83,8 @@ class FastqSplit(C.Structure):
 
 
 class SamTextExtra(C.Structure):
-    _fields_ = [("rg_id", C.c_char_p), ("comment_beg", C.c_void_p), ("comment_len", C.c_void_p), ("contig_anno", C.c_void_p), ("ref_hdr", C.c_int32)]
+    _fields_ = [("rg_id", C.c_char_p), ("comment_beg", C.c_void_p), ("comment_len", C.c_void_p), ("contig_anno", C.c_void_p), ("ref_hdr", C.c_int32),
+                ("qual_present", C.c_void_p)]
 
 
 def _host(p, n, dt):
@@ -92,11 +93,11 @@ def _host(p, n, dt):
 
 
 def sam_format(recs, xa, cigar, md, codes, offsets, contig_names, read_names=None, quals=None, n_threads=1, name_spans=None,
-               rg_id=None, comments=None, contig_anno=None, ref_hdr=False) -> bytes:
+               rg_id=None, comments=None, contig_anno=None, ref_hdr=False, qual_present=None) -> bytes:
     """bm2_sam_format: the SAM text of a batch from the records of bm2_sam_pe / bm2_sam_se (one line per record, QNAME to the last tag).
     read_names: list of names, or name_spans = (buf1, buf2 or None, name_beg int64[], name_len int32[]) as bm2_fastq_encode returns them.
     With rg_id (-R), comments = (comment_beg int64[], comment_len int32[]) into the buffers of name_spans (-C) or contig_anno (list of str)
-    with ref_hdr (-V): bm2_sam_format_ex."""
+    with ref_hdr (-V), or qual_present (uint8[] per read, 0: QUAL '*', as bm2_seq_encode returns it): bm2_sam_format_ex."""
     recs = np.ascontiguousarray(recs, SAM_REC_DT); xa = np.ascontiguousarray(xa, SAM_XA_DT)
     cigar = np.ascontiguousarray(cigar, np.uint32); md = np.ascontiguousarray(md, np.uint8)
     codes = np.ascontiguousarray(codes, np.uint8); offsets = np.ascontiguousarray(offsets, np.int64)
@@ -113,7 +114,7 @@ def sam_format(recs, xa, cigar, md, codes, offsets, contig_names, read_names=Non
         tin.name_buf[0] = b1; tin.name_buf[1] = b2
         tin.name_beg = nbeg.ctypes.data; tin.name_len = nlen.ctypes.data
     text = C.c_void_p(); n = C.c_int64()
-    if rg_id is None and comments is None and contig_anno is None and not ref_hdr:
+    if rg_id is None and comments is None and contig_anno is None and not ref_hdr and qual_present is None:
         f = lib().bm2_sam_format
         f.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
         rc = f(C.byref(tin), int(n_threads), C.byref(text), C.byref(n))
@@ -125,6 +126,9 @@ def sam_format(recs, xa, cigar, md, codes, offsets, contig_names, read_names=Non
         if contig_anno is not None:
             ca = (C.c_char_p * len(contig_anno))(*[s.encode() if isinstance(s, str) else bytes(s) for s in contig_anno])
             x.contig_anno = C.cast(ca, C.c_void_p)
+        if qual_present is not None:
+            qp = np.ascontiguousarray(qual_present, np.uint8)
+            x.qual_present = qp.ctypes.data
         f = lib().bm2_sam_format_ex
         f.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
         rc = f(C.byref(tin), C.byref(x), int(n_threads), C.byref(text), C.byref(n))
@@ -153,7 +157,7 @@ class RegResult(C.Structure):
     _fields_ = [("n", C.c_int64), ("regs", C.c_void_p), ("read_off", C.c_void_p)]
 
 
-EXPORTS = ["bm2_create_sibling", "bm2_fastq_encode", "bm2_fastq_comments", "bm2_fastq_smart_pair", "bm2_sam_format", "bm2_sam_format_ex", "bm2_free", "bm2_create_resident", "bm2_gather_probe", "bm2_set_sam_staged", "bm2_last_sam_stats", "bm2_gather64_gbs", "bm2_set_sub_batches", "bm2_seed_chain_extend_resident", "bm2_last_counters", "bm2_set_stream", "bm2_int_pipe_gops", "bm2_abi_version", "bm2_opt_init", "bm2_index_load", "bm2_index_free", "bm2_create", "bm2_destroy",
+EXPORTS = ["bm2_create_sibling", "bm2_fastq_encode", "bm2_seq_encode", "bm2_fastq_comments", "bm2_fastq_smart_pair", "bm2_sam_format", "bm2_sam_format_ex", "bm2_free", "bm2_create_resident", "bm2_gather_probe", "bm2_set_sam_staged", "bm2_last_sam_stats", "bm2_gather64_gbs", "bm2_set_sub_batches", "bm2_seed_chain_extend_resident", "bm2_last_counters", "bm2_set_stream", "bm2_int_pipe_gops", "bm2_abi_version", "bm2_opt_init", "bm2_index_load", "bm2_index_free", "bm2_create", "bm2_destroy",
            "bm2_last_error", "bm2_extend_pairs", "bm2_extend_pairs_device", "bm2_collect_smems", "bm2_seed_chain",
            "bm2_seed_chain_extend", "bm2_last_stage_ms", "bm2_gen_cigar", "bm2_pestat", "bm2_sam_pe", "bm2_sam_se", "bm2_ksw_align2"]
 
@@ -364,6 +368,9 @@ class Context:
         f = lib().bm2_fastq_encode
         f.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, C.c_char_p, C.c_int64, C.c_void_p]
         self._check(f(self._ctx, buf1, len(buf1), buf2, len(buf2) if buf2 is not None else 0, C.byref(b)), "bm2_fastq_encode")
+        return self._fq_batch(b, buf1, buf2, want_names)
+
+    def _fq_batch(self, b, buf1, buf2, want_names):
         n = b.n_reads
         self._fq_n = n
         offs = np.ctypeslib.as_array(C.cast(b.offsets, C.POINTER(C.c_int64)), shape=(n + 1,)).copy()
@@ -377,6 +384,17 @@ class Context:
         names = [bufs[r % stride][nb[r]:nb[r] + nl[r]] for r in range(n)] if want_names else None
         return dict(n_reads=n, codes=codes, offsets=offs, quals=quals, names=names, d_codes=b.d_codes, d_offsets=b.d_offsets,
                     name_spans=(buf1, buf2, nb, nl))
+
+    def seq_encode(self, buf1: bytes, buf2: bytes | None = None, want_names: bool = True):
+        """bm2_seq_encode: raw bytes of whole FASTA / FASTQ records of a chunk (two files for pairs), any shape kseq reads -> the dict of
+        fastq_encode plus qual_present (uint8 per read, 0: no qualities; their bytes in quals are then unset)."""
+        b = FastqBatch(); qp = C.c_void_p()
+        f = lib().bm2_seq_encode
+        f.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, C.c_char_p, C.c_int64, C.c_void_p, C.c_void_p]
+        self._check(f(self._ctx, buf1, len(buf1), buf2, len(buf2) if buf2 is not None else 0, C.byref(b), C.byref(qp)), "bm2_seq_encode")
+        out = self._fq_batch(b, buf1, buf2, want_names)
+        out["qual_present"] = _host(qp, out["n_reads"], np.uint8)
+        return out
 
     def fastq_comments(self):
         """bm2_fastq_comments: (comment_beg int64[], comment_len int32[]) of the reads of the last fastq_encode, into their buffers."""

@@ -26,7 +26,7 @@ struct DevIndex {                 // FM-index + reference resident in HBM (repli
 
 struct bm2_ctx {
     int device = 0, n_sm = 132;
-    int fq_n_reads = 0, fq_n_bufs = 0;   // last successful bm2_fastq_encode (fastq.cu): reads, buffers (0: none)
+    int fq_n_reads = 0, fq_n_bufs = 0;   // last successful bm2_fastq_encode / bm2_seq_encode (fastq.cu): reads, buffers (0: none)
     cudaStream_t stream = nullptr, own_stream = nullptr, side_stream = nullptr;
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     bm2_mem_opt_t opt;
@@ -36,8 +36,8 @@ struct bm2_ctx {
     // seam 1
     DevBuf io_pairs, io_ref, io_qer, bsw_jobs, bsw_outs, bsw_scratch;
     // seam 2 (pipeline.cu)
-    DevBuf d[128];         // slots: pipeline.cu 0-47, cigar.cu 48-63, sam.cu 64-83 + 90-95, ksw.cu 84-89, fastq.cu 100-126
-    HostBuf h[48];         // slots: pipeline.cu 0-7, cigar.cu 8-15, sam.cu 16-23, fastq.cu 24-47
+    DevBuf d[144];         // slots: pipeline.cu 0-47, cigar.cu 48-63, sam.cu 64-83 + 90-95, ksw.cu 84-89, fastq.cu 100-126 + 128-143
+    HostBuf h[52];         // slots: pipeline.cu 0-7, cigar.cu 8-15, sam.cu 16-23, fastq.cu 24-51
     std::vector<cudaEvent_t> events;
     std::vector<const char *> stage_names;
     std::vector<float> stage_ms;

@@ -9,6 +9,7 @@
 // Restriction (checked, reported as an error): four-line records (no wrapped sequence lines), chunks below 2 GiB per buffer.
 #include "bm2_common.cuh"
 #include "bm2_ctx.h"
+#include "seq_grammar.cuh"
 #include <cub/device/device_select.cuh>
 #include <cub/device/device_scan.cuh>
 #include <cub/iterator/counting_input_iterator.cuh>
@@ -312,5 +313,272 @@ extern "C" int bm2_fastq_smart_pair(bm2_ctx *ctx, bm2_fastq_split *out) {
         b.name_beg = nb; b.name_len = nlv;
         out->comment_beg[s] = cb; out->comment_len[s] = cl; out->read_index[s] = idx;
     }
+    return 0;
+}
+
+// ---- bm2_seq_encode: every input kseq reads (FASTA, wrapped FASTQ, mixed, junk, CRLF), parsed on the GPU by seq_grammar.cuh --------------
+// Per buffer: the positions of '\n' and of '>' / '@' by stream compaction; for every line start the first '>' / '@' at or after it - every
+// record's header character is one of these candidates (after a FASTQ record kseq skips to the next such byte, after a FASTA record the
+// header is the first byte of a line); one thread per candidate runs seq_record, whose next header is again a candidate, so next() is a
+// forest pointing right; the records are the chain from the first candidate, marked by pointer doubling (log K jump tables, marks pushed
+// from the top level down: the nodes 2^t steps apart are those 2^(t+1) apart plus one jump of 2^t from each); then one warp per record
+// walks it again and writes its codes and qualities where the sink puts them.
+// Cost of the candidate walks: one walk per line start whose first '>' / '@' differs from the previous line's - about one per record for
+// four-line FASTQ (plus one per quality line holding a '>' or '@'), one per record for FASTA (its sequence lines share the candidate),
+// and up to one per quality line for wrapped FASTQ; a walk is as long as the record it parses from its candidate.
+// sm_90a (ptxas -v), no spills in any of them: seq_gather_kernel 40 registers, seq_walk_kernel 27, seq_span_kernel 26, seq_cand_kernel 22,
+// seq_jump_kernel 12, seq_flag_kernel 12, seq_mark_kernel 8.
+namespace {
+
+struct IsHeaderChar {
+    const char *raw;
+    __device__ __forceinline__ bool operator()(const int &i) const { return raw[i] == '>' || raw[i] == '@'; }
+};
+struct HeaderCharAsInt {
+    const char *raw;
+    __device__ __forceinline__ int operator()(const int &i) const { return raw[i] == '>' || raw[i] == '@'; }
+};
+
+// what a candidate's walk leaves for the record table
+struct SeqCand { int32_t h, l_seq, name_beg, name_len, cmt_beg, cmt_len; int8_t status, has_qual, _p[2]; };
+
+// line k (0..n_nl) starts at 0 or nl[k-1] + 1: its first header character at or after the start
+__global__ void seq_cand_kernel(SeqTableSrc s, int32_t *cand) {
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k > s.n_nl) return;
+    cand[k] = (int32_t) s.hdr(k == 0 ? 0 : (int64_t) s.nl[k - 1] + 1);
+}
+
+// one thread per candidate: its record and next(); nxt[K] = K is the end of every chain
+__global__ void seq_walk_kernel(SeqTableSrc s, const int32_t *__restrict__ cand, int K, int32_t *nxt, SeqCand *info) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i > K) return;
+    if (i == K) { nxt[K] = K; return; }
+    s.k = 0;
+    const SeqRec r = seq_record(s, cand[i], SeqNullSink());
+    int j = K;
+    if (r.status == SEQ_OK && r.next < s.n) {
+        int lo = i + 1, hi = K;
+        while (lo < hi) { const int m = (lo + hi) >> 1; if (cand[m] < r.next) lo = m + 1; else hi = m; }
+        j = lo;
+    }
+    nxt[i] = j;
+    SeqCand c; c.h = cand[i]; c.l_seq = r.l_seq; c.name_beg = (int32_t) r.name_beg; c.name_len = r.name_len; c.cmt_beg = (int32_t) r.cmt_beg;
+    c.cmt_len = r.cmt_len; c.status = r.status; c.has_qual = r.l_qual > 0; c._p[0] = c._p[1] = 0;
+    info[i] = c;
+}
+
+__global__ void seq_jump_kernel(const int32_t *__restrict__ a, int K, int32_t *b) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i <= K) b[i] = a[a[i]];
+}
+
+// level t: every marked node marks its 2^t-th successor (in place: a node marked during this pass only marks nodes of the level above)
+__global__ void seq_mark_kernel(const int32_t *__restrict__ jump, int K, uint8_t *mark) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i <= K && mark[i]) mark[jump[i]] = 1;
+}
+
+__global__ void seq_flag_kernel(const uint8_t *__restrict__ mark, const SeqCand *__restrict__ info, int K, uint8_t *flag) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < K) flag[i] = mark[i] && info[i].status != SEQ_NONE;
+}
+
+// records of buffer `file` -> spans, lengths, qualities present
+__global__ void seq_span_kernel(const SeqCand *__restrict__ rec, int n_rec, int file, int stride, Span *spans, int64_t *lens, uint8_t *qp) {
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n_rec) return;
+    const SeqCand c = rec[r];
+    const int read = r * stride + file;
+    Span s; s.seq_beg = c.h; s.seq_len = c.l_seq; s.qual_beg = 0; s.name_beg = c.name_beg; s.name_len = c.name_len; s.cmt_beg = c.cmt_beg;
+    s.cmt_len = c.cmt_len; s._pad = 0;
+    spans[read] = s;
+    lens[read] = c.l_seq;
+    qp[read] = (uint8_t) c.has_qual;
+}
+
+struct SeqWarpSink {            // every lane runs the same walk; the lanes split each line's bytes
+    uint8_t *codes; char *quals; int lane; const char *raw;
+    __device__ void seq(int64_t b, int64_t k, int64_t at) const { for (int64_t i = lane; i < k; i += 32) codes[at + i] = nt4((unsigned char) raw[b + i]); }
+    __device__ void qual(int64_t b, int64_t k, int64_t at) const { for (int64_t i = lane; i < k; i += 32) quals[at + i] = raw[b + i]; }
+};
+
+// one warp per read: the record walked again from its header, its kept bytes written as codes and qualities
+__global__ void seq_gather_kernel(SeqTableSrc s0, SeqTableSrc s1, const Span *__restrict__ spans, const int64_t *__restrict__ offs, int n_reads, int stride,
+                                  uint8_t *codes, char *quals) {
+    const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31, nw = (gridDim.x * blockDim.x) >> 5;
+    for (int rd = w; rd < n_reads; rd += nw) {
+        SeqTableSrc s = (stride == 2 && (rd & 1)) ? s1 : s0;
+        s.k = 0;
+        const int64_t o = offs[rd];
+        SeqWarpSink sink = { codes + o, quals + o, lane, s.raw };
+        seq_record(s, spans[rd].seq_beg, sink);
+    }
+}
+
+enum SeqBuf { S_HP0 = 128, S_HP1, S_CAND, S_CANDU, S_INFO, S_JUMP, S_MARK, S_FLAG, S_REC0, S_REC1, S_QP, S_CNT };
+enum SeqHost { FH_QP = 48 };
+static_assert(S_CNT < 144, "bm2_ctx::d[] slots");
+
+}  // namespace
+
+extern "C" int bm2_seq_encode(bm2_ctx *ctx, const char *buf1, int64_t n1, const char *buf2, int64_t n2, bm2_fastq_batch *out, const uint8_t **qual_present) {
+    bm2_ctx *ctx_for_error = ctx;
+    if (!ctx || !out || !buf1 || n1 < 0 || (buf2 && n2 < 0)) { if (ctx) bm2_set_error(ctx, "bm2_seq_encode: bad arguments"); return 1; }
+    if (n1 >= (1LL << 31) - 16 || (buf2 && n2 >= (1LL << 31) - 16)) { bm2_set_error(ctx, "bm2_seq_encode: a chunk must stay below 2 GiB per buffer"); return 1; }
+    ctx->fq_n_reads = ctx->fq_n_bufs = 0;
+    BM2_CUDA_OK(cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->stream;
+    const int nbuf = buf2 ? 2 : 1;
+    const char *hb[2] = { buf1, buf2 }; const int64_t hn[2] = { n1, buf2 ? n2 : 0 };
+    int n_rec[2] = { 0, 0 };
+    SeqTableSrc src[2] = {};
+    int bad[2] = { -1, -1 };                                       // per buffer: index of the malformed record, -1: none
+    if (ctx->ensure(ctx->d[S_CNT], 64)) return 1;
+    int *d_cnt = (int *) ctx->d[S_CNT].p;
+    // compaction of the positions i < n where pred(raw[i]) into slot `dst` (counted first to size it)
+    auto positions = [&](int b, int slot, bool newline, int *count) -> int {
+        const char *d_raw = (const char *) ctx->d[F_RAW0 + b].p;
+        cub::CountingInputIterator<int> it(0);
+        size_t tmp = 0;
+        int h_n = 0;
+        if (newline) {
+            cub::TransformInputIterator<int, NewlineAsInt, cub::CountingInputIterator<int>> cnt_it(it, NewlineAsInt{ d_raw });
+            cub::DeviceReduce::Sum(nullptr, tmp, cnt_it, d_cnt, (int) hn[b], st);
+            if (ctx->ensure(ctx->d[F_TMP], tmp)) return 1;
+            BM2_CUDA_OK(cub::DeviceReduce::Sum(ctx->d[F_TMP].p, tmp, cnt_it, d_cnt, (int) hn[b], st));
+        } else {
+            cub::TransformInputIterator<int, HeaderCharAsInt, cub::CountingInputIterator<int>> cnt_it(it, HeaderCharAsInt{ d_raw });
+            cub::DeviceReduce::Sum(nullptr, tmp, cnt_it, d_cnt, (int) hn[b], st);
+            if (ctx->ensure(ctx->d[F_TMP], tmp)) return 1;
+            BM2_CUDA_OK(cub::DeviceReduce::Sum(ctx->d[F_TMP].p, tmp, cnt_it, d_cnt, (int) hn[b], st));
+        }
+        BM2_CUDA_OK(cudaMemcpyAsync(&h_n, d_cnt, 4, cudaMemcpyDeviceToHost, st));
+        BM2_CUDA_OK(cudaStreamSynchronize(st));
+        if (ctx->ensure(ctx->d[slot], ((size_t) h_n + 16) * 4)) return 1;
+        tmp = 0;
+        if (newline) {
+            IsNewline pred = { d_raw };
+            cub::DeviceSelect::If(nullptr, tmp, it, (int32_t *) ctx->d[slot].p, d_cnt, (int) hn[b], pred, st);
+            if (ctx->ensure(ctx->d[F_TMP], tmp)) return 1;
+            BM2_CUDA_OK(cub::DeviceSelect::If(ctx->d[F_TMP].p, tmp, it, (int32_t *) ctx->d[slot].p, d_cnt, (int) hn[b], pred, st));
+        } else {
+            IsHeaderChar pred = { d_raw };
+            cub::DeviceSelect::If(nullptr, tmp, it, (int32_t *) ctx->d[slot].p, d_cnt, (int) hn[b], pred, st);
+            if (ctx->ensure(ctx->d[F_TMP], tmp)) return 1;
+            BM2_CUDA_OK(cub::DeviceSelect::If(ctx->d[F_TMP].p, tmp, it, (int32_t *) ctx->d[slot].p, d_cnt, (int) hn[b], pred, st));
+        }
+        *count = h_n;
+        return 0;
+    };
+    for (int b = 0; b < nbuf; ++b) {
+        if (ctx->ensure(ctx->d[F_RAW0 + b], (size_t) hn[b] + 16)) return 1;
+        if (hn[b]) BM2_CUDA_OK(cudaMemcpyAsync(ctx->d[F_RAW0 + b].p, hb[b], (size_t) hn[b], cudaMemcpyHostToDevice, st));
+        int n_nl = 0, n_hp = 0;
+        if (hn[b] && (positions(b, F_NL0 + b, true, &n_nl) || positions(b, S_HP0 + b, false, &n_hp))) return 1;
+        if (!hn[b] && (ctx->ensure(ctx->d[F_NL0 + b], 64) || ctx->ensure(ctx->d[S_HP0 + b], 64))) return 1;
+        SeqTableSrc &s = src[b];
+        s.raw = (const char *) ctx->d[F_RAW0 + b].p; s.n = hn[b]; s.nl = (const int32_t *) ctx->d[F_NL0 + b].p; s.n_nl = n_nl;
+        s.hp = (const int32_t *) ctx->d[S_HP0 + b].p; s.n_hp = n_hp; s.k = 0;
+        if (n_hp == 0) { n_rec[b] = 0; if (ctx->ensure(ctx->d[S_REC0 + b], 64)) return 1; continue; }
+        // candidates: the first header character at or after each line start, deduplicated (non-decreasing in the line index)
+        const int n_ls = n_nl + 1;
+        if (ctx->ensure(ctx->d[S_CAND], (size_t) (n_ls + 16) * 4) || ctx->ensure(ctx->d[S_CANDU], (size_t) (n_ls + 16) * 4)) return 1;
+        int32_t *d_cand = (int32_t *) ctx->d[S_CAND].p, *d_cu = (int32_t *) ctx->d[S_CANDU].p;
+        seq_cand_kernel<<<(n_ls + 255) / 256, 256, 0, st>>>(s, d_cand);
+        {
+            size_t tmp = 0;
+            cub::DeviceSelect::Unique(nullptr, tmp, d_cand, d_cu, d_cnt, n_ls, st);
+            if (ctx->ensure(ctx->d[F_TMP], tmp)) return 1;
+            BM2_CUDA_OK(cub::DeviceSelect::Unique(ctx->d[F_TMP].p, tmp, d_cand, d_cu, d_cnt, n_ls, st));
+        }
+        int K = 0;
+        BM2_CUDA_OK(cudaMemcpyAsync(&K, d_cnt, 4, cudaMemcpyDeviceToHost, st));
+        BM2_CUDA_OK(cudaStreamSynchronize(st));
+        int32_t last = 0;
+        BM2_CUDA_OK(cudaMemcpyAsync(&last, d_cu + K - 1, 4, cudaMemcpyDeviceToHost, st));
+        BM2_CUDA_OK(cudaStreamSynchronize(st));
+        if (last >= hn[b]) --K;                         // "no header character after this line"
+        // next() of every candidate, then the jump tables J_t = next^(2^t), t < T with 2^T > K
+        int T = 1; while ((1LL << T) <= K) ++T;
+        if (ctx->ensure(ctx->d[S_INFO], (size_t) (K + 1) * sizeof(SeqCand)) || ctx->ensure(ctx->d[S_JUMP], (size_t) T * (K + 1) * 4) ||
+            ctx->ensure(ctx->d[S_MARK], (size_t) K + 16) || ctx->ensure(ctx->d[S_FLAG], (size_t) K + 16) ||
+            ctx->ensure(ctx->d[S_REC0 + b], (size_t) (K + 1) * sizeof(SeqCand))) return 1;
+        int32_t *d_jump = (int32_t *) ctx->d[S_JUMP].p;
+        SeqCand *d_info = (SeqCand *) ctx->d[S_INFO].p;
+        uint8_t *d_mark = (uint8_t *) ctx->d[S_MARK].p, *d_flag = (uint8_t *) ctx->d[S_FLAG].p;
+        const int gK = (K + 1 + 255) / 256;
+        seq_walk_kernel<<<gK, 256, 0, st>>>(s, d_cu, K, d_jump, d_info);
+        for (int t = 1; t < T; ++t) seq_jump_kernel<<<gK, 256, 0, st>>>(d_jump + (size_t) (t - 1) * (K + 1), K, d_jump + (size_t) t * (K + 1));
+        BM2_CUDA_OK(cudaMemsetAsync(d_mark, 0, (size_t) K + 1, st));
+        BM2_CUDA_OK(cudaMemsetAsync(d_mark, 1, 1, st));
+        for (int t = T - 1; t >= 0; --t) seq_mark_kernel<<<gK, 256, 0, st>>>(d_jump + (size_t) t * (K + 1), K, d_mark);
+        seq_flag_kernel<<<gK, 256, 0, st>>>(d_mark, d_info, K, d_flag);
+        {
+            size_t tmp = 0;
+            cub::DeviceSelect::Flagged(nullptr, tmp, d_info, d_flag, (SeqCand *) ctx->d[S_REC0 + b].p, d_cnt, K, st);
+            if (ctx->ensure(ctx->d[F_TMP], tmp)) return 1;
+            BM2_CUDA_OK(cub::DeviceSelect::Flagged(ctx->d[F_TMP].p, tmp, d_info, d_flag, (SeqCand *) ctx->d[S_REC0 + b].p, d_cnt, K, st));
+        }
+        BM2_CUDA_OK(cudaMemcpyAsync(&n_rec[b], d_cnt, 4, cudaMemcpyDeviceToHost, st));
+        BM2_CUDA_OK(cudaStreamSynchronize(st));
+        // a malformed record ends its chain (its next() is K), so only the last record of the buffer can be one
+        if (n_rec[b] > 0) {
+            SeqCand lastc;
+            BM2_CUDA_OK(cudaMemcpyAsync(&lastc, (const SeqCand *) ctx->d[S_REC0 + b].p + n_rec[b] - 1, sizeof lastc, cudaMemcpyDeviceToHost, st));
+            BM2_CUDA_OK(cudaStreamSynchronize(st));
+            if (lastc.status == SEQ_BAD) bad[b] = n_rec[b] - 1;
+        }
+    }
+    for (int b = 0; b < nbuf; ++b)                                // before the record counts: a malformed record also shortens its file
+        if (bad[b] >= 0) {
+            bm2_set_error(ctx, "bm2_seq_encode: malformed record " + std::to_string(bad[b]) + (nbuf == 2 ? (b ? " of the 2nd file" : " of the 1st file") : "") +
+                               " (a '+' line without qualities, or qualities of another length than the sequence)");
+            return 2;
+        }
+    if (nbuf == 2 && n_rec[0] != n_rec[1]) { bm2_set_error(ctx, "bm2_seq_encode: the two files hold different numbers of records"); return 2; }
+    const int n_reads = n_rec[0] * nbuf;
+    out->n_reads = n_reads;
+    if (ctx->ensure(ctx->d[F_SPANS], (size_t) (n_reads + 1) * sizeof(Span)) || ctx->ensure(ctx->d[F_LENS], (size_t) (n_reads + 2) * 8) ||
+        ctx->ensure(ctx->d[F_OFFS], (size_t) (n_reads + 2) * 8) || ctx->ensure(ctx->d[S_QP], (size_t) n_reads + 16)) return 1;
+    Span *d_spans = (Span *) ctx->d[F_SPANS].p; int64_t *d_lens = (int64_t *) ctx->d[F_LENS].p, *d_offs = (int64_t *) ctx->d[F_OFFS].p;
+    uint8_t *d_qp = (uint8_t *) ctx->d[S_QP].p;
+    BM2_CUDA_OK(cudaMemsetAsync(d_lens + n_reads, 0, 8, st));
+    for (int b = 0; b < nbuf && n_rec[b] > 0; ++b)
+        seq_span_kernel<<<(n_rec[b] + 255) / 256, 256, 0, st>>>((const SeqCand *) ctx->d[S_REC0 + b].p, n_rec[b], b, nbuf, d_spans, d_lens, d_qp);
+    {
+        size_t tmp = 0;
+        cub::DeviceScan::ExclusiveSum(nullptr, tmp, d_lens, d_offs, n_reads + 1, st);
+        if (ctx->ensure(ctx->d[F_TMP], tmp)) return 1;
+        BM2_CUDA_OK(cub::DeviceScan::ExclusiveSum(ctx->d[F_TMP].p, tmp, d_lens, d_offs, n_reads + 1, st));
+    }
+    int64_t total = 0;
+    BM2_CUDA_OK(cudaMemcpyAsync(&total, d_offs + n_reads, 8, cudaMemcpyDeviceToHost, st));
+    BM2_CUDA_OK(cudaStreamSynchronize(st));
+    if (ctx->ensure(ctx->d[F_CODES], (size_t) total + 16) || ctx->ensure(ctx->d[F_QUALS], (size_t) total + 16)) return 1;
+    if (n_reads > 0) {
+        int blocks = (n_reads + 7) / 8; if (blocks > ctx->n_sm * 16) blocks = ctx->n_sm * 16;
+        seq_gather_kernel<<<blocks, 256, 0, st>>>(src[0], nbuf == 2 ? src[1] : src[0], d_spans, d_offs, n_reads, nbuf, (uint8_t *) ctx->d[F_CODES].p,
+                                                  (char *) ctx->d[F_QUALS].p);
+    }
+    if (ctx->ensure_host(ctx->h[FH_OFFS], (size_t) (n_reads + 1) * 8) || ctx->ensure_host(ctx->h[FH_CODES], (size_t) total + 16) ||
+        ctx->ensure_host(ctx->h[FH_QUALS], (size_t) total + 16) || ctx->ensure_host(ctx->h[FH_SPANS], (size_t) (n_reads + 1) * sizeof(Span)) ||
+        ctx->ensure_host(ctx->h[FH_NAMEBEG], (size_t) (n_reads + 1) * 8) || ctx->ensure_host(ctx->h[FH_NAMELEN], (size_t) (n_reads + 1) * 4) ||
+        ctx->ensure_host(ctx->h[FH_QP], (size_t) n_reads + 16)) return 1;
+    BM2_CUDA_OK(cudaMemcpyAsync(ctx->h[FH_OFFS].p, d_offs, (size_t) (n_reads + 1) * 8, cudaMemcpyDeviceToHost, st));
+    if (total) BM2_CUDA_OK(cudaMemcpyAsync(ctx->h[FH_CODES].p, ctx->d[F_CODES].p, (size_t) total, cudaMemcpyDeviceToHost, st));
+    if (total) BM2_CUDA_OK(cudaMemcpyAsync(ctx->h[FH_QUALS].p, ctx->d[F_QUALS].p, (size_t) total, cudaMemcpyDeviceToHost, st));
+    if (n_reads) BM2_CUDA_OK(cudaMemcpyAsync(ctx->h[FH_SPANS].p, d_spans, (size_t) n_reads * sizeof(Span), cudaMemcpyDeviceToHost, st));
+    if (n_reads) BM2_CUDA_OK(cudaMemcpyAsync(ctx->h[FH_QP].p, d_qp, (size_t) n_reads, cudaMemcpyDeviceToHost, st));
+    BM2_CUDA_OK(cudaStreamSynchronize(st));
+    BM2_CUDA_OK(cudaGetLastError());
+    const Span *hs = (const Span *) ctx->h[FH_SPANS].p;
+    int64_t *nb = (int64_t *) ctx->h[FH_NAMEBEG].p; int32_t *nlv = (int32_t *) ctx->h[FH_NAMELEN].p;
+    for (int r = 0; r < n_reads; ++r) { nb[r] = hs[r].name_beg; nlv[r] = hs[r].name_len; }
+    out->d_codes = (const uint8_t *) ctx->d[F_CODES].p; out->d_offsets = d_offs;
+    out->codes = (const uint8_t *) ctx->h[FH_CODES].p; out->offsets = (const int64_t *) ctx->h[FH_OFFS].p;
+    out->quals = (const char *) ctx->h[FH_QUALS].p; out->name_beg = nb; out->name_len = nlv;
+    if (qual_present) *qual_present = (const uint8_t *) ctx->h[FH_QP].p;
+    ctx->fq_n_reads = n_reads; ctx->fq_n_bufs = nbuf;
     return 0;
 }

@@ -66,7 +66,7 @@ void format_read_range(Job &j) {
         const int64_t k0 = j.first_rec_of_read[rd], k1 = j.first_rec_of_read[rd + 1];
         const int64_t so = rb.offsets[rd], l_seq = rb.offsets[rd + 1] - so;
         const uint8_t *seq = rb.codes + so;
-        const char *qual = in.quals ? in.quals + so : nullptr;
+        const char *qual = in.quals && !(j.x && j.x->qual_present && !j.x->qual_present[rd]) ? in.quals + so : nullptr;
         for (int64_t k = k0; k < k1; ++k) {
             const bm2_sam_rec &r = res.recs[k];
             Out &o = j.out;

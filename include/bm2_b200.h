@@ -360,6 +360,14 @@ typedef struct bm2_fastq_split {
     const int32_t *read_index[2];
 } bm2_fastq_split;
 int  bm2_fastq_smart_pair(bm2_ctx *ctx, bm2_fastq_split *out);
+/* Every input kseq reads (kseq_read, src/kseq.h:185-227, as bseq_read_orig calls it, src/bwa.cpp:170-216): FASTA and FASTQ, wrapped or not and
+ * mixed in one file, blank lines, junk before and between records, CRLF line ends - parsed on the GPU by the grammar of csrc/seq_grammar.cuh,
+ * with kseq's '\r' rule and trim_readno.  The contract is that of bm2_fastq_encode: whole records of a chunk in (buf2 NULL: single-end), the same
+ * batch out, and bm2_fastq_comments / bm2_fastq_smart_pair work on it.  *qual_present (HOST, n_reads, owned by the context): 0 where kseq leaves
+ * the read without qualities (a FASTA record, or an empty quality string) and SAM prints '*'; the read's bytes in out->quals are then unset.
+ * A malformed record (a '+' line without a line end, or qualities of another length than the sequence: kseq_read returns -2) is an error naming
+ * the record; the reference instead stops reading there without a message.  A chunk must stay below 2 GiB per buffer. */
+int  bm2_seq_encode(bm2_ctx *ctx, const char *buf1, int64_t n1, const char *buf2, int64_t n2, bm2_fastq_batch *out, const uint8_t **qual_present);
 
 /* ---- seam 5 (SURVEY 8f item 3, host I/O on the fast side): SAM text of a chunk --------------------------------------------------------
  * The formatting half of mem_aln2sam (src/bwamem.cpp:1592-1730): QNAME, the tab-separated columns, SEQ / QUAL trimmed by the record's
@@ -387,6 +395,7 @@ typedef struct bm2_sam_text_extra {
     const int32_t *comment_len;
     const char *const *contig_anno;               /* annotation by contig id (bntann1_t::anno, "" for none); NULL: none    */
     int32_t ref_hdr;                              /* -V                                                                      */
+    const uint8_t *qual_present;                  /* NULL: every read has qualities; qual_present[r] == 0: QUAL '*'         */
 } bm2_sam_text_extra;
 /* bm2_sam_format with the additions; x == NULL is bm2_sam_format. */
 int  bm2_sam_format_ex(const bm2_sam_text_in *in, const bm2_sam_text_extra *x, int n_threads, char **text, int64_t *len);
