@@ -159,7 +159,8 @@ class RegResult(C.Structure):
 
 EXPORTS = ["bm2_create_sibling", "bm2_fastq_encode", "bm2_seq_encode", "bm2_fastq_comments", "bm2_fastq_smart_pair", "bm2_sam_format", "bm2_sam_format_ex", "bm2_free", "bm2_create_resident", "bm2_gather_probe", "bm2_set_sam_staged", "bm2_last_sam_stats", "bm2_gather64_gbs", "bm2_set_sub_batches", "bm2_seed_chain_extend_resident", "bm2_last_counters", "bm2_set_stream", "bm2_int_pipe_gops", "bm2_abi_version", "bm2_opt_init", "bm2_index_load", "bm2_index_free", "bm2_create", "bm2_destroy",
            "bm2_last_error", "bm2_extend_pairs", "bm2_extend_pairs_device", "bm2_collect_smems", "bm2_seed_chain",
-           "bm2_seed_chain_extend", "bm2_last_stage_ms", "bm2_gen_cigar", "bm2_pestat", "bm2_sam_pe", "bm2_sam_se", "bm2_ksw_align2"]
+           "bm2_seed_chain_extend", "bm2_last_stage_ms", "bm2_gen_cigar", "bm2_pestat", "bm2_sam_pe", "bm2_sam_se", "bm2_ksw_align2",
+           "bm2_fasta_pack", "bm2_index_build"]
 
 _lib = None
 
@@ -206,6 +207,43 @@ def pestat(opt, l_pac, regs, read_off):
     if rc:
         raise Bm2Error(f"bm2_pestat failed ({rc})")
     return out
+
+
+class FastaPackStats(C.Structure):
+    _fields_ = [("l_pac", C.c_int64), ("n_seqs", C.c_int64), ("n_holes", C.c_int64), ("seconds", C.c_double)]
+
+
+class IndexBuildStats(C.Structure):
+    _fields_ = [("n", C.c_int64), ("peak_device_bytes", C.c_int64), ("rounds", C.c_int32), ("groups", C.c_int32), ("windows", C.c_int32),
+                ("pieces", C.c_int64), ("unresolved", C.c_int64), ("unresolved_on_host", C.c_int32),
+                ("load_s", C.c_double), ("pass1_s", C.c_double), ("refine_s", C.c_double), ("emit_s", C.c_double), ("total_s", C.c_double)]
+
+
+def _stats_dict(st) -> dict:
+    return {name: getattr(st, name) for name, _ in st._fields_}
+
+
+def fasta_pack(path: str, prefix: str) -> dict:
+    """bm2_fasta_pack (host only): <prefix>.pac / .ann / .amb of a FASTA or FASTQ file, plain or gzip, as `bwa-mem2 index` writes them."""
+    st = FastaPackStats()
+    f = lib().bm2_fasta_pack
+    f.restype = C.c_int
+    f.argtypes = [C.c_char_p, C.c_char_p, C.c_void_p]
+    if f(path.encode(), prefix.encode(), C.byref(st)):
+        raise Bm2Error(lib().bm2_last_error(None).decode())
+    return _stats_dict(st)
+
+
+def index_build(prefix: str, device: int = 0, work_bytes: int = 0) -> dict:
+    """bm2_index_build: <prefix>.0123 and <prefix>.bwt.2bit.64 from <prefix>.pac on the GPU.  work_bytes sizes the working buffers
+    (0: from the free device memory); returns the build's stats (peak device bytes, rounds, groups, pieces, windows, stage times)."""
+    st = IndexBuildStats()
+    f = lib().bm2_index_build
+    f.restype = C.c_int
+    f.argtypes = [C.c_int, C.c_char_p, C.c_int64, C.c_void_p]
+    if f(int(device), prefix.encode(), int(work_bytes), C.byref(st)):
+        raise Bm2Error(lib().bm2_last_error(None).decode())
+    return _stats_dict(st)
 
 
 class Index:

@@ -30,6 +30,7 @@ struct SeqRec {
     int64_t plus, qual_last;      // position of the '+' and start of the last quality line (-1: FASTA)
     int32_t l_seq, l_qual;
     int32_t lines;                // lines from the header line to the last line read
+    int32_t name_full_len;        // name length as kseq_read returns it, before trim_readno (bm2_fasta_pack keeps it)
     int8_t status;                // SEQ_OK, SEQ_NONE (no record: end of input), SEQ_BAD (kseq_read would return -2)
     int8_t simple;                // four-line FASTQ that fastq_spans_kernel parses to the same record (see seq_record)
 };
@@ -66,12 +67,13 @@ template <class Src, class Sink> BM2_HD SeqRec seq_record(const Src &s, int64_t 
     const char *raw = s.raw; const int64_t n = s.n;
     SeqRec r;
     r.next = n; r.end = n; r.name_beg = h + 1; r.cmt_beg = 0; r.name_len = 0; r.cmt_len = 0;
-    r.seq_first = r.seq_last = r.plus = r.qual_last = -1; r.l_seq = r.l_qual = 0; r.lines = 1; r.status = SEQ_NONE; r.simple = 0;
+    r.seq_first = r.seq_last = r.plus = r.qual_last = -1; r.l_seq = r.l_qual = 0; r.lines = 1; r.name_full_len = 0; r.status = SEQ_NONE; r.simple = 0;
     if (h + 1 >= n) return r;
     // name: up to the first isspace byte (ks_getuntil, KS_SEP_SPACE)
     int64_t i = h + 1;
     while (i < n && !seq_isspace((unsigned char) raw[i])) ++i;
     int32_t nl = (int32_t) (i - (h + 1));
+    r.name_full_len = nl;
     if (nl > 2 && raw[h + nl - 1] == '/' && raw[h + nl] >= '0' && raw[h + nl] <= '9') nl -= 2;
     r.name_len = nl;
     const unsigned char c0 = i < n ? (unsigned char) raw[i] : 0;

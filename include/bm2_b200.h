@@ -413,6 +413,35 @@ int bm2_set_sam_staged(bm2_ctx *ctx, int on);
  * alignments computed in place by the per-pair kernel (staged mode only), of those the ones whose window had moved, waves.  n_ms >= 4, n_counts >= 6. */
 int bm2_last_sam_stats(const bm2_ctx *ctx, double *ms, unsigned long long *counts, int n_ms, int n_counts);
 
+/* ---- bm2_index: `bwa-mem2 index` (bwa_idx_build, src/bwtindex.cpp:61-80) in two steps ---- */
+
+/* Step 1, host only: bns_fasta2bntseq(fp, prefix, 1) (src/bntseq.cpp:249-356).  Reads `path` (FASTA or FASTQ as kseq reads them, plain or gzip,
+ * every gzip member) and writes <prefix>.pac, .ann and .amb byte for byte as the reference does: ambiguous bases become lrand48() & 3 after
+ * srand48(11) (drawn from a private state; the caller's drand48 state is untouched), runs of the same ambiguous byte are holes in .amb.
+ * Unlike the reference, a malformed record (kseq_read's -2) and an input without bases (l_pac == 0) are errors (bm2_last_error(NULL)). */
+typedef struct bm2_fasta_pack_stats {
+    int64_t l_pac, n_seqs, n_holes;
+    double seconds;
+} bm2_fasta_pack_stats;
+int bm2_fasta_pack(const char *path, const char *prefix, bm2_fasta_pack_stats *stats);
+
+/* Step 2, on the GPU: FMI_search::build_index + build_fm_index (src/FMI_search.cpp:83-302, :306-382).  Reads <prefix>.pac and writes
+ * <prefix>.0123 and <prefix>.bwt.2bit.64 byte for byte as the reference does, from the suffix array of the forward + reverse-complement text
+ * (n = 2 l_pac), which is built on `device` and never held whole: the device keeps the text (2 bits per base) and a 5-byte inverse suffix array,
+ * and every other buffer is sized from work_bytes (0: from the free device memory).  Errors (bm2_last_error(NULL)) name the bytes needed and
+ * free when the persistent state does not fit. */
+typedef struct bm2_index_build_stats {
+    int64_t n;                          /* text length 2 l_pac                                                       */
+    int64_t peak_device_bytes;          /* the most device memory the build held at once                            */
+    int32_t rounds;                     /* prefix-doubling rounds after the 31-mer sort                              */
+    int32_t groups, windows;            /* bucket groups of the first pass, row windows of the emit                 */
+    int64_t pieces;                     /* refinement pieces over all rounds                                         */
+    int64_t unresolved;                 /* suffixes still tied after the 31-mer sort                                 */
+    int32_t unresolved_on_host;         /* 1 when the tied positions did not fit on the device                       */
+    double load_s, pass1_s, refine_s, emit_s, total_s;
+} bm2_index_build_stats;
+int bm2_index_build(int device, const char *prefix, int64_t work_bytes, bm2_index_build_stats *stats);
+
 #ifdef __cplusplus
 }
 #endif
