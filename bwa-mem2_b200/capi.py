@@ -140,6 +140,49 @@ def sam_format(recs, xa, cigar, md, codes, offsets, contig_names, read_names=Non
     return out
 
 
+def bam_format(recs, xa, cigar, md, codes, offsets, contig_names, read_names=None, quals=None, n_threads=1, name_spans=None,
+               rg_id=None, comments=None, contig_anno=None, ref_hdr=False, qual_present=None):
+    """bm2_bam_format_ex: the records of sam_format(...) (same arguments) as uncompressed BAM records -> (bytes, read_off int64[n_reads + 1]:
+    where each read's records start).  A long QNAME or a comment that is not SAM tags raises Bm2Error naming the read."""
+    recs = np.ascontiguousarray(recs, SAM_REC_DT); xa = np.ascontiguousarray(xa, SAM_XA_DT)
+    cigar = np.ascontiguousarray(cigar, np.uint32); md = np.ascontiguousarray(md, np.uint8)
+    codes = np.ascontiguousarray(codes, np.uint8); offsets = np.ascontiguousarray(offsets, np.int64)
+    res = SamResult(len(recs), recs.ctypes.data, len(xa), xa.ctypes.data, len(cigar), cigar.ctypes.data, len(md), md.ctypes.data)
+    rb = ReadBatch(len(offsets) - 1, codes.ctypes.data, offsets.ctypes.data)
+    cn = (C.c_char_p * len(contig_names))(*[s.encode() for s in contig_names])
+    rn = (C.c_char_p * len(read_names))(*[s.encode() if isinstance(s, str) else bytes(s) for s in read_names]) if read_names is not None else None
+    q = np.ascontiguousarray(np.frombuffer(quals, np.uint8) if isinstance(quals, (bytes, bytearray)) else quals, np.uint8) if quals is not None else None
+    tin = SamTextIn(C.cast(C.byref(res), C.c_void_p), C.cast(C.byref(rb), C.c_void_p), C.cast(rn, C.c_void_p) if rn is not None else None,
+                    q.ctypes.data if q is not None else None, C.cast(cn, C.c_void_p))
+    keep = []
+    if name_spans is not None:
+        b1, b2, nbeg, nlen = name_spans
+        nbeg = np.ascontiguousarray(nbeg, np.int64); nlen = np.ascontiguousarray(nlen, np.int32); keep += [nbeg, nlen]
+        tin.name_buf[0] = b1; tin.name_buf[1] = b2
+        tin.name_beg = nbeg.ctypes.data; tin.name_len = nlen.ctypes.data
+    x = SamTextExtra(rg_id.encode() if isinstance(rg_id, str) else rg_id, None, None, None, int(bool(ref_hdr)))
+    if comments is not None:
+        cb = np.ascontiguousarray(comments[0], np.int64); cl = np.ascontiguousarray(comments[1], np.int32); keep += [cb, cl]
+        x.comment_beg = cb.ctypes.data; x.comment_len = cl.ctypes.data
+    if contig_anno is not None:
+        ca = (C.c_char_p * len(contig_anno))(*[s.encode() if isinstance(s, str) else bytes(s) for s in contig_anno]); keep.append(ca)
+        x.contig_anno = C.cast(ca, C.c_void_p)
+    if qual_present is not None:
+        qp = np.ascontiguousarray(qual_present, np.uint8); keep.append(qp)
+        x.qual_present = qp.ctypes.data
+    buf = C.c_void_p(); n = C.c_int64(); ro = C.c_void_p()
+    f = lib().bm2_bam_format_ex
+    f.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+    rc = f(C.byref(tin), C.byref(x), int(n_threads), C.byref(buf), C.byref(n), C.byref(ro))
+    if rc:
+        raise Bm2Error(f"bm2_bam_format failed ({rc}): " + (lib().bm2_last_error(None) or b"").decode(errors="replace"))
+    out = C.string_at(buf, n.value)
+    off = _host(ro, rb.n_reads + 1, np.int64)
+    lib().bm2_free.argtypes = [C.c_void_p]
+    lib().bm2_free(buf); lib().bm2_free(ro)
+    return out, off
+
+
 class ReadBatch(C.Structure):
     _fields_ = [("n_reads", C.c_int32), ("codes", C.c_void_p), ("offsets", C.c_void_p)]
 
@@ -160,7 +203,7 @@ class RegResult(C.Structure):
 EXPORTS = ["bm2_create_sibling", "bm2_fastq_encode", "bm2_seq_encode", "bm2_fastq_comments", "bm2_fastq_smart_pair", "bm2_sam_format", "bm2_sam_format_ex", "bm2_free", "bm2_create_resident", "bm2_gather_probe", "bm2_set_sam_staged", "bm2_last_sam_stats", "bm2_gather64_gbs", "bm2_set_sub_batches", "bm2_seed_chain_extend_resident", "bm2_last_counters", "bm2_set_stream", "bm2_int_pipe_gops", "bm2_abi_version", "bm2_opt_init", "bm2_index_load", "bm2_index_free", "bm2_create", "bm2_destroy",
            "bm2_last_error", "bm2_extend_pairs", "bm2_extend_pairs_device", "bm2_collect_smems", "bm2_seed_chain",
            "bm2_seed_chain_extend", "bm2_last_stage_ms", "bm2_gen_cigar", "bm2_pestat", "bm2_sam_pe", "bm2_sam_se", "bm2_ksw_align2",
-           "bm2_fasta_pack", "bm2_index_build"]
+           "bm2_fasta_pack", "bm2_index_build", "bm2_bam_format_ex", "bm2_bgzf_compress", "bm2_last_bgzf_stats"]
 
 _lib = None
 
@@ -459,6 +502,20 @@ class Context:
                             comment_beg=_host(sp.comment_beg[s], n, np.int64), comment_len=_host(sp.comment_len[s], n, np.int32),
                             read_index=_host(sp.read_index[s], n, np.int32), d_codes=b.d_codes, d_offsets=b.d_offsets))
         return out
+
+    def bgzf_compress(self, data: bytes, cut=None):
+        """bm2_bgzf_compress: BGZF members of data (bytes) on this context's GPU, blocks cut at the record starts cut (int64[], ascending; None:
+        one record) by htslib's rule -> (members bytes, device ms, member count).  No EOF block."""
+        cut = np.ascontiguousarray(cut if cut is not None else np.zeros(0), np.int64)
+        buf = np.frombuffer(data, np.uint8) if len(data) else np.zeros(1, np.uint8)
+        out = C.c_void_p(); n = C.c_int64()
+        f = lib().bm2_bgzf_compress
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+        self._check(f(self._ctx, buf.ctypes.data, len(data), cut.ctypes.data, len(cut), C.byref(out), C.byref(n)), "bm2_bgzf_compress")
+        ms = C.c_double(); m = C.c_int64()
+        lib().bm2_last_bgzf_stats.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        lib().bm2_last_bgzf_stats(self._ctx, C.byref(ms), C.byref(m))
+        return (C.string_at(out, n.value) if n.value else b""), ms.value, m.value
 
     def set_sam_staged(self, on: int):
         """bm2_set_sam_staged: 1 / 2 = the rescue's local alignments as a batch (one window per warp / per thread) before the per-pair kernel, 0 = inside it."""

@@ -58,13 +58,20 @@ struct bm2_ctx {
     cudaEvent_t sam_ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
     double sam_ms[4] = {0, 0, 0, 0};
     unsigned long long sam_counts[6] = {0, 0, 0, 0, 0, 0};        // staged, jobs, looked up, computed in place, of those: window moved, waves
+    // bm2_bgzf_compress (bgzf.cu): buffers, events around its two kernels, the last call's device time and member count
+    DevBuf bgzf_d[7];
+    HostBuf bgzf_h[2];
+    cudaEvent_t bgzf_ev[4] = {nullptr, nullptr, nullptr, nullptr};
+    double bgzf_ms = 0;
+    int64_t bgzf_members = 0;
 
     int ensure(DevBuf &b, size_t bytes);
     int ensure_host(HostBuf &b, size_t bytes);
     std::vector<DevBuf *> all_dev() {
         std::vector<DevBuf *> v = {&io_pairs, &io_ref, &io_qer, &bsw_jobs, &bsw_outs, &bsw_scratch};
         for (auto &x : d) v.push_back(&x);
+        for (auto &x : bgzf_d) v.push_back(&x);
         return v;
     }
-    std::vector<HostBuf *> all_host() { std::vector<HostBuf *> v; for (auto &x : h) v.push_back(&x); return v; }
+    std::vector<HostBuf *> all_host() { std::vector<HostBuf *> v; for (auto &x : h) v.push_back(&x); for (auto &x : bgzf_h) v.push_back(&x); return v; }
 };

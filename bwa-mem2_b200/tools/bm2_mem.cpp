@@ -1,4 +1,4 @@
-// bm2_mem — FASTQ in, SAM out, on the GPU path: the host side of `bwa-mem2 mem` for the seams of libbm2b200.so (C++, as the reference's host
+// bm2_mem — FASTQ in, SAM or BAM out, on the GPU path: the host side of `bwa-mem2 mem` for the seams of libbm2b200.so (C++, as the reference's host
 // code; only the C ABI of include/bm2_b200.h is used).
 //
 //   bm2_mem [options] <index prefix> <reads_1.fq> [reads_2.fq]
@@ -19,6 +19,7 @@
 //   bm2_pestat                    mem_pestat, or the -I values                                        (src/bwamem.cpp:1368-1378)
 //   bm2_sam_pe / bm2_sam_se       worker_sam's arithmetic                                             (src/bwamem.cpp:1262-1336)
 //   bm2_sam_format_ex             mem_aln2sam's text with RG / the -C comment / XR                    (src/bwamem.cpp:1592-1730)
+//     or bm2_bam_format_ex        --bam: the same records as BAM, then bm2_bgzf_compress: BGZF members compressed on the GPU
 // Chunks in flight: the reference's kt_pipeline runs its three steps (read, process, write) on two worker threads so that one chunk's I/O
 // overlaps another's computation (src/fastmap.cpp:952-1003, src/kthread.cpp:122-176).  Here -p workers (default 2) each own a context
 // (bm2_create_sibling: one index in HBM) and take whole chunks off a queue; the GPU interleaves the kernels of the two chunks, the host side of
@@ -60,6 +61,7 @@ struct Shared {
     std::deque<Chunk> queue; bool done = false;
     long long next_to_write = 0;
     double t_loop = 0;
+    double t_bam = 0, t_bgzf = 0; long long bam_bytes = 0, bgzf_bytes = 0;       // --bam: encoding (host), compression (device), sizes
     double t_enc = 0, t_aln = 0, t_pes = 0, t_sam = 0, t_fmt = 0, t_write = 0, t_turn = 0;
     std::vector<double> chunk_s, chunk_done_s; std::vector<long long> chunk_reads;
     long long n_processed = 0;
@@ -68,7 +70,7 @@ struct Shared {
     bool paired = false, smart = false; int threads = 1; FILE *out = nullptr;
     const bm2_pestat_t *pes0 = nullptr;                          // -I: used instead of bm2_pestat
     bm2_sam_text_extra extra{};                                  // -R / -C / -V
-    bool copy_comment = false;
+    bool copy_comment = false, bam = false;
     double t_split = 0;
     long long seq_chunks = 0;                                    // chunks that went through bm2_seq_encode
     size_t in_flight = 0;                                        // bytes of the chunks queued or being aligned
@@ -76,12 +78,12 @@ struct Shared {
 
 [[noreturn]] void die(const char *what, const bm2_ctx *ctx) { fprintf(stderr, "bm2_mem: %s%s%s\n", what, ctx ? ": " : "", ctx ? bm2_last_error(ctx) : ""); fflush(stderr); _Exit(3); }
 
-struct Times { double aln = 0, pes = 0, sam = 0, fmt = 0; };
+struct Times { double aln = 0, pes = 0, sam = 0, fmt = 0, bam = 0; };
 
-// one batch through seams 2, 4 and 5: its SAM text (malloc'd) and, when lines != nullptr, the number of lines of every read
-// qual_present: NULL, or 0 for the reads without qualities (QUAL '*')
+// one batch through seams 2, 4 and 5: its SAM text or, with --bam, its BAM records (malloc'd) and, when read_end != nullptr, where the output
+// of every read ends; qual_present: NULL, or 0 for the reads without qualities (QUAL '*')
 char *align_and_format(Shared *sh, bm2_ctx *ctx, const bm2_fastq_batch &fq, const char *buf0, const char *buf1, const int64_t *cmt_beg,
-                       const int32_t *cmt_len, const uint8_t *qual_present, bool paired, long long id_base, int64_t *len, std::vector<int> *lines, Times &t) {
+                       const int32_t *cmt_len, const uint8_t *qual_present, bool paired, long long id_base, int64_t *len, std::vector<int64_t> *read_end, Times &t) {
     const double t1 = now_s();
     bm2_read_batch rb = { fq.n_reads, fq.codes, fq.offsets };
     bm2_reg_result rr;
@@ -103,23 +105,34 @@ char *align_and_format(Shared *sh, bm2_ctx *ctx, const bm2_fastq_batch &fq, cons
     bm2_sam_text_extra x = sh->extra;
     x.comment_beg = cmt_beg; x.comment_len = cmt_len; x.qual_present = qual_present;
     char *text = nullptr;
-    if (bm2_sam_format_ex(&tin, &x, sh->threads, &text, len)) die("bm2_sam_format_ex failed", nullptr);
-    if (lines) {
-        lines->assign((size_t) fq.n_reads, 0);
-        for (int64_t k = 0; k < sr.n_recs; ++k) ++(*lines)[(size_t) sr.recs[k].read];
+    if (sh->bam) {
+        int64_t *ro = nullptr;
+        if (bm2_bam_format_ex(&tin, &x, sh->threads, &text, len, &ro)) { fprintf(stderr, "[E::bm2_mem] %s\n", bm2_last_error(nullptr)); fflush(stderr); _Exit(1); }
+        if (read_end) read_end->assign(ro + 1, ro + fq.n_reads + 1);
+        bm2_free(ro);
+        t.bam += now_s() - t4;
+    } else {
+        if (bm2_sam_format_ex(&tin, &x, sh->threads, &text, len)) die("bm2_sam_format_ex failed", nullptr);
+        if (read_end) {                                                  // lines per read, then where they end
+            read_end->assign((size_t) fq.n_reads, 0);
+            for (int64_t k = 0; k < sr.n_recs; ++k) ++(*read_end)[(size_t) sr.recs[k].read];
+            const char *q = text;
+            for (int64_t &e : *read_end) { for (int64_t k = e; k > 0; --k) q = (const char *) memchr(q, '\n', (size_t) (text + *len - q)) + 1; e = q - text; }
+        }
+        t.fmt += now_s() - t4;
     }
-    t.aln += t2 - t1; t.pes += t3 - t2; t.sam += t4 - t3; t.fmt += now_s() - t4;
+    t.aln += t2 - t1; t.pes += t3 - t2; t.sam += t4 - t3;
     return text;
 }
 
 // -p: the single-end set and the pairs of a chunk as the reference's two mem_process_seqs calls (src/fastmap.cpp:260-285), the reads' lines
-// merged back into file order (the records of a read are consecutive)
+// (or BAM records) merged back into file order (the records of a read are consecutive)
 char *smart_pair_chunk(Shared *sh, bm2_ctx *ctx, const Chunk &ck, int n_reads, const uint8_t *qual_present, int64_t *len, Times &t) {
     const double t0 = now_s();
     bm2_fastq_split sp;
     if (bm2_fastq_smart_pair(ctx, &sp)) die("bm2_fastq_smart_pair", ctx);
     const double t_split = now_s() - t0;
-    char *text[2] = { nullptr, nullptr }; int64_t tl[2] = { 0, 0 }; std::vector<int> lines[2];
+    char *text[2] = { nullptr, nullptr }; int64_t tl[2] = { 0, 0 }; std::vector<int64_t> ends[2];
     const long long base[2] = { ck.first_read, (ck.first_read + sp.set[0].n_reads) >> 1 };
     std::vector<uint8_t> qp[2];
     for (int s = 0; s < 2 && qual_present; ++s)
@@ -128,7 +141,7 @@ char *smart_pair_chunk(Shared *sh, bm2_ctx *ctx, const Chunk &ck, int n_reads, c
         if (sp.set[s].n_reads)
             text[s] = align_and_format(sh, ctx, sp.set[s], ck.c1, nullptr, sh->copy_comment ? sp.comment_beg[s] : nullptr,
                                        sh->copy_comment ? sp.comment_len[s] : nullptr, qual_present ? qp[s].data() : nullptr, s == 1, base[s],
-                                       &tl[s], &lines[s], t);
+                                       &tl[s], &ends[s], t);
     std::vector<int8_t> set_of((size_t) n_reads, -1);
     for (int s = 0; s < 2; ++s) for (int j = 0; j < sp.set[s].n_reads; ++j) set_of[(size_t) sp.read_index[s][j]] = (int8_t) s;
     char *merged = (char *) malloc((size_t) (tl[0] + tl[1]) + 1);
@@ -137,8 +150,7 @@ char *smart_pair_chunk(Shared *sh, bm2_ctx *ctx, const Chunk &ck, int n_reads, c
     for (int i = 0; i < n_reads; ++i) {
         const int s = set_of[(size_t) i];
         if (s < 0) die("bm2_fastq_smart_pair: a read in neither set", nullptr);
-        const char *q = p[s];
-        for (int k = lines[s][(size_t) next[s]++]; k > 0; --k) q = (const char *) memchr(q, '\n', (size_t) (text[s] + tl[s] - q)) + 1;
+        const char *q = text[s] + ends[s][(size_t) next[s]++];
         memcpy(w, p[s], (size_t) (q - p[s])); w += q - p[s]; p[s] = q;
     }
     *w = 0; *len = w - merged;
@@ -174,18 +186,28 @@ void worker(Shared *sh, bm2_ctx *ctx) {
             text = align_and_format(sh, ctx, fq, ck.c1, sh->paired ? ck.c2 : nullptr, cb, cl, qp, sh->paired,
                                     sh->paired ? ck.first_read >> 1 : ck.first_read, &len, nullptr, t);
         }
+        const uint8_t *outp = (const uint8_t *) text; int64_t out_len = len;
+        double bgzf_ms = 0;
+        if (sh->bam) {                                                   // BGZF blocks cut at the records' starts, within the chunk
+            std::vector<int64_t> cut;
+            for (int64_t q = 0; q + 4 <= len; q += 4 + *(const int32_t *) (text + q)) cut.push_back(q);
+            if (bm2_bgzf_compress(ctx, (const uint8_t *) text, len, cut.data(), (int64_t) cut.size(), &outp, &out_len)) die("bm2_bgzf_compress", ctx);
+            int64_t members = 0;
+            bm2_last_bgzf_stats(ctx, &bgzf_ms, &members);
+        }
         const double t5 = now_s();
         {   // the output keeps the chunk order
             std::unique_lock<std::mutex> lk(sh->mu);
             sh->cv_turn.wait(lk, [&] { return sh->next_to_write == ck.index; });
         }
         const double t6 = now_s();
-        fwrite(text, 1, (size_t) len, sh->out);
+        fwrite(outp, 1, (size_t) out_len, sh->out);
         bm2_free(text);
         const double t7 = now_s();
         {
             std::lock_guard<std::mutex> lk(sh->mu);
             sh->t_enc += t1 - t0; sh->t_aln += t.aln; sh->t_pes += t.pes; sh->t_sam += t.sam; sh->t_fmt += t.fmt; sh->t_turn += t6 - t5; sh->t_write += t7 - t6;
+            sh->t_bam += t.bam; sh->t_bgzf += bgzf_ms / 1e3; sh->bam_bytes += sh->bam ? len : 0; sh->bgzf_bytes += sh->bam ? out_len : 0;
             sh->n_processed += fq.n_reads; sh->seq_chunks += !ck.simple; sh->in_flight -= ck.bytes.size();
             sh->chunk_s.push_back(t7 - t0); sh->chunk_done_s.push_back(t7 - sh->t_loop); sh->chunk_reads.push_back(fq.n_reads);
             ++sh->next_to_write;
@@ -252,6 +274,7 @@ void usage(const bm2_mem_opt_t &o) {
 "  -p INT      chunks in flight, one GPU context each (1-4) [2].  A -p given as a separate argument and followed by a positive decimal\n"
 "              integer is this count; any other -p (alone, or in a cluster like -5SP) is smart pairing.  An index prefix that is a bare\n"
 "              integer must then be written as a path (./2) after a smart-pairing -p.\n"
+"  --bam       write BAM (BGZF-compressed on the GPU) instead of SAM; the same records, header and @PG line\n"
 "  --dump-opt  print the parsed options, the -I values, the read group and the header as JSON, and exit before any GPU work\n"
 "  --dump-chunks  print the chunks the input is cut into (first read, byte ranges, whether bm2_fastq_encode takes them) as JSON lines,\n"
 "              and exit without loading the index\n",
@@ -307,14 +330,15 @@ bool is_count(const char *s) {
 
 int main(int argc, char **argv) {
     static const char *const optstring = "51qpaMCSPVYjk:c:v:s:r:t:R:A:B:O:E:U:w:L:d:T:Q:D:m:I:N:W:x:G:h:y:K:X:H:o:f:";
-    // this program's own arguments first: `-p N` (worker count) and --dump-opt are taken out of the list, walking it the way getopt will
+    // this program's own arguments first: `-p N` (worker count), --bam and --dump-opt are taken out of the list, walking it the way getopt will
     // (option arguments skipped, `--` ends the options), so that everything left is parsed as main_mem parses it
-    int workers = 2; bool dump = false, dump_chunks = false;
+    int workers = 2; bool dump = false, dump_chunks = false, bam = false;
     std::vector<char *> av = { argv[0] };
     for (int i = 1; i < argc; ++i) {
         char *s = argv[i];
         if (!strcmp(s, "--")) { for (; i < argc; ++i) av.push_back(argv[i]); break; }
         if (!strcmp(s, "--dump-opt")) { dump = true; continue; }
+        if (!strcmp(s, "--bam")) { bam = true; continue; }
         if (!strcmp(s, "--dump-chunks")) { dump_chunks = true; continue; }
         if (!strcmp(s, "-p") && i + 1 < argc && is_count(argv[i + 1])) { workers = atoi(argv[++i]); continue; }
         av.push_back(s);
@@ -521,12 +545,15 @@ int main(int argc, char **argv) {
         printf("], \"pes\": ");
         if (use_pes) printf("{\"low\": %d, \"high\": %d, \"avg\": %.17g, \"std\": %.17g}", pes[1].low, pes[1].high, pes[1].avg, pes[1].std);
         else printf("null");
-        printf(", \"rg_id\": %s, \"copy_comment\": %s, \"ignore_alt\": %s, \"smart_pairing\": %s, \"workers\": %d, \"files\": %d, \"header\": %s}\n",
+        printf(", \"rg_id\": %s, \"copy_comment\": %s, \"ignore_alt\": %s, \"smart_pairing\": %s, \"workers\": %d, \"files\": %d, \"bam\": %s, \"header\": %s}\n",
                have_rg ? json_str(rg_id).c_str() : "null", copy_comment ? "true" : "false", ignore_alt ? "true" : "false", smart ? "true" : "false",
-               workers, f2 ? 2 : 1, json_str(header).c_str());
+               workers, f2 ? 2 : 1, bam ? "true" : "false", json_str(header).c_str());
         bm2_index_free(idx);
         return 0;
     }
+    if (bam)                                                          // BAM stores l_ref as int32 (SAMv1 §4.2)
+        for (size_t i = 0; i < names.size(); ++i)
+            if (lens[i] > INT32_MAX) { fprintf(stderr, "[E::bm2_mem] contig %s is %lld bp long: BAM cannot store a contig longer than 2^31-1\n", names[i].c_str(), lens[i]); return 1; }
     std::vector<const char *> cnames, canno;
     for (size_t i = 0; i < names.size(); ++i) { cnames.push_back(names[i].c_str()); canno.push_back(annos[i].c_str()); }
     std::vector<bm2_ctx *> ctxs((size_t) workers, nullptr);
@@ -538,13 +565,23 @@ int main(int argc, char **argv) {
     if (!in.open(f1, f2)) return 2;
     FILE *out = out_path ? fopen(out_path, "wb") : stdout;
     if (!out) { fprintf(stderr, "bm2_mem: cannot open %s\n", out_path); return 2; }
-    fwrite(header.data(), 1, header.size(), out);
-    fprintf(out, "@PG\tID:bm2_mem\tPN:bm2_mem\tVN:b200-r2\tCL:%s", argv[0]);
-    for (int i = 1; i < argc; ++i) fprintf(out, " %s", argv[i]);
-    fprintf(out, "\n");
+    header += std::string("@PG\tID:bm2_mem\tPN:bm2_mem\tVN:b200-r2\tCL:") + argv[0];
+    for (int i = 1; i < argc; ++i) header += std::string(" ") + argv[i];
+    header += "\n";
+    if (!bam) fwrite(header.data(), 1, header.size(), out);
+    else {   // SAMv1 §4.2: magic, the header text, then the index's contigs (refIDs index this list, whatever -H put in the text), in blocks of its own
+        std::string h("BAM\1", 4);
+        auto i32 = [&](int32_t v) { h.append((const char *) &v, 4); };
+        i32((int32_t) header.size()); h += header;
+        i32((int32_t) names.size());
+        for (size_t i = 0; i < names.size(); ++i) { i32((int32_t) names[i].size() + 1); h.append(names[i].c_str(), names[i].size() + 1); i32((int32_t) lens[i]); }
+        const uint8_t *z = nullptr; int64_t zl = 0;
+        if (bm2_bgzf_compress(ctxs[0], (const uint8_t *) h.data(), (int64_t) h.size(), nullptr, 0, &z, &zl)) die("bm2_bgzf_compress", ctxs[0]);
+        fwrite(z, 1, (size_t) zl, out);
+    }
     Shared sh;
     sh.opt = &opt; sh.idx = idx; sh.cnames = cnames.data(); sh.paired = f2 != nullptr; sh.smart = smart; sh.threads = threads; sh.out = out;
-    sh.pes0 = use_pes ? pes : nullptr; sh.copy_comment = copy_comment;
+    sh.pes0 = use_pes ? pes : nullptr; sh.copy_comment = copy_comment; sh.bam = bam;
     sh.extra.rg_id = have_rg ? rg_id.c_str() : nullptr; sh.extra.contig_anno = canno.data(); sh.extra.ref_hdr = (opt.flag & 0x100) != 0;
     sh.t_loop = now_s();
     std::vector<std::thread> pool;
@@ -562,6 +599,10 @@ int main(int argc, char **argv) {
     sh.cv_work.notify_all();
     for (auto &t : pool) t.join();
     const double loop_s = now_s() - sh.t_loop;
+    if (bam) {                                                        // the BGZF end-of-file marker (SAMv1 §4.1.2)
+        static const uint8_t eof[28] = { 0x1f, 0x8b, 8, 4, 0, 0, 0, 0, 0, 0xff, 6, 0, 0x42, 0x43, 2, 0, 0x1b, 0, 3, 0, 0, 0, 0, 0, 0, 0, 0, 0 };
+        fwrite(eof, 1, sizeof eof, out);
+    }
     if (out != stdout) fclose(out);
     fprintf(stderr, "{\"reads\": %lld, \"chunks\": %lld, \"workers\": %d, \"loop_s\": %.6f, \"index_and_context_s\": %.3f, \"fastq_encode_s\": %.6f, \"seed_chain_extend_s\": %.6f, "
                     "\"pestat_s\": %.6f, \"sam_stage_s\": %.6f, \"sam_format_s\": %.6f, \"wait_for_turn_s\": %.6f, \"write_s\": %.6f, \"chunk_s\": [",
@@ -571,8 +612,10 @@ int main(int argc, char **argv) {
     for (size_t i = 0; i < sh.chunk_done_s.size(); ++i) fprintf(stderr, "%s%.6f", i ? ", " : "", sh.chunk_done_s[i]);
     fprintf(stderr, "], \"chunk_reads\": [");
     for (size_t i = 0; i < sh.chunk_reads.size(); ++i) fprintf(stderr, "%s%lld", i ? ", " : "", sh.chunk_reads[i]);
-    fprintf(stderr, "], \"smart_pair_split_s\": %.6f, \"seq_encode_chunks\": %lld, \"read_s\": %.6f, \"gzip_members\": %lld, \"input_peak_bytes\": %zu}\n",
+    fprintf(stderr, "], \"smart_pair_split_s\": %.6f, \"seq_encode_chunks\": %lld, \"read_s\": %.6f, \"gzip_members\": %lld, \"input_peak_bytes\": %zu",
             sh.t_split, sh.seq_chunks, read_s, (long long) (in.s[0].gzip_members + in.s[1].gzip_members), input_peak);
+    if (bam) fprintf(stderr, ", \"bam_format_s\": %.6f, \"bgzf_s\": %.6f, \"bam_bytes\": %lld, \"bgzf_bytes\": %lld", sh.t_bam, sh.t_bgzf, sh.bam_bytes, sh.bgzf_bytes);
+    fprintf(stderr, "}\n");
     for (int w = workers - 1; w >= 0; --w) bm2_destroy(ctxs[w]);
     bm2_index_free(idx);
     return 0;

@@ -399,7 +399,27 @@ typedef struct bm2_sam_text_extra {
 } bm2_sam_text_extra;
 /* bm2_sam_format with the additions; x == NULL is bm2_sam_format. */
 int  bm2_sam_format_ex(const bm2_sam_text_in *in, const bm2_sam_text_extra *x, int n_threads, char **text, int64_t *len);
+/* The binary twin of bm2_sam_format_ex: the same records, fields and tags in the same order, as uncompressed BAM records (SAMv1 §4.2), each
+ * what `samtools view -b` makes of the SAM line: SEQ in 4-bit codes, QUAL minus 33 (0xFF x l_seq without qualities; l_seq 0 on a true
+ * secondary), 0-based pos / next_pos (-1 where the column is 0), bin = reg2bin of the CIGAR's reference span (4680 unplaced), integer tags in
+ * the smallest type that holds them (c / s / i when negative, else C / S / I), pa as the float of its %.3f text, MD MC SA XA RG XR as Z.  More
+ * than 65535 CIGAR operations: the placeholder <l_seq>S<ref_len>N and the operations in a CG:B,I tag after the others.  With a comment (-C) the
+ * comment must be tab-separated TG:T:VALUE fields (types A c C s S i I f Z H B), stored typed as sam_parse1 stores them.
+ * *bam: malloc'd (bm2_free), *len bytes; *read_off: malloc'd (bm2_free), n_reads + 1 offsets, where each read's records start.
+ * Errors: a QNAME longer than 254 bytes, or a comment that does not parse, returns 4 with a message naming the read (bm2_last_error(NULL)). */
+int  bm2_bam_format_ex(const bm2_sam_text_in *in, const bm2_sam_text_extra *x, int n_threads, char **bam, int64_t *len, int64_t **read_off);
 void bm2_free(void *p);
+
+/* ---- BGZF compression on the GPU (SAMv1 §4.1) -------------------------------------------------------------------------------------
+ * in: n uncompressed bytes (HOST); cut: the n_cut ascending offsets where records start (bytes before cut[0] are a record of their own; NULL
+ * with n_cut == 0: one record).  Blocks are cut as htslib's writer cuts them: at most 65280 bytes, a record that would overflow a non-empty
+ * block starts the next one, a record larger than a block spans blocks.  Each block becomes one BGZF member of at most 65536 bytes: gzip header
+ * with the BC subfield, raw DEFLATE (one dynamic Huffman block, or a stored block when that is not smaller), CRC32, ISIZE - compressed on the
+ * context's device and stream, one block per CTA; the bytes depend on each block's input alone.  No EOF block is added.  *out: HOST, owned by the
+ * context, valid until its next bm2_bgzf_compress call; *out_len bytes (0 for n == 0). */
+int  bm2_bgzf_compress(bm2_ctx *ctx, const uint8_t *in, int64_t n, const int64_t *cut, int64_t n_cut, const uint8_t **out, int64_t *out_len);
+/* The last bm2_bgzf_compress call: device time of its kernels (CUDA events, ms) and its member count. */
+int  bm2_last_bgzf_stats(const bm2_ctx *ctx, double *device_ms, int64_t *members);
 
 /* Staged mate rescue inside bm2_sam_pe (same records, other kernels): the windows mem_matesw (src/bwamem_pair.cpp:150-283) can ask for are
  * listed for all pairs of a wave from the regions before any rescue, aligned as one batch with one window per warp (the job shape of
