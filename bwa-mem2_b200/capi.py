@@ -200,10 +200,20 @@ class RegResult(C.Structure):
     _fields_ = [("n", C.c_int64), ("regs", C.c_void_p), ("read_off", C.c_void_p)]
 
 
+# bm2_bam_sort_compress: per record in output order (include/bm2_b200.h)
+SORT_REC_DT = np.dtype([("rid", "<i4"), ("pos", "<i4"), ("end", "<i4"), ("bin", "<u2"), ("flag", "<u2"), ("block", "<i8"), ("offset", "<i4"), ("_pad", "<i4")])
+
+
+class SortOut(C.Structure):
+    _fields_ = [("z", C.c_void_p), ("z_len", C.c_int64), ("member_size", C.c_void_p), ("n_members", C.c_int64), ("carry", C.c_void_p),
+                ("carry_len", C.c_int64), ("recs", C.c_void_p), ("n_recs", C.c_int64)]
+
+
 EXPORTS = ["bm2_create_sibling", "bm2_fastq_encode", "bm2_seq_encode", "bm2_fastq_comments", "bm2_fastq_smart_pair", "bm2_sam_format", "bm2_sam_format_ex", "bm2_free", "bm2_create_resident", "bm2_gather_probe", "bm2_set_sam_staged", "bm2_last_sam_stats", "bm2_gather64_gbs", "bm2_set_sub_batches", "bm2_seed_chain_extend_resident", "bm2_last_counters", "bm2_set_stream", "bm2_int_pipe_gops", "bm2_abi_version", "bm2_opt_init", "bm2_index_load", "bm2_index_free", "bm2_create", "bm2_destroy",
            "bm2_last_error", "bm2_extend_pairs", "bm2_extend_pairs_device", "bm2_collect_smems", "bm2_seed_chain",
            "bm2_seed_chain_extend", "bm2_last_stage_ms", "bm2_gen_cigar", "bm2_pestat", "bm2_sam_pe", "bm2_sam_se", "bm2_ksw_align2",
-           "bm2_fasta_pack", "bm2_index_build", "bm2_bam_format_ex", "bm2_bgzf_compress", "bm2_last_bgzf_stats"]
+           "bm2_fasta_pack", "bm2_index_build", "bm2_bam_format_ex", "bm2_bgzf_compress", "bm2_last_bgzf_stats",
+           "bm2_bam_sort_compress", "bm2_last_sort_stats", "bm2_bam_sort_memory"]
 
 _lib = None
 
@@ -516,6 +526,27 @@ class Context:
         lib().bm2_last_bgzf_stats.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         lib().bm2_last_bgzf_stats(self._ctx, C.byref(ms), C.byref(m))
         return (C.string_at(out, n.value) if n.value else b""), ms.value, m.value
+
+    def bam_sort_compress(self, data: bytes, starts, carry: bytes = b"", last: bool = True):
+        """bm2_bam_sort_compress: the records of data (uncompressed BAM) starting at starts, stably sorted by the coordinate key and compressed
+        after carry -> dict(z: whole members, member_size, carry: the unfinished block's bytes, recs: SORT_REC_DT in output order,
+        ms: device ms of keys, sort, gather, BGZF)."""
+        starts = np.ascontiguousarray(starts, np.int64)
+        buf = np.frombuffer(data, np.uint8) if len(data) else np.zeros(1, np.uint8)
+        cb = np.frombuffer(carry, np.uint8) if len(carry) else np.zeros(1, np.uint8)
+        o = SortOut()
+        f = lib().bm2_bam_sort_compress
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int, C.c_void_p]
+        self._check(f(self._ctx, buf.ctypes.data, len(data), starts.ctypes.data, len(starts), cb.ctypes.data, len(carry), int(last), C.byref(o)),
+                    "bm2_bam_sort_compress")
+        ms = (C.c_double * 4)()
+        lib().bm2_last_sort_stats.argtypes = [C.c_void_p, C.c_void_p]
+        lib().bm2_last_sort_stats(self._ctx, ms)
+        recs = np.ctypeslib.as_array(C.cast(o.recs, C.POINTER(C.c_uint8)), shape=(o.n_recs * SORT_REC_DT.itemsize,)).view(SORT_REC_DT).copy() \
+            if o.n_recs else np.zeros(0, SORT_REC_DT)
+        sizes = _host(o.member_size, o.n_members, np.int32) if o.n_members else np.zeros(0, np.int32)
+        return dict(z=C.string_at(o.z, o.z_len) if o.z_len else b"", member_size=sizes, carry=C.string_at(o.carry, o.carry_len) if o.carry_len else b"",
+                    recs=recs, ms=dict(keys=ms[0], sort=ms[1], gather=ms[2], bgzf=ms[3]))
 
     def set_sam_staged(self, on: int):
         """bm2_set_sam_staged: 1 / 2 = the rescue's local alignments as a batch (one window per warp / per thread) before the per-pair kernel, 0 = inside it."""

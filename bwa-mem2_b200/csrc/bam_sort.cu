@@ -1,0 +1,211 @@
+// bam_sort.cu — coordinate sort of BAM records on the GPU, compressed as they leave (bm2_bam_sort_compress): one buffer of records (a
+// sorted run of bm2_mem --sort, or a merge window) in, BGZF members of carry + the sorted records out, with every record's index data.
+//   upload      the records and their starts (host)
+//   keys        one thread per record: its fixed fields, end and bin (bam_sort_device.cuh), its length, and the largest refID and pos + 1
+//   pack        the coordinate key squeezed into the bits the refIDs and positions use (refID -1 ranked after the largest refID), the
+//               ordinal as the value; then cub::DeviceRadixSort::SortPairs over those bits only: LSD radix sort is stable, so ties keep
+//               input order
+//   scan        the lengths in sorted order, an exclusive scan: each record's place after the carry
+//   gather      one warp per record, 16-byte copies when source and destination agree modulo 16
+//   BGZF        the blocks are cut on the host (bam_sort_layout) from the scan, and bm2_bgzf_compress's kernels compress them straight from the
+//               sorted device buffer; the unfinished last block goes back as the carry
+#include "bm2_common.cuh"
+#include "bm2_ctx.h"
+#include "bam_sort_device.cuh"
+#include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
+#include <vector>
+
+namespace {
+
+constexpr int kRecBytes = 300;      // a short read's record, for bm2_bam_sort_memory's estimate
+
+__global__ void sort_key_kernel(const uint8_t *__restrict__ in, const int64_t *__restrict__ starts, int64_t n, bm2_sort_rec *info,
+                                int64_t *len, unsigned *maxes) {
+    const int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
+    unsigned mr = 0, mp = 0;
+    if (i < n) {
+        const uint8_t *r = in + starts[i];
+        const bm2_sort_rec s = bam_sort_rec(r);
+        info[i] = s;
+        len[i] = 4 + (int64_t) bam_le32(r);
+        mr = s.rid >= 0 ? (unsigned) s.rid + 1 : 0;
+        mp = (unsigned) (s.pos + 1);
+    }
+    for (int o = 16; o; o >>= 1) { mr = max(mr, __shfl_xor_sync(0xFFFFFFFFu, mr, o)); mp = max(mp, __shfl_xor_sync(0xFFFFFFFFu, mp, o)); }
+    if ((threadIdx.x & 31) == 0) { atomicMax(maxes, mr); atomicMax(maxes + 1, mp); }
+}
+
+// rank(refID) << (pos_bits + 1) | (pos + 1) << 1 | reverse: the order of samtools' key, in rank_bits + pos_bits + 1 bits
+__global__ void sort_pack_kernel(const bm2_sort_rec *__restrict__ info, int64_t n, unsigned unplaced_rank, int pos_bits, uint64_t *keys,
+                                 uint32_t *vals) {
+    const int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const bm2_sort_rec s = info[i];
+    const uint64_t rank = s.rid >= 0 ? (uint64_t) s.rid : unplaced_rank;
+    keys[i] = rank << (pos_bits + 1) | (uint64_t) (uint32_t) (s.pos + 1) << 1 | (uint64_t) ((s.flag & 16) ? 1 : 0);
+    vals[i] = (uint32_t) i;
+}
+
+__global__ void sort_permute_kernel(const uint32_t *__restrict__ ord, int64_t n, const int64_t *__restrict__ len, const bm2_sort_rec *__restrict__ info,
+                                    int64_t *len_sorted, bm2_sort_rec *info_sorted) {
+    const int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
+    if (i > n) return;
+    if (i == n) { len_sorted[n] = 0; return; }
+    const uint32_t k = ord[i];
+    len_sorted[i] = len[k]; info_sorted[i] = info[k];
+}
+
+// one warp per record: in + starts[ord[i]] -> out + base + offs[i]
+__global__ void sort_gather_kernel(const uint8_t *__restrict__ in, const int64_t *__restrict__ starts, const uint32_t *__restrict__ ord,
+                                   const int64_t *__restrict__ offs, const int64_t *__restrict__ len, int64_t n, int64_t base, uint8_t *out) {
+    const int64_t w = ((int64_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (w >= n) return;
+    const uint8_t *s = in + starts[ord[w]];
+    uint8_t *d = out + base + offs[w];
+    const int64_t m = len[w];
+    int64_t head = 0, body = 0;
+    if ((((uintptr_t) s ^ (uintptr_t) d) & 15) == 0) {
+        head = bm2_min<int64_t>(m, (16 - ((uintptr_t) d & 15)) & 15);
+        body = (m - head) & ~(int64_t) 15;
+    }
+    for (int64_t k = lane; k < head; k += 32) d[k] = s[k];
+    const uint4 *s4 = (const uint4 *) (s + head);
+    uint4 *d4 = (uint4 *) (d + head);
+    for (int64_t k = lane; k < body / 16; k += 32) d4[k] = s4[k];
+    for (int64_t k = head + body + lane; k < m; k += 32) d[k] = s[k];
+}
+
+enum { SD_IN, SD_STARTS, SD_INFO, SD_LEN, SD_KEYS0, SD_KEYS1, SD_VALS0, SD_VALS1, SD_LENS, SD_OFFS, SD_TEMP, SD_OUT, SD_SINFO, SD_MAX };
+static_assert(SD_MAX + 1 <= (int) (sizeof(((bm2_ctx *) nullptr)->sort_d) / sizeof(DevBuf)), "sort buffers");
+
+int bits_of(uint64_t v) { int b = 0; while (v >> b) ++b; return b; }
+
+}  // namespace
+
+extern "C" int bm2_bam_sort_compress(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int64_t *starts, int64_t n_recs, const uint8_t *carry,
+                                     int64_t carry_len, int last, bm2_sort_out *out) {
+    bm2_ctx *ctx_for_error = ctx;
+    if (!ctx || !out || n < 0 || (n && !recs) || n_recs < 0 || (n_recs && !starts) || carry_len < 0 || carry_len >= BGZF_BLOCK ||
+        (carry_len && !carry)) {
+        if (ctx) bm2_set_error(ctx, "bm2_bam_sort_compress: bad arguments");
+        return 1;
+    }
+    if (n_recs >= (1LL << 31) - 1) { bm2_set_error(ctx, "bm2_bam_sort_compress: 2^31-1 records or more in one call"); return 1; }
+    for (int64_t i = 0; i < n_recs; ++i) {                       // each record whole inside the buffer, in order, not overlapping the next
+        const int64_t s = starts[i];
+        if (s < 0 || s + 36 > n || (i && s < starts[i - 1] + 4 + (int64_t) bam_le32(recs + starts[i - 1]))) {
+            bm2_set_error(ctx, "bm2_bam_sort_compress: record " + std::to_string(i) + " does not lie within the buffer after the one before");
+            return 1;
+        }
+        const int64_t m = 4 + (int64_t) bam_le32(recs + s);
+        const int32_t rid = bam_le32(recs + s + 4);
+        if (m < 36 || s + m > n || rid < -1) { bm2_set_error(ctx, "bm2_bam_sort_compress: record " + std::to_string(i) + " is malformed"); return 1; }
+    }
+    memset(out, 0, sizeof *out);
+    for (double &x : ctx->sort_ms) x = 0;
+    BM2_CUDA_OK(cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->stream;
+    DevBuf *b = ctx->sort_d;
+    const int64_t nr = n_recs;
+    size_t temp = 0;
+    {
+        cub::DoubleBuffer<uint64_t> k((uint64_t *) nullptr, nullptr); cub::DoubleBuffer<uint32_t> v((uint32_t *) nullptr, nullptr);
+        BM2_CUDA_OK(cub::DeviceRadixSort::SortPairs(nullptr, temp, k, v, (int) bm2_max<int64_t>(nr, 1), 0, 64, st));
+        size_t t2 = 0;
+        BM2_CUDA_OK(cub::DeviceScan::ExclusiveSum(nullptr, t2, (int64_t *) nullptr, (int64_t *) nullptr, (int) nr + 1, st));
+        temp = bm2_max(temp, t2);
+    }
+    if (ctx->ensure(b[SD_IN], (size_t) n + 16) || ctx->ensure(b[SD_STARTS], (size_t) nr * 8 + 8) ||
+        ctx->ensure(b[SD_INFO], (size_t) nr * sizeof(bm2_sort_rec) + 8) || ctx->ensure(b[SD_LEN], (size_t) nr * 8 + 8) ||
+        ctx->ensure(b[SD_KEYS0], (size_t) nr * 8 + 8) || ctx->ensure(b[SD_KEYS1], (size_t) nr * 8 + 8) ||
+        ctx->ensure(b[SD_VALS0], (size_t) nr * 4 + 8) || ctx->ensure(b[SD_VALS1], (size_t) nr * 4 + 8) ||
+        ctx->ensure(b[SD_LENS], (size_t) nr * 8 + 8) || ctx->ensure(b[SD_OFFS], (size_t) nr * 8 + 8) || ctx->ensure(b[SD_TEMP], temp + 16) ||
+        ctx->ensure(b[SD_OUT], (size_t) (carry_len + n) + 16) || ctx->ensure(b[SD_SINFO], (size_t) nr * sizeof(bm2_sort_rec) + 8) ||
+        ctx->ensure(b[SD_MAX], 16) || ctx->ensure_host(ctx->sort_h[0], (size_t) nr * 8 + 16) ||
+        ctx->ensure_host(ctx->sort_h[1], (size_t) nr * sizeof(bm2_sort_rec) + 16)) return 1;
+    for (cudaEvent_t &ev : ctx->sort_ev) if (!ev) BM2_CUDA_OK(cudaEventCreate(&ev));
+    if (carry_len) BM2_CUDA_OK(cudaMemcpy(b[SD_OUT].p, carry, (size_t) carry_len, cudaMemcpyHostToDevice));   // carry may be this context's last carry
+    int64_t *h_offs = (int64_t *) ctx->sort_h[0].p;
+    bm2_sort_rec *h_info = (bm2_sort_rec *) ctx->sort_h[1].p;
+    const uint32_t *ord = (const uint32_t *) b[SD_VALS0].p;
+    if (nr) {
+        BM2_CUDA_OK(cudaMemcpyAsync(b[SD_IN].p, recs, (size_t) n, cudaMemcpyHostToDevice, st));
+        BM2_CUDA_OK(cudaMemcpyAsync(b[SD_STARTS].p, starts, (size_t) nr * 8, cudaMemcpyHostToDevice, st));
+        BM2_CUDA_OK(cudaMemsetAsync(b[SD_MAX].p, 0, 8, st));
+        const unsigned g = (unsigned) ((nr + 255) / 256), g1 = (unsigned) ((nr + 256) / 256);
+        BM2_CUDA_OK(cudaEventRecord(ctx->sort_ev[0], st));
+        sort_key_kernel<<<g, 256, 0, st>>>((const uint8_t *) b[SD_IN].p, (const int64_t *) b[SD_STARTS].p, nr, (bm2_sort_rec *) b[SD_INFO].p,
+                                           (int64_t *) b[SD_LEN].p, (unsigned *) b[SD_MAX].p);
+        BM2_CUDA_OK(cudaGetLastError());
+        BM2_CUDA_OK(cudaEventRecord(ctx->sort_ev[1], st));
+        unsigned mx[2] = { 0, 0 };
+        BM2_CUDA_OK(cudaMemcpyAsync(mx, b[SD_MAX].p, 8, cudaMemcpyDeviceToHost, st));
+        BM2_CUDA_OK(cudaStreamSynchronize(st));
+        const int pos_bits = bits_of(mx[1]), end_bit = bm2_max(1, bits_of(mx[0]) + pos_bits + 1);   // ranks 0..mx[0] (mx[0]: refID -1)
+        sort_pack_kernel<<<g, 256, 0, st>>>((const bm2_sort_rec *) b[SD_INFO].p, nr, mx[0], pos_bits, (uint64_t *) b[SD_KEYS0].p,
+                                            (uint32_t *) b[SD_VALS0].p);
+        BM2_CUDA_OK(cudaGetLastError());
+        cub::DoubleBuffer<uint64_t> kb((uint64_t *) b[SD_KEYS0].p, (uint64_t *) b[SD_KEYS1].p);
+        cub::DoubleBuffer<uint32_t> vb((uint32_t *) b[SD_VALS0].p, (uint32_t *) b[SD_VALS1].p);
+        size_t tb = b[SD_TEMP].cap;
+        BM2_CUDA_OK(cub::DeviceRadixSort::SortPairs(b[SD_TEMP].p, tb, kb, vb, (int) nr, 0, end_bit, st));
+        ord = vb.Current();
+        BM2_CUDA_OK(cudaEventRecord(ctx->sort_ev[2], st));
+        sort_permute_kernel<<<g1, 256, 0, st>>>(ord, nr, (const int64_t *) b[SD_LEN].p, (const bm2_sort_rec *) b[SD_INFO].p, (int64_t *) b[SD_LENS].p,
+                                                (bm2_sort_rec *) b[SD_SINFO].p);
+        BM2_CUDA_OK(cudaGetLastError());
+        tb = b[SD_TEMP].cap;
+        BM2_CUDA_OK(cub::DeviceScan::ExclusiveSum(b[SD_TEMP].p, tb, (const int64_t *) b[SD_LENS].p, (int64_t *) b[SD_OFFS].p, (int) nr + 1, st));
+        sort_gather_kernel<<<(unsigned) ((nr * 32 + 255) / 256), 256, 0, st>>>((const uint8_t *) b[SD_IN].p, (const int64_t *) b[SD_STARTS].p, ord,
+                                                                               (const int64_t *) b[SD_OFFS].p, (const int64_t *) b[SD_LENS].p, nr,
+                                                                               carry_len, (uint8_t *) b[SD_OUT].p);
+        BM2_CUDA_OK(cudaGetLastError());
+        BM2_CUDA_OK(cudaEventRecord(ctx->sort_ev[3], st));
+        BM2_CUDA_OK(cudaMemcpyAsync(h_offs, b[SD_OFFS].p, (size_t) (nr + 1) * 8, cudaMemcpyDeviceToHost, st));
+        BM2_CUDA_OK(cudaMemcpyAsync(h_info, b[SD_SINFO].p, (size_t) nr * sizeof(bm2_sort_rec), cudaMemcpyDeviceToHost, st));
+        BM2_CUDA_OK(cudaStreamSynchronize(st));
+        float ms[3] = { 0, 0, 0 };
+        for (int k = 0; k < 3; ++k) BM2_CUDA_OK(cudaEventElapsedTime(&ms[k], ctx->sort_ev[k], ctx->sort_ev[k + 1]));
+        for (int k = 0; k < 3; ++k) ctx->sort_ms[k] = ms[k];
+    } else h_offs[0] = 0;
+    const int64_t total = h_offs[nr];
+    std::vector<int64_t> cut;
+    SortLayout L;
+    bam_sort_layout(carry_len, h_offs, nr, total, last != 0, cut, L, h_info);
+    // the members: the sorted buffer is free after the gather, so the compressed bytes are gathered into the records' input buffer
+    const uint8_t *z = nullptr; int64_t zl = 0;
+    if (bgzf_compress_device(ctx, (const uint8_t *) b[SD_OUT].p, L.starts.data(), L.n_full, &z, &zl, &b[SD_IN])) return 1;
+    ctx->sort_ms[3] = ctx->bgzf_ms;
+    const int64_t c0 = L.starts[(size_t) L.n_full], c1 = carry_len + total;
+    ctx->sort_carry.resize((size_t) (c1 - c0));
+    if (c1 > c0) BM2_CUDA_OK(cudaMemcpy(ctx->sort_carry.data(), (const uint8_t *) b[SD_OUT].p + c0, (size_t) (c1 - c0), cudaMemcpyDeviceToHost));
+    ctx->sort_recs.assign(h_info, h_info + nr);
+    out->z = z; out->z_len = zl;
+    out->member_size = ctx->bgzf_sizes.data(); out->n_members = L.n_full;
+    out->carry = ctx->sort_carry.data(); out->carry_len = c1 - c0;
+    out->recs = ctx->sort_recs.data(); out->n_recs = nr;
+    return 0;
+}
+
+extern "C" int bm2_last_sort_stats(const bm2_ctx *ctx, double ms[4]) {
+    if (!ctx || !ms) return 1;
+    for (int k = 0; k < 4; ++k) ms[k] = ctx->sort_ms[k];
+    return 0;
+}
+
+extern "C" int bm2_bam_sort_memory(const bm2_ctx *ctx, int64_t run_bytes, int64_t *needed, int64_t *free_bytes) {
+    if (!ctx || run_bytes < 0 || !needed || !free_bytes) return 1;
+    bm2_ctx *ctx_for_error = (bm2_ctx *) ctx;
+    // what the buffers of one call ask for, each rounded up by 1.25 as bm2_ctx::ensure allocates: records in (reused for the compressed
+    // members), the sorted stream, the BGZF slots (one 64 KiB slot per 65280-byte block), and 120 bytes per record of keys, ordinals, lengths,
+    // offsets and index data (twice for the radix sort's double buffers)
+    const double r = (double) run_bytes, recs = r / kRecBytes + 1;
+    const double bytes = 1.25 * (r + (r + BGZF_BLOCK) + (r / BGZF_BLOCK + 2) * BGZF_MAX_MEMBER + 120 * recs) + 64.0 * (1 << 20);
+    size_t fr = 0, tot = 0;
+    BM2_CUDA_OK(cudaSetDevice(ctx->device));
+    BM2_CUDA_OK(cudaMemGetInfo(&fr, &tot));
+    *needed = (int64_t) bytes; *free_bytes = (int64_t) fr;
+    return 0;
+}

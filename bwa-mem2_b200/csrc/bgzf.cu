@@ -147,31 +147,27 @@ enum { BG_IN, BG_STARTS, BG_ITEMS, BG_SLOTS, BG_SIZES, BG_OFFS, BG_OUT };
 
 }  // namespace
 
-extern "C" int bm2_bgzf_compress(bm2_ctx *ctx, const uint8_t *in, int64_t n, const int64_t *cut, int64_t n_cut, const uint8_t **out, int64_t *out_len) {
+// the members of the nb blocks [starts[b], starts[b+1]) of d_in (device, on ctx's stream) -> *out (host, ctx's) and member sizes (ctx->bgzf_sizes);
+// gather: the device buffer the members are gathered into (nullptr: the context's own)
+int bgzf_compress_device(bm2_ctx *ctx, const uint8_t *d_in, const int64_t *starts, int64_t nb, const uint8_t **out, int64_t *out_len, DevBuf *gather) {
     bm2_ctx *ctx_for_error = ctx;
-    if (!ctx || !out || !out_len || n < 0 || (n && !in) || n_cut < 0 || (n_cut && !cut)) { if (ctx) bm2_set_error(ctx, "bm2_bgzf_compress: bad arguments"); return 1; }
-    for (int64_t i = 0; i < n_cut; ++i)
-        if (cut[i] < 0 || cut[i] > n || (i && cut[i] < cut[i - 1])) { bm2_set_error(ctx, "bm2_bgzf_compress: cut points must ascend within [0, n]"); return 1; }
-    ctx->bgzf_ms = 0; ctx->bgzf_members = 0;
+    ctx->bgzf_ms = 0; ctx->bgzf_members = 0; ctx->bgzf_sizes.clear();
     *out = nullptr; *out_len = 0;
-    std::vector<int64_t> starts;
-    const int64_t nb = bgzf_cut_blocks(n, cut, n_cut, starts);
     if (nb == 0) return 0;
     if (nb >= (1LL << 31)) { bm2_set_error(ctx, "bm2_bgzf_compress: too many blocks"); return 1; }
     BM2_CUDA_OK(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
     const int grid = (int) bm2_min<int64_t>(nb, ctx->n_sm);
     DevBuf *bg = ctx->bgzf_d;
-    if (ctx->ensure(bg[BG_IN], (size_t) n + 16) || ctx->ensure(bg[BG_STARTS], (size_t) (nb + 1) * 8) ||
+    if (ctx->ensure(bg[BG_STARTS], (size_t) (nb + 1) * 8) ||
         ctx->ensure(bg[BG_ITEMS], (size_t) grid * BGZF_BLOCK * 2) || ctx->ensure(bg[BG_SLOTS], (size_t) nb * BGZF_MAX_MEMBER) ||
         ctx->ensure(bg[BG_SIZES], (size_t) nb * 4) || ctx->ensure(bg[BG_OFFS], (size_t) (nb + 1) * 8) ||
         ctx->ensure_host(ctx->bgzf_h[0], (size_t) (nb + 1) * 8)) return 1;
     for (cudaEvent_t &ev : ctx->bgzf_ev) if (!ev) BM2_CUDA_OK(cudaEventCreate(&ev));
     BM2_CUDA_OK(cudaFuncSetAttribute(bgzf_block_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) kSmem));
-    BM2_CUDA_OK(cudaMemcpyAsync(bg[BG_IN].p, in, (size_t) n, cudaMemcpyHostToDevice, st));
-    BM2_CUDA_OK(cudaMemcpyAsync(bg[BG_STARTS].p, starts.data(), (size_t) (nb + 1) * 8, cudaMemcpyHostToDevice, st));
+    BM2_CUDA_OK(cudaMemcpyAsync(bg[BG_STARTS].p, starts, (size_t) (nb + 1) * 8, cudaMemcpyHostToDevice, st));
     BM2_CUDA_OK(cudaEventRecord(ctx->bgzf_ev[0], st));
-    bgzf_block_kernel<<<grid, kThreads, kSmem, st>>>((const uint8_t *) bg[BG_IN].p, (const int64_t *) bg[BG_STARTS].p, (int) nb, bgzf_x2n(),
+    bgzf_block_kernel<<<grid, kThreads, kSmem, st>>>(d_in, (const int64_t *) bg[BG_STARTS].p, (int) nb, bgzf_x2n(),
                                                      (uint16_t *) bg[BG_ITEMS].p, (uint8_t *) bg[BG_SLOTS].p, (int32_t *) bg[BG_SIZES].p);
     BM2_CUDA_OK(cudaGetLastError());
     BM2_CUDA_OK(cudaEventRecord(ctx->bgzf_ev[1], st));
@@ -183,15 +179,17 @@ extern "C" int bm2_bgzf_compress(bm2_ctx *ctx, const uint8_t *in, int64_t n, con
         if (hs[b] < 26 || hs[b] > BGZF_MAX_MEMBER) { bm2_set_error(ctx, "bm2_bgzf_compress: a member of " + std::to_string(hs[b]) + " bytes"); return 2; }
         offs[(size_t) b + 1] = offs[(size_t) b] + hs[b];
     }
+    ctx->bgzf_sizes.assign(hs, hs + nb);
     const int64_t total = offs[(size_t) nb];
-    if (ctx->ensure(bg[BG_OUT], (size_t) total + 16) || ctx->ensure_host(ctx->bgzf_h[1], (size_t) total + 16)) return 1;
+    DevBuf &dst = gather ? *gather : bg[BG_OUT];
+    if (ctx->ensure(dst, (size_t) total + 16) || ctx->ensure_host(ctx->bgzf_h[1], (size_t) total + 16)) return 1;
     BM2_CUDA_OK(cudaMemcpyAsync(bg[BG_OFFS].p, offs.data(), (size_t) (nb + 1) * 8, cudaMemcpyHostToDevice, st));
     BM2_CUDA_OK(cudaEventRecord(ctx->bgzf_ev[2], st));
     bgzf_gather_kernel<<<(unsigned) nb, 256, 0, st>>>((const uint8_t *) bg[BG_SLOTS].p, (const int32_t *) bg[BG_SIZES].p, (const int64_t *) bg[BG_OFFS].p,
-                                                      (uint8_t *) bg[BG_OUT].p);
+                                                      (uint8_t *) dst.p);
     BM2_CUDA_OK(cudaGetLastError());
     BM2_CUDA_OK(cudaEventRecord(ctx->bgzf_ev[3], st));
-    BM2_CUDA_OK(cudaMemcpyAsync(ctx->bgzf_h[1].p, bg[BG_OUT].p, (size_t) total, cudaMemcpyDeviceToHost, st));
+    BM2_CUDA_OK(cudaMemcpyAsync(ctx->bgzf_h[1].p, dst.p, (size_t) total, cudaMemcpyDeviceToHost, st));
     BM2_CUDA_OK(cudaStreamSynchronize(st));
     float ms0 = 0, ms1 = 0;
     BM2_CUDA_OK(cudaEventElapsedTime(&ms0, ctx->bgzf_ev[0], ctx->bgzf_ev[1]));
@@ -199,6 +197,23 @@ extern "C" int bm2_bgzf_compress(bm2_ctx *ctx, const uint8_t *in, int64_t n, con
     ctx->bgzf_ms = (double) ms0 + ms1; ctx->bgzf_members = nb;
     *out = (const uint8_t *) ctx->bgzf_h[1].p; *out_len = total;
     return 0;
+}
+
+extern "C" int bm2_bgzf_compress(bm2_ctx *ctx, const uint8_t *in, int64_t n, const int64_t *cut, int64_t n_cut, const uint8_t **out, int64_t *out_len) {
+    bm2_ctx *ctx_for_error = ctx;
+    if (!ctx || !out || !out_len || n < 0 || (n && !in) || n_cut < 0 || (n_cut && !cut)) { if (ctx) bm2_set_error(ctx, "bm2_bgzf_compress: bad arguments"); return 1; }
+    for (int64_t i = 0; i < n_cut; ++i)
+        if (cut[i] < 0 || cut[i] > n || (i && cut[i] < cut[i - 1])) { bm2_set_error(ctx, "bm2_bgzf_compress: cut points must ascend within [0, n]"); return 1; }
+    ctx->bgzf_ms = 0; ctx->bgzf_members = 0;
+    *out = nullptr; *out_len = 0;
+    std::vector<int64_t> starts;
+    const int64_t nb = bgzf_cut_blocks(n, cut, n_cut, starts);
+    if (nb == 0) return 0;
+    BM2_CUDA_OK(cudaSetDevice(ctx->device));
+    DevBuf *bg = ctx->bgzf_d;
+    if (ctx->ensure(bg[BG_IN], (size_t) n + 16)) return 1;
+    BM2_CUDA_OK(cudaMemcpyAsync(bg[BG_IN].p, in, (size_t) n, cudaMemcpyHostToDevice, ctx->stream));
+    return bgzf_compress_device(ctx, (const uint8_t *) bg[BG_IN].p, starts.data(), nb, out, out_len, nullptr);
 }
 
 extern "C" int bm2_last_bgzf_stats(const bm2_ctx *ctx, double *device_ms, int64_t *members) {

@@ -64,6 +64,14 @@ struct bm2_ctx {
     cudaEvent_t bgzf_ev[4] = {nullptr, nullptr, nullptr, nullptr};
     double bgzf_ms = 0;
     int64_t bgzf_members = 0;
+    std::vector<int32_t> bgzf_sizes;       // the last call's member sizes
+    // bm2_bam_sort_compress (bam_sort.cu): buffers, events around its stages, the last call's device times and outputs
+    DevBuf sort_d[14];
+    HostBuf sort_h[2];
+    cudaEvent_t sort_ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+    double sort_ms[4] = {0, 0, 0, 0};
+    std::vector<uint8_t> sort_carry;
+    std::vector<bm2_sort_rec> sort_recs;
 
     int ensure(DevBuf &b, size_t bytes);
     int ensure_host(HostBuf &b, size_t bytes);
@@ -71,7 +79,12 @@ struct bm2_ctx {
         std::vector<DevBuf *> v = {&io_pairs, &io_ref, &io_qer, &bsw_jobs, &bsw_outs, &bsw_scratch};
         for (auto &x : d) v.push_back(&x);
         for (auto &x : bgzf_d) v.push_back(&x);
+        for (auto &x : sort_d) v.push_back(&x);
         return v;
     }
-    std::vector<HostBuf *> all_host() { std::vector<HostBuf *> v; for (auto &x : h) v.push_back(&x); for (auto &x : bgzf_h) v.push_back(&x); return v; }
+    std::vector<HostBuf *> all_host() { std::vector<HostBuf *> v; for (auto &x : h) v.push_back(&x); for (auto &x : bgzf_h) v.push_back(&x); for (auto &x : sort_h) v.push_back(&x); return v; }
 };
+
+// bgzf.cu: the members of the nb blocks [starts[b], starts[b+1]) of the device bytes d_in, on ctx's stream (the body of bm2_bgzf_compress),
+// gathered into *gather (nullptr: the context's own buffer) before they are copied to the host
+int bgzf_compress_device(bm2_ctx *ctx, const uint8_t *d_in, const int64_t *starts, int64_t nb, const uint8_t **out, int64_t *out_len, DevBuf *gather);

@@ -20,6 +20,7 @@
 //   bm2_sam_pe / bm2_sam_se       worker_sam's arithmetic                                             (src/bwamem.cpp:1262-1336)
 //   bm2_sam_format_ex             mem_aln2sam's text with RG / the -C comment / XR                    (src/bwamem.cpp:1592-1730)
 //     or bm2_bam_format_ex        --bam: the same records as BAM, then bm2_bgzf_compress: BGZF members compressed on the GPU
+//        then bm2_bam_sort_compress  --sort: the records in sorted runs, merged, compressed on the GPU, and the BAI (bam_sort.h)
 // Chunks in flight: the reference's kt_pipeline runs its three steps (read, process, write) on two worker threads so that one chunk's I/O
 // overlaps another's computation (src/fastmap.cpp:952-1003, src/kthread.cpp:122-176).  Here -p workers (default 2) each own a context
 // (bm2_create_sibling: one index in HBM) and take whole chunks off a queue; the GPU interleaves the kernels of the two chunks, the host side of
@@ -33,6 +34,7 @@
 #include "bm2_b200.h"
 #include "../csrc/seq_grammar.cuh"
 #include "../csrc/read_input.h"
+#include "../csrc/bam_sort.h"
 #include <algorithm>
 #include <chrono>
 #include <condition_variable>
@@ -42,6 +44,7 @@
 #include <thread>
 #include <cmath>
 #include <cctype>
+#include <cerrno>
 #include <cstdio>
 #include <unistd.h>
 #include <cstdlib>
@@ -71,6 +74,7 @@ struct Shared {
     const bm2_pestat_t *pes0 = nullptr;                          // -I: used instead of bm2_pestat
     bm2_sam_text_extra extra{};                                  // -R / -C / -V
     bool copy_comment = false, bam = false;
+    BamSortSink *sink = nullptr;                                 // --sort: the records go to the sorted runs instead of the output
     double t_split = 0;
     long long seq_chunks = 0;                                    // chunks that went through bm2_seq_encode
     size_t in_flight = 0;                                        // bytes of the chunks queued or being aligned
@@ -188,7 +192,7 @@ void worker(Shared *sh, bm2_ctx *ctx) {
         }
         const uint8_t *outp = (const uint8_t *) text; int64_t out_len = len;
         double bgzf_ms = 0;
-        if (sh->bam) {                                                   // BGZF blocks cut at the records' starts, within the chunk
+        if (sh->bam && !sh->sink) {                                      // BGZF blocks cut at the records' starts, within the chunk
             std::vector<int64_t> cut;
             for (int64_t q = 0; q + 4 <= len; q += 4 + *(const int32_t *) (text + q)) cut.push_back(q);
             if (bm2_bgzf_compress(ctx, (const uint8_t *) text, len, cut.data(), (int64_t) cut.size(), &outp, &out_len)) die("bm2_bgzf_compress", ctx);
@@ -201,13 +205,14 @@ void worker(Shared *sh, bm2_ctx *ctx) {
             sh->cv_turn.wait(lk, [&] { return sh->next_to_write == ck.index; });
         }
         const double t6 = now_s();
-        fwrite(outp, 1, (size_t) out_len, sh->out);
+        if (sh->sink) sh->sink->add(outp, out_len);
+        else fwrite(outp, 1, (size_t) out_len, sh->out);
         bm2_free(text);
         const double t7 = now_s();
         {
             std::lock_guard<std::mutex> lk(sh->mu);
             sh->t_enc += t1 - t0; sh->t_aln += t.aln; sh->t_pes += t.pes; sh->t_sam += t.sam; sh->t_fmt += t.fmt; sh->t_turn += t6 - t5; sh->t_write += t7 - t6;
-            sh->t_bam += t.bam; sh->t_bgzf += bgzf_ms / 1e3; sh->bam_bytes += sh->bam ? len : 0; sh->bgzf_bytes += sh->bam ? out_len : 0;
+            sh->t_bam += t.bam; sh->t_bgzf += bgzf_ms / 1e3; sh->bam_bytes += sh->bam ? len : 0; sh->bgzf_bytes += sh->bam && !sh->sink ? out_len : 0;
             sh->n_processed += fq.n_reads; sh->seq_chunks += !ck.simple; sh->in_flight -= ck.bytes.size();
             sh->chunk_s.push_back(t7 - t0); sh->chunk_done_s.push_back(t7 - sh->t_loop); sh->chunk_reads.push_back(fq.n_reads);
             ++sh->next_to_write;
@@ -275,6 +280,10 @@ void usage(const bm2_mem_opt_t &o) {
 "              integer is this count; any other -p (alone, or in a cluster like -5SP) is smart pairing.  An index prefix that is a bare\n"
 "              integer must then be written as a path (./2) after a smart-pairing -p.\n"
 "  --bam       write BAM (BGZF-compressed on the GPU) instead of SAM; the same records, header and @PG line\n"
+"  --sort      write coordinate-sorted BAM (implies --bam), sorted on the GPU in runs merged through temporary files next to -o\n"
+"              (<out>.tmp.NNNN) or, on standard output, in ${TMPDIR:-/tmp}; the header's @HD line gets SO:coordinate\n"
+"  --sort-mem SIZE  uncompressed BAM bytes per sorted run, with a K, M or G suffix [2G]\n"
+"  --write-index  write the BAI index <out>.bai (needs --sort and -o)\n"
 "  --dump-opt  print the parsed options, the -I values, the read group and the header as JSON, and exit before any GPU work\n"
 "  --dump-chunks  print the chunks the input is cut into (first read, byte ranges, whether bm2_fastq_encode takes them) as JSON lines,\n"
 "              and exit without loading the index\n",
@@ -320,6 +329,44 @@ void int_pair(const char *arg, int *a, int *b) {
     if (*p != 0 && ispunct((unsigned char) *p) && isdigit((unsigned char) p[1])) *b = (int) strtol(p + 1, &p, 10);
 }
 
+// "SIZE" of --sort-mem: a positive decimal integer, optionally followed by one of K M G (binary multiples, either case)
+bool parse_size(const char *s, long long *v) {
+    char *e;
+    if (!isdigit((unsigned char) *s)) return false;
+    errno = 0;
+    const unsigned long long x = strtoull(s, &e, 10);
+    int shift = 0;
+    if (*e == 'k' || *e == 'K') shift = 10, ++e;
+    else if (*e == 'm' || *e == 'M') shift = 20, ++e;
+    else if (*e == 'g' || *e == 'G') shift = 30, ++e;
+    if (*e || errno || x == 0 || x > (unsigned long long) (INT64_MAX >> shift)) return false;
+    *v = (long long) (x << shift);
+    return true;
+}
+
+// --sort: the header's @HD line first, with SO:coordinate; an @HD line from -H keeps its other fields
+std::string coordinate_header(const std::string &h) {
+    std::string hd, rest;
+    for (size_t b = 0; b < h.size();) {
+        size_t e = h.find('\n', b); if (e == std::string::npos) e = h.size();
+        const std::string line = h.substr(b, e - b);
+        if (hd.empty() && (line == "@HD" || line.compare(0, 4, "@HD\t") == 0)) {
+            hd = "@HD";
+            bool so = false;
+            for (size_t p = 3; p < line.size();) {
+                size_t q = line.find('\t', p + 1); if (q == std::string::npos) q = line.size();
+                const std::string f = line.substr(p + 1, q - p - 1);
+                if (f.compare(0, 3, "SO:") == 0) { if (!so) hd += "\tSO:coordinate"; so = true; }
+                else hd += "\t" + f;
+                p = q;
+            }
+            if (!so) hd += "\tSO:coordinate";
+        } else rest += line + "\n";
+        b = e + 1;
+    }
+    return (hd.empty() ? std::string("@HD\tVN:1.6\tSO:coordinate") : hd) + "\n" + rest;
+}
+
 bool is_count(const char *s) {
     if (!*s) return false;
     for (const char *p = s; *p; ++p) if (!isdigit((unsigned char) *p)) return false;
@@ -332,13 +379,22 @@ int main(int argc, char **argv) {
     static const char *const optstring = "51qpaMCSPVYjk:c:v:s:r:t:R:A:B:O:E:U:w:L:d:T:Q:D:m:I:N:W:x:G:h:y:K:X:H:o:f:";
     // this program's own arguments first: `-p N` (worker count), --bam and --dump-opt are taken out of the list, walking it the way getopt will
     // (option arguments skipped, `--` ends the options), so that everything left is parsed as main_mem parses it
-    int workers = 2; bool dump = false, dump_chunks = false, bam = false;
+    int workers = 2; bool dump = false, dump_chunks = false, bam = false, sort = false, write_index = false;
+    long long sort_mem = 2LL << 30;
     std::vector<char *> av = { argv[0] };
     for (int i = 1; i < argc; ++i) {
         char *s = argv[i];
         if (!strcmp(s, "--")) { for (; i < argc; ++i) av.push_back(argv[i]); break; }
         if (!strcmp(s, "--dump-opt")) { dump = true; continue; }
         if (!strcmp(s, "--bam")) { bam = true; continue; }
+        if (!strcmp(s, "--sort")) { sort = bam = true; continue; }
+        if (!strcmp(s, "--write-index")) { write_index = true; continue; }
+        if (!strcmp(s, "--sort-mem")) {
+            if (i + 1 >= argc || !parse_size(argv[i + 1], &sort_mem)) {
+                fprintf(stderr, "[E::bm2_mem] --sort-mem takes a positive byte count with an optional K, M or G suffix\n"); return 1;
+            }
+            ++i; continue;
+        }
         if (!strcmp(s, "--dump-chunks")) { dump_chunks = true; continue; }
         if (!strcmp(s, "-p") && i + 1 < argc && is_count(argv[i + 1])) { workers = atoi(argv[++i]); continue; }
         av.push_back(s);
@@ -480,6 +536,7 @@ int main(int argc, char **argv) {
     }
     const int threads = opt.n_threads;
     if (workers > 4) workers = 4;
+    if (write_index && (!sort || !out_path)) { fprintf(stderr, "[E::bm2_mem] --write-index needs --sort and -o FILE\n"); return 1; }
     const bool smart = (opt.flag & 0x400) != 0;
     const char *prefix = v[optind], *f1 = v[optind + 1], *f2 = optind + 2 < ac ? v[optind + 2] : nullptr;
     if (f2 && smart) { fprintf(stderr, "[W::bm2_mem] when '-p' is in use, the second query file is ignored.\n"); f2 = nullptr; }
@@ -529,6 +586,7 @@ int main(int argc, char **argv) {
             for (size_t i = 0; i < names.size(); ++i)
                 header += "@SQ\tSN:" + names[i] + "\tLN:" + std::to_string(lens[i]) + (idx->ann_is_alt && idx->ann_is_alt[i] ? "\tAH:*\n" : "\n");
         if (have_hdr) header += hdr_line + "\n";
+        if (sort) header = coordinate_header(header);
     }
     if (dump) {
         const bm2_mem_opt_t &o = opt;
@@ -545,25 +603,41 @@ int main(int argc, char **argv) {
         printf("], \"pes\": ");
         if (use_pes) printf("{\"low\": %d, \"high\": %d, \"avg\": %.17g, \"std\": %.17g}", pes[1].low, pes[1].high, pes[1].avg, pes[1].std);
         else printf("null");
-        printf(", \"rg_id\": %s, \"copy_comment\": %s, \"ignore_alt\": %s, \"smart_pairing\": %s, \"workers\": %d, \"files\": %d, \"bam\": %s, \"header\": %s}\n",
+        printf(", \"rg_id\": %s, \"copy_comment\": %s, \"ignore_alt\": %s, \"smart_pairing\": %s, \"workers\": %d, \"files\": %d, \"bam\": %s, ",
                have_rg ? json_str(rg_id).c_str() : "null", copy_comment ? "true" : "false", ignore_alt ? "true" : "false", smart ? "true" : "false",
-               workers, f2 ? 2 : 1, bam ? "true" : "false", json_str(header).c_str());
+               workers, f2 ? 2 : 1, bam ? "true" : "false");
+        if (sort) printf("\"sort\": true, \"sort_mem\": %lld, \"write_index\": %s, ", sort_mem, write_index ? "true" : "false");
+        printf("\"header\": %s}\n", json_str(header).c_str());
         bm2_index_free(idx);
         return 0;
     }
     if (bam)                                                          // BAM stores l_ref as int32 (SAMv1 §4.2)
         for (size_t i = 0; i < names.size(); ++i)
             if (lens[i] > INT32_MAX) { fprintf(stderr, "[E::bm2_mem] contig %s is %lld bp long: BAM cannot store a contig longer than 2^31-1\n", names[i].c_str(), lens[i]); return 1; }
+    if (write_index)                                                  // BAI's bins reach 2^29 (SAMv1 §5.3); longer contigs need CSI
+        for (size_t i = 0; i < names.size(); ++i)
+            if (lens[i] > (1LL << 29) - 1) { fprintf(stderr, "[E::bm2_mem] contig %s is %lld bp long: BAI cannot index a contig longer than 2^29-1\n", names[i].c_str(), lens[i]); return 1; }
     std::vector<const char *> cnames, canno;
     for (size_t i = 0; i < names.size(); ++i) { cnames.push_back(names[i].c_str()); canno.push_back(annos[i].c_str()); }
     std::vector<bm2_ctx *> ctxs((size_t) workers, nullptr);
     if (bm2_create(&ctxs[0], 0, idx, &opt)) { fprintf(stderr, "bm2_mem: %s\n", bm2_last_error(nullptr)); return 3; }
     for (int w = 1; w < workers; ++w)
         if (bm2_create_sibling(&ctxs[w], ctxs[0])) { fprintf(stderr, "bm2_mem: %s\n", bm2_last_error(ctxs[0])); return 3; }
+    bm2_ctx *sort_ctx = nullptr;                                      // --sort: the runs are sorted on a context of their own
+    if (sort) {
+        if (bm2_create_sibling(&sort_ctx, ctxs[0])) { fprintf(stderr, "bm2_mem: %s\n", bm2_last_error(ctxs[0])); return 3; }
+        int64_t need = 0, avail = 0;
+        if (bm2_bam_sort_memory(sort_ctx, sort_mem, &need, &avail)) die("bm2_bam_sort_memory", sort_ctx);
+        if (need > avail) {
+            fprintf(stderr, "[E::bm2_mem] --sort-mem %lld: one run sort needs %lld bytes of device memory, %lld bytes free\n", sort_mem, (long long) need, (long long) avail);
+            return 3;
+        }
+    }
     const double t_index = now_s() - t_start;
     Inputs in;
     if (!in.open(f1, f2)) return 2;
     FILE *out = out_path ? fopen(out_path, "wb") : stdout;
+    int64_t header_z = 0;
     if (!out) { fprintf(stderr, "bm2_mem: cannot open %s\n", out_path); return 2; }
     header += std::string("@PG\tID:bm2_mem\tPN:bm2_mem\tVN:b200-r2\tCL:") + argv[0];
     for (int i = 1; i < argc; ++i) header += std::string(" ") + argv[i];
@@ -578,10 +652,29 @@ int main(int argc, char **argv) {
         const uint8_t *z = nullptr; int64_t zl = 0;
         if (bm2_bgzf_compress(ctxs[0], (const uint8_t *) h.data(), (int64_t) h.size(), nullptr, 0, &z, &zl)) die("bm2_bgzf_compress", ctxs[0]);
         fwrite(z, 1, (size_t) zl, out);
+        header_z = zl;
+    }
+    BamSortSink sink;
+    if (sort) {
+        sink.sort = [sort_ctx](const uint8_t *r, int64_t n, const int64_t *st, int64_t nr, const uint8_t *c, int64_t cl, int last, bm2_sort_out *o,
+                               double *device_s) {
+            const int rc = bm2_bam_sort_compress(sort_ctx, r, n, st, nr, c, cl, last, o);
+            double ms[4] = { 0, 0, 0, 0 };
+            bm2_last_sort_stats(sort_ctx, ms);
+            *device_s = (ms[0] + ms[1] + ms[2] + ms[3]) / 1e3;
+            return rc;
+        };
+        sink.fail = [sort_ctx](const std::string &m) { die(m.c_str(), m == "bm2_bam_sort_compress" ? sort_ctx : nullptr); };
+        sink.run_bytes = sort_mem; sink.threads = threads;
+        if (out_path) sink.tmp_prefix = std::string(out_path) + ".tmp.";
+        else {
+            const char *td = getenv("TMPDIR");
+            sink.tmp_prefix = std::string(td && *td ? td : "/tmp") + "/bm2_mem." + std::to_string((long long) getpid()) + ".";
+        }
     }
     Shared sh;
     sh.opt = &opt; sh.idx = idx; sh.cnames = cnames.data(); sh.paired = f2 != nullptr; sh.smart = smart; sh.threads = threads; sh.out = out;
-    sh.pes0 = use_pes ? pes : nullptr; sh.copy_comment = copy_comment; sh.bam = bam;
+    sh.pes0 = use_pes ? pes : nullptr; sh.copy_comment = copy_comment; sh.bam = bam; sh.sink = sort ? &sink : nullptr;
     sh.extra.rg_id = have_rg ? rg_id.c_str() : nullptr; sh.extra.contig_anno = canno.data(); sh.extra.ref_hdr = (opt.flag & 0x100) != 0;
     sh.t_loop = now_s();
     std::vector<std::thread> pool;
@@ -599,6 +692,18 @@ int main(int argc, char **argv) {
     sh.cv_work.notify_all();
     for (auto &t : pool) t.join();
     const double loop_s = now_s() - sh.t_loop;
+    BaiBuilder bai((int) names.size());
+    double index_s = 0;
+    if (sort) {
+        sink.finish(out, (uint64_t) header_z, write_index ? &bai : nullptr);
+        if (write_index) {
+            const double t0 = now_s();
+            const std::string b = bai.bytes(), path = std::string(out_path) + ".bai";
+            FILE *f = fopen(path.c_str(), "wb");
+            if (!f || fwrite(b.data(), 1, b.size(), f) != b.size() || fclose(f)) { fprintf(stderr, "bm2_mem: cannot write %s\n", path.c_str()); return 2; }
+            index_s = now_s() - t0;
+        }
+    }
     if (bam) {                                                        // the BGZF end-of-file marker (SAMv1 §4.1.2)
         static const uint8_t eof[28] = { 0x1f, 0x8b, 8, 4, 0, 0, 0, 0, 0, 0xff, 6, 0, 0x42, 0x43, 2, 0, 0x1b, 0, 3, 0, 0, 0, 0, 0, 0, 0, 0, 0 };
         fwrite(eof, 1, sizeof eof, out);
@@ -615,7 +720,11 @@ int main(int argc, char **argv) {
     fprintf(stderr, "], \"smart_pair_split_s\": %.6f, \"seq_encode_chunks\": %lld, \"read_s\": %.6f, \"gzip_members\": %lld, \"input_peak_bytes\": %zu",
             sh.t_split, sh.seq_chunks, read_s, (long long) (in.s[0].gzip_members + in.s[1].gzip_members), input_peak);
     if (bam) fprintf(stderr, ", \"bam_format_s\": %.6f, \"bgzf_s\": %.6f, \"bam_bytes\": %lld, \"bgzf_bytes\": %lld", sh.t_bam, sh.t_bgzf, sh.bam_bytes, sh.bgzf_bytes);
+    if (sort)
+        fprintf(stderr, ", \"sort_runs\": %lld, \"spill_bytes\": %lld, \"sort_s\": %.6f, \"merge_s\": %.6f, \"merge_windows\": %lld, \"index_s\": %.6f",
+                (long long) std::max<size_t>(sink.runs.size(), 1), (long long) sink.spill_bytes, sink.sort_s, sink.merge_s, (long long) sink.merge_windows, index_s);
     fprintf(stderr, "}\n");
+    if (sort_ctx) bm2_destroy(sort_ctx);
     for (int w = workers - 1; w >= 0; --w) bm2_destroy(ctxs[w]);
     bm2_index_free(idx);
     return 0;

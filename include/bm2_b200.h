@@ -421,6 +421,33 @@ int  bm2_bgzf_compress(bm2_ctx *ctx, const uint8_t *in, int64_t n, const int64_t
 /* The last bm2_bgzf_compress call: device time of its kernels (CUDA events, ms) and its member count. */
 int  bm2_last_bgzf_stats(const bm2_ctx *ctx, double *device_ms, int64_t *members);
 
+/* ---- Coordinate sort of BAM records on the GPU, compressed as they leave (bm2_mem --sort) -----------------------------------------------
+ * One buffer of records (a sorted run, or a merge window) is stably sorted by samtools' coordinate key
+ *   ((uint32) refID << 32) | ((uint32) (pos + 1) << 1) | (flag & 16 ? 1 : 0)
+ * (refID -1 last, ties in input order) and compressed by bm2_bgzf_compress's kernels straight from device memory.  The stream is
+ * carry + the sorted records, cut by htslib's rule over all of it: called window after window with each call's carry passed to the next, the
+ * BGZF bytes are those of the whole sorted stream compressed at once.
+ * recs: n bytes (HOST); starts: the n_recs record offsets, ascending, each record within n.  carry: carry_len (< 65280) bytes of the previous
+ * call's unfinished block (HOST, may be the previous *out's carry).  last != 0: the final block is compressed too and the carry is empty.
+ * Out (owned by the context, valid until its next call):
+ *   z / z_len                  whole BGZF members, no EOF block; member_size[k]: the size of member k, n_members of them
+ *   carry / carry_len          the unfinished last block's uncompressed bytes (0 when last or when the stream ends on a full block)
+ *   recs[n_recs]               per record in output order: refID, pos, end (bam_endpos), bin = reg2bin(pos, end) (4680 for refID -1), flag,
+ *                              block (0 = the member that starts with the carry; n_members = the new carry's block) and offset in it */
+typedef struct { int32_t rid, pos, end; uint16_t bin, flag; int64_t block; int32_t offset, _pad; } bm2_sort_rec;
+typedef struct {
+    const uint8_t *z; int64_t z_len;
+    const int32_t *member_size; int64_t n_members;
+    const uint8_t *carry; int64_t carry_len;
+    const bm2_sort_rec *recs; int64_t n_recs;
+} bm2_sort_out;
+int  bm2_bam_sort_compress(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int64_t *starts, int64_t n_recs, const uint8_t *carry,
+                           int64_t carry_len, int last, bm2_sort_out *out);
+/* The last bm2_bam_sort_compress call: device ms (CUDA events) of its stages: ms[0] keys, ms[1] radix sort, ms[2] scan + gather, ms[3] BGZF. */
+int  bm2_last_sort_stats(const bm2_ctx *ctx, double ms[4]);
+/* Device bytes one bm2_bam_sort_compress call on run_bytes of records of about 300 bytes needs, and the bytes free on ctx's device now. */
+int  bm2_bam_sort_memory(const bm2_ctx *ctx, int64_t run_bytes, int64_t *needed, int64_t *free_bytes);
+
 /* Staged mate rescue inside bm2_sam_pe (same records, other kernels): the windows mem_matesw (src/bwamem_pair.cpp:150-283) can ask for are
  * listed for all pairs of a wave from the regions before any rescue, aligned as one batch with one window per warp (the job shape of
  * bm2_ksw_align2; the reference batches the same alignments across pairs in its kswv path, src/bwamem_pair.cpp:930-1248, src/kswv.cpp),
