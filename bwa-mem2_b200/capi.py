@@ -204,6 +204,10 @@ class RegResult(C.Structure):
 SORT_REC_DT = np.dtype([("rid", "<i4"), ("pos", "<i4"), ("end", "<i4"), ("bin", "<u2"), ("flag", "<u2"), ("block", "<i8"), ("offset", "<i4"), ("_pad", "<i4")])
 
 
+# bm2_dup_signatures / bm2_dup_resolve: one entry of a duplicate space (include/bm2_b200.h); kind 0 pair, 1 fragment, 2 pair end
+DUP_ENTRY_DT = np.dtype([("k1", "<u8"), ("k2", "<u8"), ("tid", "<i8"), ("score", "<i4"), ("kind", "<i4")])
+
+
 class SortOut(C.Structure):
     _fields_ = [("z", C.c_void_p), ("z_len", C.c_int64), ("member_size", C.c_void_p), ("n_members", C.c_int64), ("carry", C.c_void_p),
                 ("carry_len", C.c_int64), ("recs", C.c_void_p), ("n_recs", C.c_int64)]
@@ -213,7 +217,8 @@ EXPORTS = ["bm2_create_sibling", "bm2_fastq_encode", "bm2_seq_encode", "bm2_fast
            "bm2_last_error", "bm2_extend_pairs", "bm2_extend_pairs_device", "bm2_collect_smems", "bm2_seed_chain",
            "bm2_seed_chain_extend", "bm2_last_stage_ms", "bm2_gen_cigar", "bm2_pestat", "bm2_sam_pe", "bm2_sam_se", "bm2_ksw_align2",
            "bm2_fasta_pack", "bm2_index_build", "bm2_bam_format_ex", "bm2_bgzf_compress", "bm2_last_bgzf_stats",
-           "bm2_bam_sort_compress", "bm2_last_sort_stats", "bm2_bam_sort_memory"]
+           "bm2_bam_sort_compress", "bm2_last_sort_stats", "bm2_bam_sort_memory", "bm2_bam_sort_memory_ex", "bm2_bam_sort_compress_ex",
+           "bm2_dup_signatures", "bm2_dup_resolve", "bm2_last_dup_stats", "bm2_dup_set"]
 
 _lib = None
 
@@ -547,6 +552,73 @@ class Context:
         sizes = _host(o.member_size, o.n_members, np.int32) if o.n_members else np.zeros(0, np.int32)
         return dict(z=C.string_at(o.z, o.z_len) if o.z_len else b"", member_size=sizes, carry=C.string_at(o.carry, o.carry_len) if o.carry_len else b"",
                     recs=recs, ms=dict(keys=ms[0], sort=ms[1], gather=ms[2], bgzf=ms[3]))
+
+    def bam_sort_compress_ex(self, data: bytes, starts, tids, carry: bytes = b"", last: bool = True):
+        """bm2_bam_sort_compress_ex: bam_sort_compress with each record's template id (int64[]) carried through the sort; records of the
+        templates set by dup_set get 0x400 unless unmapped -> bam_sort_compress's dict plus tids (int64[], output order)."""
+        starts = np.ascontiguousarray(starts, np.int64); tids = np.ascontiguousarray(tids, np.int64)
+        assert len(tids) == len(starts)
+        buf = np.frombuffer(data, np.uint8) if len(data) else np.zeros(1, np.uint8)
+        cb = np.frombuffer(carry, np.uint8) if len(carry) else np.zeros(1, np.uint8)
+        tb = tids if len(tids) else np.zeros(1, np.int64)
+        o = SortOut(); to = C.c_void_p()
+        f = lib().bm2_bam_sort_compress_ex
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]
+        self._check(f(self._ctx, buf.ctypes.data, len(data), starts.ctypes.data, len(starts), tb.ctypes.data, cb.ctypes.data, len(carry), int(last),
+                      C.byref(o), C.byref(to)), "bm2_bam_sort_compress_ex")
+        ms = (C.c_double * 4)()
+        lib().bm2_last_sort_stats.argtypes = [C.c_void_p, C.c_void_p]
+        lib().bm2_last_sort_stats(self._ctx, ms)
+        recs = np.ctypeslib.as_array(C.cast(o.recs, C.POINTER(C.c_uint8)), shape=(o.n_recs * SORT_REC_DT.itemsize,)).view(SORT_REC_DT).copy() \
+            if o.n_recs else np.zeros(0, SORT_REC_DT)
+        sizes = _host(o.member_size, o.n_members, np.int32) if o.n_members else np.zeros(0, np.int32)
+        return dict(z=C.string_at(o.z, o.z_len) if o.z_len else b"", member_size=sizes, carry=C.string_at(o.carry, o.carry_len) if o.carry_len else b"",
+                    recs=recs, tids=_host(to.value, o.n_recs, np.int64) if o.n_recs else np.zeros(0, np.int64),
+                    ms=dict(keys=ms[0], sort=ms[1], gather=ms[2], bgzf=ms[3]))
+
+    def dup_signatures(self, data: bytes, starts, tmpl_first, tmpl_id):
+        """bm2_dup_signatures: the entries of the templates [tmpl_first[t], tmpl_first[t+1]) of the records of data (uncompressed BAM) starting
+        at starts, with ids tmpl_id -> (pair entries, fragment-space entries, device ms), DUP_ENTRY_DT in template order."""
+        starts = np.ascontiguousarray(starts, np.int64); tf = np.ascontiguousarray(tmpl_first, np.int64); ti = np.ascontiguousarray(tmpl_id, np.int64)
+        buf = np.frombuffer(data, np.uint8) if len(data) else np.zeros(1, np.uint8)
+        sb = starts if len(starts) else np.zeros(1, np.int64)
+        tib = ti if len(ti) else np.zeros(1, np.int64)
+        p, f_ = C.c_void_p(), C.c_void_p(); n_p, n_f = C.c_int64(), C.c_int64()
+        f = lib().bm2_dup_signatures
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64] + [C.c_void_p] * 4
+        self._check(f(self._ctx, buf.ctypes.data, len(data), sb.ctypes.data, len(starts), tf.ctypes.data, tib.ctypes.data, len(ti),
+                      C.byref(p), C.byref(n_p), C.byref(f_), C.byref(n_f)), "bm2_dup_signatures")
+        ms = C.c_double()
+        lib().bm2_last_dup_stats.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        lib().bm2_last_dup_stats(self._ctx, C.byref(ms), None)
+        return (_host(p.value, n_p.value, DUP_ENTRY_DT) if n_p.value else np.zeros(0, DUP_ENTRY_DT),
+                _host(f_.value, n_f.value, DUP_ENTRY_DT) if n_f.value else np.zeros(0, DUP_ENTRY_DT), ms.value)
+
+    def dup_resolve(self, entries, resolve: bool = True):
+        """bm2_dup_resolve: entries (DUP_ENTRY_DT) of one space sorted by (k1, k2, score descending, tid) -> (the sorted entries, device ms)
+        when not resolve, else (the duplicates' template ids in sorted order, device ms)."""
+        e = np.ascontiguousarray(entries, DUP_ENTRY_DT)
+        eb = e if len(e) else np.zeros(1, DUP_ENTRY_DT)
+        srt, d = C.c_void_p(), C.c_void_p(); nd = C.c_int64()
+        f = lib().bm2_dup_resolve
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+        self._check(f(self._ctx, eb.ctypes.data, len(e), int(resolve), None if resolve else C.byref(srt), C.byref(d) if resolve else None,
+                      C.byref(nd) if resolve else None), "bm2_dup_resolve")
+        ms = C.c_double()
+        lib().bm2_last_dup_stats.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        lib().bm2_last_dup_stats(self._ctx, None, C.byref(ms))
+        if resolve:
+            return (_host(d.value, nd.value, np.int64) if nd.value else np.zeros(0, np.int64)), ms.value
+        return (_host(srt.value, len(e), DUP_ENTRY_DT) if len(e) else np.zeros(0, DUP_ENTRY_DT)), ms.value
+
+    def dup_set(self, dup_tids, n_bits: int):
+        """bm2_dup_set: the bitset of n_bits bits with the templates dup_tids set, kept on this context for bam_sort_compress_ex."""
+        bits = np.zeros(max((n_bits + 63) // 64, 1), np.uint64)
+        for t in np.asarray(dup_tids, np.int64):
+            bits[t >> 6] |= np.uint64(1) << np.uint64(t & 63)
+        f = lib().bm2_dup_set
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
+        self._check(f(self._ctx, bits.ctypes.data, int(n_bits)), "bm2_dup_set")
 
     def set_sam_staged(self, on: int):
         """bm2_set_sam_staged: 1 / 2 = the rescue's local alignments as a batch (one window per warp / per thread) before the per-pair kernel, 0 = inside it."""

@@ -9,9 +9,13 @@
 //   gather      one warp per record, 16-byte copies when source and destination agree modulo 16
 //   BGZF        the blocks are cut on the host (bam_sort_layout) from the scan, and bm2_bgzf_compress's kernels compress them straight from the
 //               sorted device buffer; the unfinished last block goes back as the carry
+// bm2_bam_sort_compress_ex is the same code with one template id per record carried through the permutation; with a duplicate bitset on the
+// context (bm2_dup_set, markdup.cu) the key kernel sets 0x400 in the index data of the records of duplicate templates and the gather writes it
+// into the copied record.
 #include "bm2_common.cuh"
 #include "bm2_ctx.h"
 #include "bam_sort_device.cuh"
+#include "markdup_device.cuh"
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 #include <vector>
@@ -20,13 +24,15 @@ namespace {
 
 constexpr int kRecBytes = 300;      // a short read's record, for bm2_bam_sort_memory's estimate
 
+// tids / dup_bits (bm2_bam_sort_compress_ex with a bitset): a record of a duplicate template that lacks 0x4 gets 0x400 in its info's flag
 __global__ void sort_key_kernel(const uint8_t *__restrict__ in, const int64_t *__restrict__ starts, int64_t n, bm2_sort_rec *info,
-                                int64_t *len, unsigned *maxes) {
+                                int64_t *len, unsigned *maxes, const int64_t *__restrict__ tids, const uint64_t *__restrict__ dup_bits, int64_t n_bits) {
     const int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
     unsigned mr = 0, mp = 0;
     if (i < n) {
         const uint8_t *r = in + starts[i];
-        const bm2_sort_rec s = bam_sort_rec(r);
+        bm2_sort_rec s = bam_sort_rec(r);
+        if (dup_bits) s.flag = dup_marked_flag(s.flag, tids[i], dup_bits, n_bits);
         info[i] = s;
         len[i] = 4 + (int64_t) bam_le32(r);
         mr = s.rid >= 0 ? (unsigned) s.rid + 1 : 0;
@@ -48,17 +54,19 @@ __global__ void sort_pack_kernel(const bm2_sort_rec *__restrict__ info, int64_t 
 }
 
 __global__ void sort_permute_kernel(const uint32_t *__restrict__ ord, int64_t n, const int64_t *__restrict__ len, const bm2_sort_rec *__restrict__ info,
-                                    int64_t *len_sorted, bm2_sort_rec *info_sorted) {
+                                    int64_t *len_sorted, bm2_sort_rec *info_sorted, const int64_t *__restrict__ tids, int64_t *tids_sorted) {
     const int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
     if (i > n) return;
     if (i == n) { len_sorted[n] = 0; return; }
     const uint32_t k = ord[i];
     len_sorted[i] = len[k]; info_sorted[i] = info[k];
+    if (tids) tids_sorted[i] = tids[k];
 }
 
-// one warp per record: in + starts[ord[i]] -> out + base + offs[i]
+// one warp per record: in + starts[ord[i]] -> out + base + offs[i]; with info_sorted (marking), a flag with 0x400 replaces the copied one
 __global__ void sort_gather_kernel(const uint8_t *__restrict__ in, const int64_t *__restrict__ starts, const uint32_t *__restrict__ ord,
-                                   const int64_t *__restrict__ offs, const int64_t *__restrict__ len, int64_t n, int64_t base, uint8_t *out) {
+                                   const int64_t *__restrict__ offs, const int64_t *__restrict__ len, int64_t n, int64_t base, uint8_t *out,
+                                   const bm2_sort_rec *__restrict__ info_sorted) {
     const int64_t w = ((int64_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
     if (w >= n) return;
@@ -75,23 +83,31 @@ __global__ void sort_gather_kernel(const uint8_t *__restrict__ in, const int64_t
     uint4 *d4 = (uint4 *) (d + head);
     for (int64_t k = lane; k < body / 16; k += 32) d4[k] = s4[k];
     for (int64_t k = head + body + lane; k < m; k += 32) d[k] = s[k];
+    if (info_sorted) {
+        const uint16_t f = info_sorted[w].flag;
+        __syncwarp();
+        if (lane == 0 && (f & 0x400)) { d[18] = (uint8_t) f; d[19] = (uint8_t) (f >> 8); }
+    }
 }
 
-enum { SD_IN, SD_STARTS, SD_INFO, SD_LEN, SD_KEYS0, SD_KEYS1, SD_VALS0, SD_VALS1, SD_LENS, SD_OFFS, SD_TEMP, SD_OUT, SD_SINFO, SD_MAX };
-static_assert(SD_MAX + 1 <= (int) (sizeof(((bm2_ctx *) nullptr)->sort_d) / sizeof(DevBuf)), "sort buffers");
+enum { SD_IN, SD_STARTS, SD_INFO, SD_LEN, SD_KEYS0, SD_KEYS1, SD_VALS0, SD_VALS1, SD_LENS, SD_OFFS, SD_TEMP, SD_OUT, SD_SINFO, SD_MAX, SD_TIDS,
+       SD_STIDS, SD_END };
+static_assert(SD_END <= (int) (sizeof(((bm2_ctx *) nullptr)->sort_d) / sizeof(DevBuf)), "sort buffers");
 
 int bits_of(uint64_t v) { int b = 0; while (v >> b) ++b; return b; }
 
 }  // namespace
 
-extern "C" int bm2_bam_sort_compress(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int64_t *starts, int64_t n_recs, const uint8_t *carry,
-                                     int64_t carry_len, int last, bm2_sort_out *out) {
+// bm2_bam_sort_compress and bm2_bam_sort_compress_ex: tids (may be NULL) carried into ctx->sort_tids; marking when tids and a bitset are there
+static int sort_compress(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int64_t *starts, int64_t n_recs, const int64_t *tids, const uint8_t *carry,
+                         int64_t carry_len, int last, bm2_sort_out *out) {
     bm2_ctx *ctx_for_error = ctx;
     if (!ctx || !out || n < 0 || (n && !recs) || n_recs < 0 || (n_recs && !starts) || carry_len < 0 || carry_len >= BGZF_BLOCK ||
         (carry_len && !carry)) {
         if (ctx) bm2_set_error(ctx, "bm2_bam_sort_compress: bad arguments");
         return 1;
     }
+    const bool mark = tids && ctx->dup_n_bits > 0;
     if (n_recs >= (1LL << 31) - 1) { bm2_set_error(ctx, "bm2_bam_sort_compress: 2^31-1 records or more in one call"); return 1; }
     for (int64_t i = 0; i < n_recs; ++i) {                       // each record whole inside the buffer, in order, not overlapping the next
         const int64_t s = starts[i];
@@ -125,6 +141,9 @@ extern "C" int bm2_bam_sort_compress(bm2_ctx *ctx, const uint8_t *recs, int64_t 
         ctx->ensure(b[SD_OUT], (size_t) (carry_len + n) + 16) || ctx->ensure(b[SD_SINFO], (size_t) nr * sizeof(bm2_sort_rec) + 8) ||
         ctx->ensure(b[SD_MAX], 16) || ctx->ensure_host(ctx->sort_h[0], (size_t) nr * 8 + 16) ||
         ctx->ensure_host(ctx->sort_h[1], (size_t) nr * sizeof(bm2_sort_rec) + 16)) return 1;
+    if (tids && (ctx->ensure(b[SD_TIDS], (size_t) nr * 8 + 8) || ctx->ensure(b[SD_STIDS], (size_t) nr * 8 + 8))) return 1;
+    int64_t *d_tids = tids ? (int64_t *) b[SD_TIDS].p : nullptr, *d_stids = tids ? (int64_t *) b[SD_STIDS].p : nullptr;
+    ctx->sort_tids.resize(tids ? (size_t) nr : 0);
     for (cudaEvent_t &ev : ctx->sort_ev) if (!ev) BM2_CUDA_OK(cudaEventCreate(&ev));
     if (carry_len) BM2_CUDA_OK(cudaMemcpy(b[SD_OUT].p, carry, (size_t) carry_len, cudaMemcpyHostToDevice));   // carry may be this context's last carry
     int64_t *h_offs = (int64_t *) ctx->sort_h[0].p;
@@ -134,10 +153,12 @@ extern "C" int bm2_bam_sort_compress(bm2_ctx *ctx, const uint8_t *recs, int64_t 
         BM2_CUDA_OK(cudaMemcpyAsync(b[SD_IN].p, recs, (size_t) n, cudaMemcpyHostToDevice, st));
         BM2_CUDA_OK(cudaMemcpyAsync(b[SD_STARTS].p, starts, (size_t) nr * 8, cudaMemcpyHostToDevice, st));
         BM2_CUDA_OK(cudaMemsetAsync(b[SD_MAX].p, 0, 8, st));
+        if (tids) BM2_CUDA_OK(cudaMemcpyAsync(d_tids, tids, (size_t) nr * 8, cudaMemcpyHostToDevice, st));
         const unsigned g = (unsigned) ((nr + 255) / 256), g1 = (unsigned) ((nr + 256) / 256);
         BM2_CUDA_OK(cudaEventRecord(ctx->sort_ev[0], st));
         sort_key_kernel<<<g, 256, 0, st>>>((const uint8_t *) b[SD_IN].p, (const int64_t *) b[SD_STARTS].p, nr, (bm2_sort_rec *) b[SD_INFO].p,
-                                           (int64_t *) b[SD_LEN].p, (unsigned *) b[SD_MAX].p);
+                                           (int64_t *) b[SD_LEN].p, (unsigned *) b[SD_MAX].p, d_tids,
+                                           mark ? (const uint64_t *) ctx->dup_bits.p : nullptr, ctx->dup_n_bits);
         BM2_CUDA_OK(cudaGetLastError());
         BM2_CUDA_OK(cudaEventRecord(ctx->sort_ev[1], st));
         unsigned mx[2] = { 0, 0 };
@@ -154,17 +175,19 @@ extern "C" int bm2_bam_sort_compress(bm2_ctx *ctx, const uint8_t *recs, int64_t 
         ord = vb.Current();
         BM2_CUDA_OK(cudaEventRecord(ctx->sort_ev[2], st));
         sort_permute_kernel<<<g1, 256, 0, st>>>(ord, nr, (const int64_t *) b[SD_LEN].p, (const bm2_sort_rec *) b[SD_INFO].p, (int64_t *) b[SD_LENS].p,
-                                                (bm2_sort_rec *) b[SD_SINFO].p);
+                                                (bm2_sort_rec *) b[SD_SINFO].p, d_tids, d_stids);
         BM2_CUDA_OK(cudaGetLastError());
         tb = b[SD_TEMP].cap;
         BM2_CUDA_OK(cub::DeviceScan::ExclusiveSum(b[SD_TEMP].p, tb, (const int64_t *) b[SD_LENS].p, (int64_t *) b[SD_OFFS].p, (int) nr + 1, st));
         sort_gather_kernel<<<(unsigned) ((nr * 32 + 255) / 256), 256, 0, st>>>((const uint8_t *) b[SD_IN].p, (const int64_t *) b[SD_STARTS].p, ord,
                                                                                (const int64_t *) b[SD_OFFS].p, (const int64_t *) b[SD_LENS].p, nr,
-                                                                               carry_len, (uint8_t *) b[SD_OUT].p);
+                                                                               carry_len, (uint8_t *) b[SD_OUT].p,
+                                                                               mark ? (const bm2_sort_rec *) b[SD_SINFO].p : nullptr);
         BM2_CUDA_OK(cudaGetLastError());
         BM2_CUDA_OK(cudaEventRecord(ctx->sort_ev[3], st));
         BM2_CUDA_OK(cudaMemcpyAsync(h_offs, b[SD_OFFS].p, (size_t) (nr + 1) * 8, cudaMemcpyDeviceToHost, st));
         BM2_CUDA_OK(cudaMemcpyAsync(h_info, b[SD_SINFO].p, (size_t) nr * sizeof(bm2_sort_rec), cudaMemcpyDeviceToHost, st));
+        if (tids) BM2_CUDA_OK(cudaMemcpyAsync(ctx->sort_tids.data(), d_stids, (size_t) nr * 8, cudaMemcpyDeviceToHost, st));
         BM2_CUDA_OK(cudaStreamSynchronize(st));
         float ms[3] = { 0, 0, 0 };
         for (int k = 0; k < 3; ++k) BM2_CUDA_OK(cudaEventElapsedTime(&ms[k], ctx->sort_ev[k], ctx->sort_ev[k + 1]));
@@ -189,6 +212,18 @@ extern "C" int bm2_bam_sort_compress(bm2_ctx *ctx, const uint8_t *recs, int64_t 
     return 0;
 }
 
+extern "C" int bm2_bam_sort_compress(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int64_t *starts, int64_t n_recs, const uint8_t *carry,
+                                     int64_t carry_len, int last, bm2_sort_out *out) {
+    return sort_compress(ctx, recs, n, starts, n_recs, nullptr, carry, carry_len, last, out);
+}
+
+extern "C" int bm2_bam_sort_compress_ex(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int64_t *starts, int64_t n_recs, const int64_t *tids,
+                                        const uint8_t *carry, int64_t carry_len, int last, bm2_sort_out *out, const int64_t **tids_out) {
+    if (sort_compress(ctx, recs, n, starts, n_recs, tids, carry, carry_len, last, out)) return 1;
+    if (tids_out) *tids_out = tids ? ctx->sort_tids.data() : nullptr;
+    return 0;
+}
+
 extern "C" int bm2_last_sort_stats(const bm2_ctx *ctx, double ms[4]) {
     if (!ctx || !ms) return 1;
     for (int k = 0; k < 4; ++k) ms[k] = ctx->sort_ms[k];
@@ -196,13 +231,17 @@ extern "C" int bm2_last_sort_stats(const bm2_ctx *ctx, double ms[4]) {
 }
 
 extern "C" int bm2_bam_sort_memory(const bm2_ctx *ctx, int64_t run_bytes, int64_t *needed, int64_t *free_bytes) {
+    return bm2_bam_sort_memory_ex(ctx, run_bytes, 0, needed, free_bytes);
+}
+
+extern "C" int bm2_bam_sort_memory_ex(const bm2_ctx *ctx, int64_t run_bytes, int with_tids, int64_t *needed, int64_t *free_bytes) {
     if (!ctx || run_bytes < 0 || !needed || !free_bytes) return 1;
     bm2_ctx *ctx_for_error = (bm2_ctx *) ctx;
     // what the buffers of one call ask for, each rounded up by 1.25 as bm2_ctx::ensure allocates: records in (reused for the compressed
     // members), the sorted stream, the BGZF slots (one 64 KiB slot per 65280-byte block), and 120 bytes per record of keys, ordinals, lengths,
     // offsets and index data (twice for the radix sort's double buffers)
     const double r = (double) run_bytes, recs = r / kRecBytes + 1;
-    const double bytes = 1.25 * (r + (r + BGZF_BLOCK) + (r / BGZF_BLOCK + 2) * BGZF_MAX_MEMBER + 120 * recs) + 64.0 * (1 << 20);
+    const double bytes = 1.25 * (r + (r + BGZF_BLOCK) + (r / BGZF_BLOCK + 2) * BGZF_MAX_MEMBER + (with_tids ? 136 : 120) * recs) + 64.0 * (1 << 20);
     size_t fr = 0, tot = 0;
     BM2_CUDA_OK(cudaSetDevice(ctx->device));
     BM2_CUDA_OK(cudaMemGetInfo(&fr, &tot));

@@ -14,9 +14,21 @@
 //           before when that one ends where it starts; the 16 kbp linear index, empty windows filled from the one before; pseudo-bin 37450
 //           with the reference's offset span and its mapped / unmapped counts; n_no_coor.
 //
-// The device call is a parameter, so that tests/host_emul/bam_sort_emul.cpp runs all of this with the GPU swapped for a CPU restatement.
+//   markdup (--markdup, markdup_device.cuh's rule) each record comes with its template's id, and each chunk with its templates' entries.
+//           The ids travel with the records: a spilled run writes its ids in sorted order to a second temporary file (8 bytes per record,
+//           opened and unlinked the same way), and the merge reads them in step.  The entries are held up to sig_bytes (--sort-mem / 8, a
+//           chosen figure, not a measured one), half of it filling while the sorter thread sorts the other half on the device and spills it
+//           as a sorted run.  At finish, with the last record run spilled, the duplicates are resolved: in one call per space when nothing
+//           spilled, else window by window over the sorted runs of each space, with the record merge's settle rule except that only keys
+//           strictly below T are settled, so that every group is resolved whole (a group larger than a window grows the window: host memory
+//           then grows by one entry per member of the largest group).  The duplicate templates become a bitset of 1 bit per input read,
+//           uploaded to the sort context before the one-run sort or the first merge window, which set 0x400 on their records.
+//
+// The device calls are parameters, so that tests/host_emul/bam_sort_emul.cpp and markdup_emul.cpp run all of this with the GPU swapped for a
+// CPU restatement.
 #pragma once
 #include "bam_sort_device.cuh"
+#include "markdup_device.cuh"
 #include <algorithm>
 #include <atomic>
 #include <chrono>
@@ -33,6 +45,14 @@
 // one buffer of records sorted and compressed (bm2_bam_sort_compress's arguments); device_s: its device time.  Returns 0 on success.
 using SortCall = std::function<int(const uint8_t *recs, int64_t n, const int64_t *starts, int64_t n_recs, const uint8_t *carry, int64_t carry_len,
                                    int last, bm2_sort_out *out, double *device_s)>;
+// the same with one template id per record (tids, may be null) carried through the sort (bm2_bam_sort_compress_ex): *tids_out gets them sorted
+using SortCallEx = std::function<int(const uint8_t *recs, int64_t n, const int64_t *starts, int64_t n_recs, const int64_t *tids, const uint8_t *carry,
+                                     int64_t carry_len, int last, bm2_sort_out *out, const int64_t **tids_out, double *device_s)>;
+// the entries of one duplicate space sorted (resolve 0) or resolved into the duplicates' template ids (bm2_dup_resolve's arguments)
+using DupCall = std::function<int(const bm2_dup_entry *e, int64_t n, int resolve, const bm2_dup_entry **sorted, const int64_t **dups, int64_t *n_dups,
+                                  double *device_s)>;
+// the duplicate bitset to the sort context (bm2_dup_set)
+using DupSetCall = std::function<int(const uint64_t *bits, int64_t n_bits)>;
 // reports an error and does not return
 using SortFail = std::function<void(const std::string &)>;
 
@@ -92,15 +112,22 @@ struct BaiBuilder {
 
 // the sorted stream's writer: each call's members go to the file, each record's virtual offset to the index
 struct SortedWriter {
-    SortCall sort; SortFail fail; FILE *out = nullptr; BaiBuilder *bai = nullptr;
+    SortCallEx sort; SortFail fail; FILE *out = nullptr; BaiBuilder *bai = nullptr;
     uint64_t file_off = 0;                       // compressed bytes before the next member
     std::vector<uint8_t> carry;
     double device_s = 0;
-    void write(const uint8_t *recs, int64_t n, const int64_t *starts, int64_t n_recs, bool last) {
+    int64_t marked = 0;                          // records written with 0x400
+    // tids: the records' template ids or null; tids_out: where their sorted ids go, or null
+    void write(const uint8_t *recs, int64_t n, const int64_t *starts, int64_t n_recs, const int64_t *tids, bool last,
+               std::vector<int64_t> *tids_out = nullptr) {
         bm2_sort_out o;
         double ds = 0;
-        if (sort(recs, n, starts, n_recs, carry.data(), (int64_t) carry.size(), last ? 1 : 0, &o, &ds)) fail("bm2_bam_sort_compress");
+        const int64_t *ts = nullptr;
+        if (sort(recs, n, starts, n_recs, tids, carry.data(), (int64_t) carry.size(), last ? 1 : 0, &o, tids ? &ts : nullptr, &ds))
+            fail("bm2_bam_sort_compress");
         device_s += ds;
+        if (tids_out) tids_out->assign(ts, ts + (ts ? n_recs : 0));
+        for (int64_t i = 0; i < o.n_recs; ++i) marked += (o.recs[i].flag & 0x400) != 0;
         if (o.z_len && fwrite(o.z, 1, (size_t) o.z_len, out) != (size_t) o.z_len) fail("cannot write the sorted BAM");
         if (bai) {
             std::vector<uint64_t> addr((size_t) o.n_members + 1, file_off);
@@ -114,42 +141,109 @@ struct SortedWriter {
 };
 
 struct BamSortSink {
-    struct Run { FILE *f = nullptr; std::vector<int32_t> members; };
+    struct Run { FILE *f = nullptr, *tf = nullptr; std::vector<int32_t> members; };
+    struct SigRun { FILE *f = nullptr; int64_t n = 0; };
     // settings
     SortCall sort; SortFail fail;
+    SortCallEx sort_ex;                          // when set, used instead of sort
+    DupCall dup; DupSetCall dup_set;             // --markdup when dup is set (sort_ex must be set then)
     int64_t run_bytes = (int64_t) 2 << 30;
-    std::string tmp_prefix;                      // runs go to <tmp_prefix>NNNN
+    int64_t sig_bytes = (int64_t) 256 << 20;     // entries held on the host (--sort-mem / 8)
+    int64_t n_reads = 0;                         // the duplicate bitset's bits: set before finish
+    std::string tmp_prefix;                      // runs go to <tmp_prefix>NNNN (their ids to <tmp_prefix>NNNN.id), signature runs to <tmp_prefix>dNNNN
     int threads = 1;
     // state
-    std::vector<uint8_t> cur; std::vector<int64_t> cur_starts;
-    std::vector<uint8_t> pend; std::vector<int64_t> pend_starts;
+    std::vector<uint8_t> cur; std::vector<int64_t> cur_starts, cur_tids;
+    std::vector<uint8_t> pend; std::vector<int64_t> pend_starts, pend_tids;
     std::thread sorter;
     std::vector<Run> runs;
+    std::vector<bm2_dup_entry> sig_cur[2], sig_pend[2];   // [0] pair space, [1] fragment space
+    std::vector<SigRun> sig_runs[2];
     // stats
-    double sort_s = 0, merge_s = 0;
+    double sort_s = 0, merge_s = 0, markdup_s = 0;
     int64_t spill_bytes = 0, merge_windows = 0;
+    int64_t dup_templates = 0, dup_pair_templates = 0, dup_frag_templates = 0, dup_records = 0, dup_sig_runs = 0, dup_sig_bytes = 0;
 
-    ~BamSortSink() { if (sorter.joinable()) sorter.join(); for (Run &r : runs) if (r.f) fclose(r.f); }
+    ~BamSortSink() {
+        if (sorter.joinable()) sorter.join();
+        for (Run &r : runs) { if (r.f) fclose(r.f); if (r.tf) fclose(r.tf); }
+        for (auto &v : sig_runs) for (SigRun &r : v) if (r.f) fclose(r.f);
+    }
 
-    // the records of one chunk, in output order
-    void add(const uint8_t *p, int64_t len) {
-        for (int64_t q = 0; q + 4 <= len;) {
+    SortCallEx call() const {
+        if (sort_ex) return sort_ex;
+        SortCall s = sort;
+        return [s](const uint8_t *r, int64_t n, const int64_t *st, int64_t nr, const int64_t *, const uint8_t *c, int64_t cl, int last, bm2_sort_out *o,
+                   const int64_t **tids_out, double *ds) {
+            if (tids_out) *tids_out = nullptr;
+            return s(r, n, st, nr, c, cl, last, o, ds);
+        };
+    }
+
+    // the records of one chunk, in output order; with --markdup, tids: each record's template id
+    void add(const uint8_t *p, int64_t len, const int64_t *tids = nullptr) {
+        int64_t k = 0;
+        for (int64_t q = 0; q + 4 <= len; ++k) {
             int32_t bs; memcpy(&bs, p + q, 4);
             const int64_t m = 4 + (int64_t) bs;
             if (bs < 32 || q + m > len) fail("a malformed BAM record");
             if (!cur_starts.empty() && (int64_t) cur.size() + m > run_bytes) hand_off();
             cur_starts.push_back((int64_t) cur.size());
             cur.insert(cur.end(), p + q, p + q + m);
+            if (dup) cur_tids.push_back(tids ? tids[k] : -1);
             q += m;
         }
+    }
+
+    // the entries of one chunk's templates (bm2_dup_signatures), in chunk order
+    void add_sigs(const bm2_dup_entry *pairs, int64_t n_pairs, const bm2_dup_entry *frags, int64_t n_frags) {
+        dup_templates += n_pairs;
+        for (int64_t i = 0; i < n_frags; ++i) dup_templates += frags[i].kind == 1;
+        sig_cur[0].insert(sig_cur[0].end(), pairs, pairs + n_pairs);
+        sig_cur[1].insert(sig_cur[1].end(), frags, frags + n_frags);
+        if ((int64_t) ((sig_cur[0].size() + sig_cur[1].size()) * sizeof(bm2_dup_entry)) > sig_bytes / 2) {
+            if (sorter.joinable()) sorter.join();
+            for (int s = 0; s < 2; ++s) { sig_pend[s].swap(sig_cur[s]); sig_cur[s].clear(); }
+            sorter = std::thread([this] { spill_sigs(); });
+        }
+    }
+
+    // the pending entries, sorted on the device, as one more signature run of each space
+    void spill_sigs() {
+        for (int s = 0; s < 2; ++s) {
+            std::vector<bm2_dup_entry> &v = sig_pend[s];
+            if (v.empty()) continue;
+            char name[32];
+            snprintf(name, sizeof name, "d%04d", (int) (sig_runs[0].size() + sig_runs[1].size()));
+            const std::string path = tmp_prefix + name;
+            SigRun r;
+            r.f = open_tmp(path, fail);
+            const bm2_dup_entry *sorted = nullptr; double ds = 0;
+            if (dup(v.data(), (int64_t) v.size(), 0, &sorted, nullptr, nullptr, &ds)) fail("bm2_dup_resolve");
+            markdup_s += ds;
+            if (fwrite(sorted, sizeof(bm2_dup_entry), v.size(), r.f) != v.size() || fflush(r.f) || fseek(r.f, 0, SEEK_SET))
+                fail("cannot write the temporary file " + path);
+            r.n = (int64_t) v.size();
+            dup_sig_bytes += r.n * (int64_t) sizeof(bm2_dup_entry);
+            sig_runs[s].push_back(r);
+            std::vector<bm2_dup_entry>().swap(v);
+        }
+        ++dup_sig_runs;
     }
 
     // the current run to the sorter thread, once the one before is on disk
     void hand_off() {
         if (sorter.joinable()) sorter.join();
-        pend.swap(cur); pend_starts.swap(cur_starts);
-        cur.clear(); cur_starts.clear();
+        pend.swap(cur); pend_starts.swap(cur_starts); pend_tids.swap(cur_tids);
+        cur.clear(); cur_starts.clear(); cur_tids.clear();
         sorter = std::thread([this] { spill(); });
+    }
+
+    static FILE *open_tmp(const std::string &path, const SortFail &fail) {
+        FILE *f = fopen(path.c_str(), "w+b");
+        if (!f) fail("cannot create the temporary file " + path);
+        unlink(path.c_str());
+        return f;
     }
 
     void spill() {
@@ -157,12 +251,19 @@ struct BamSortSink {
         snprintf(name, sizeof name, "%04d", (int) runs.size());
         const std::string path = tmp_prefix + name;
         Run r;
-        r.f = fopen(path.c_str(), "w+b");
-        if (!r.f) fail("cannot create the temporary file " + path);
-        unlink(path.c_str());
-        SortedWriter w{sort, fail, r.f, nullptr};
-        w.write(pend.data(), (int64_t) pend.size(), pend_starts.data(), (int64_t) pend_starts.size(), true);
+        r.f = open_tmp(path, fail);
+        SortedWriter w{call(), fail, r.f, nullptr};
+        std::vector<int64_t> ids;
+        w.write(pend.data(), (int64_t) pend.size(), pend_starts.data(), (int64_t) pend_starts.size(), dup ? pend_tids.data() : nullptr, true,
+                dup ? &ids : nullptr);
         sort_s += w.device_s;
+        if (dup) {                                // the ids in sorted order, 8 bytes per record
+            r.tf = open_tmp(path + ".id", fail);
+            if (fwrite(ids.data(), 8, ids.size(), r.tf) != ids.size() || fflush(r.tf) || fseek(r.tf, 0, SEEK_SET))
+                fail("cannot write the temporary file " + path + ".id");
+            spill_bytes += (int64_t) ids.size() * 8;
+            std::vector<int64_t>().swap(pend_tids);
+        }
         // the members' sizes, from their BSIZE fields, read back as the merge will read them
         if (fflush(r.f) || fseek(r.f, 0, SEEK_SET)) fail("cannot write the temporary file " + path);
         spill_bytes += (int64_t) w.file_off;
@@ -181,21 +282,88 @@ struct BamSortSink {
 
     // everything has been added: the sorted records to out (its compressed offset now: out_off), the index to bai when not null
     void finish(FILE *out, uint64_t out_off, BaiBuilder *bai) {
-        SortedWriter w{sort, fail, out, bai, out_off};
-        if (!sorter.joinable() && runs.empty()) {
-            w.write(cur.data(), (int64_t) cur.size(), cur_starts.data(), (int64_t) cur_starts.size(), true);
+        SortedWriter w{call(), fail, out, bai, out_off};
+        if (sorter.joinable()) sorter.join();
+        const bool one_run = runs.empty();
+        if (!one_run && !cur_starts.empty()) { hand_off(); sorter.join(); }
+        if (dup) resolve();
+        if (one_run) {
+            w.write(cur.data(), (int64_t) cur.size(), cur_starts.data(), (int64_t) cur_starts.size(), dup ? cur_tids.data() : nullptr, true);
             sort_s += w.device_s;
-            return;
+        } else merge(w);
+        dup_records = w.marked;
+    }
+
+    static bool key_less(const bm2_dup_entry &a, const bm2_dup_entry &b) { return a.k1 != b.k1 ? a.k1 < b.k1 : a.k2 < b.k2; }
+
+    // every duplicate template of both spaces, as the bitset given to dup_set
+    void resolve() {
+        std::vector<uint64_t> bits((size_t) ((n_reads + 63) / 64), 0);
+        const bool spilled = dup_sig_runs > 0;
+        if (spilled && (!sig_cur[0].empty() || !sig_cur[1].empty())) {
+            for (int s = 0; s < 2; ++s) { sig_pend[s].swap(sig_cur[s]); sig_cur[s].clear(); }
+            spill_sigs();
         }
-        if (!cur_starts.empty()) hand_off();
-        sorter.join();
-        merge(w);
+        for (int s = 0; s < 2; ++s) {
+            int64_t &count = s ? dup_frag_templates : dup_pair_templates;
+            auto take = [&](const std::vector<bm2_dup_entry> &v) {
+                const int64_t *d = nullptr; int64_t nd = 0; double ds = 0;
+                if (dup(v.data(), (int64_t) v.size(), 1, nullptr, &d, &nd, &ds)) fail("bm2_dup_resolve");
+                markdup_s += ds;
+                for (int64_t i = 0; i < nd; ++i) {
+                    if (d[i] < 0 || d[i] >= n_reads) fail("a duplicate template id beyond the reads");
+                    bits[(size_t) (d[i] >> 6)] |= (uint64_t) 1 << (d[i] & 63);
+                }
+                count += nd;
+            };
+            if (!spilled) { take(sig_cur[s]); std::vector<bm2_dup_entry>().swap(sig_cur[s]); continue; }
+            // the sorted runs window by window: keys strictly below T settle, so every group is resolved whole
+            std::vector<SigRun> &rs = sig_runs[s];
+            const size_t nr = rs.size();
+            if (!nr) continue;
+            const int64_t quota = std::max<int64_t>(sig_bytes / (int64_t) sizeof(bm2_dup_entry) / (int64_t) nr, 1);
+            std::vector<std::vector<bm2_dup_entry>> buf(nr);
+            std::vector<int64_t> left(nr);
+            for (size_t r = 0; r < nr; ++r) left[r] = rs[r].n;
+            auto load = [&](size_t r, int64_t k) {
+                k = std::min(k, left[r]);
+                if (k <= 0) return;
+                const size_t at = buf[r].size();
+                buf[r].resize(at + (size_t) k);
+                if (fread(buf[r].data() + at, sizeof(bm2_dup_entry), (size_t) k, rs[r].f) != (size_t) k) fail("cannot read a temporary file");
+                left[r] -= k;
+            };
+            std::vector<bm2_dup_entry> win;
+            for (bool grow = false;;) {
+                for (size_t r = 0; r < nr; ++r) if (!grow) load(r, quota - (int64_t) buf[r].size());
+                grow = false;
+                bool open = false; bm2_dup_entry T{};
+                for (size_t r = 0; r < nr; ++r)
+                    if (left[r] > 0 && (!open || key_less(buf[r].back(), T))) { T = buf[r].back(); open = true; }
+                win.clear();
+                for (size_t r = 0; r < nr; ++r) {
+                    size_t k = 0;
+                    while (k < buf[r].size() && (!open || key_less(buf[r][k], T))) ++k;
+                    win.insert(win.end(), buf[r].begin(), buf[r].begin() + (long) k);
+                    buf[r].erase(buf[r].begin(), buf[r].begin() + (long) k);
+                }
+                if (open && win.empty()) {               // one group fills the window: load more of the runs that end in it
+                    for (size_t r = 0; r < nr; ++r) if (left[r] > 0 && !key_less(T, buf[r].back())) load(r, quota);
+                    grow = true;
+                    continue;
+                }
+                if (!win.empty()) take(win);
+                if (!open) break;
+            }
+        }
+        if (dup_set(bits.data(), n_reads)) fail("bm2_dup_set");
     }
 
     struct Cursor {                              // a run being merged
         size_t next = 0;                          // next member to load
         std::vector<uint8_t> buf; size_t pos = 0; // loaded bytes, consumed up to pos
         std::vector<size_t> recs;                 // whole records at buf[pos..]: their starts
+        std::vector<int64_t> tids;                // --markdup: their template ids
     };
 
     static uint64_t key_at(const uint8_t *r) { const BamFixed f = bam_fixed(r); return bam_coord_key(f.rid, f.pos, f.flag); }
@@ -205,7 +373,7 @@ struct BamSortSink {
         const size_t nr = runs.size();
         const int64_t quota = std::max<int64_t>(run_bytes / (int64_t) nr, BGZF_BLOCK);
         std::vector<Cursor> c(nr);
-        std::vector<uint8_t> win; std::vector<int64_t> win_starts;
+        std::vector<uint8_t> win; std::vector<int64_t> win_starts, win_tids;
         for (;;) {
             for (int round = 0;; ++round) {               // load until every unfinished run holds a quota and at least one whole record
                 struct Job { size_t run; std::vector<uint8_t> z; size_t at; uint32_t isize; };
@@ -253,6 +421,11 @@ struct BamSortSink {
                     while (q + 4 <= x.buf.size() && q + 4 + (size_t) bam_le32(x.buf.data() + q) <= x.buf.size()) {
                         x.recs.push_back(q); q += 4 + (size_t) bam_le32(x.buf.data() + q);
                     }
+                    if (dup && x.tids.size() < x.recs.size()) {                       // their ids, read in step
+                        const size_t at = x.tids.size();
+                        x.tids.resize(x.recs.size());
+                        if (fread(x.tids.data() + at, 8, x.tids.size() - at, runs[r].tf) != x.tids.size() - at) fail("cannot read a temporary file");
+                    }
                 }
             }
             // T and r* over the runs not fully loaded
@@ -262,7 +435,7 @@ struct BamSortSink {
                 const uint64_t k = key_at(c[r].buf.data() + c[r].recs.back());
                 if (!open || k < T) { T = k; rs = r; open = true; }
             }
-            win.clear(); win_starts.clear();
+            win.clear(); win_starts.clear(); win_tids.clear();
             for (size_t r = 0; r < nr; ++r) {
                 Cursor &x = c[r];
                 size_t k = 0;
@@ -276,9 +449,10 @@ struct BamSortSink {
                 for (size_t i = 0; i < k; ++i) win_starts.push_back((int64_t) (win.size() + x.recs[i] - b));
                 win.insert(win.end(), x.buf.begin() + (long) b, x.buf.begin() + (long) e);
                 x.recs.erase(x.recs.begin(), x.recs.begin() + (long) k);
+                if (dup) { win_tids.insert(win_tids.end(), x.tids.begin(), x.tids.begin() + (long) k); x.tids.erase(x.tids.begin(), x.tids.begin() + (long) k); }
                 x.pos = e;
             }
-            w.write(win.data(), (int64_t) win.size(), win_starts.data(), (int64_t) win_starts.size(), !open);
+            w.write(win.data(), (int64_t) win.size(), win_starts.data(), (int64_t) win_starts.size(), dup ? win_tids.data() : nullptr, !open);
             ++merge_windows;
             if (!open) break;
         }

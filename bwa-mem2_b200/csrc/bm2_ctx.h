@@ -66,20 +66,30 @@ struct bm2_ctx {
     int64_t bgzf_members = 0;
     std::vector<int32_t> bgzf_sizes;       // the last call's member sizes
     // bm2_bam_sort_compress (bam_sort.cu): buffers, events around its stages, the last call's device times and outputs
-    DevBuf sort_d[14];
+    DevBuf sort_d[16];
     HostBuf sort_h[2];
     cudaEvent_t sort_ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
     double sort_ms[4] = {0, 0, 0, 0};
     std::vector<uint8_t> sort_carry;
     std::vector<bm2_sort_rec> sort_recs;
+    std::vector<int64_t> sort_tids;        // bm2_bam_sort_compress_ex: the template ids in output order
+    // bm2_dup_signatures / bm2_dup_resolve / bm2_dup_set (markdup.cu): buffers, events, the last calls' device times and outputs, the bitset
+    DevBuf dup_d[14];
+    DevBuf dup_bits;
+    int64_t dup_n_bits = 0;
+    cudaEvent_t dup_ev[4] = {nullptr, nullptr, nullptr, nullptr};
+    double dup_sig_ms = 0, dup_resolve_ms = 0;
+    std::vector<bm2_dup_entry> dup_pairs, dup_frags, dup_sorted;
+    std::vector<int64_t> dup_ids;
 
     int ensure(DevBuf &b, size_t bytes);
     int ensure_host(HostBuf &b, size_t bytes);
     std::vector<DevBuf *> all_dev() {
-        std::vector<DevBuf *> v = {&io_pairs, &io_ref, &io_qer, &bsw_jobs, &bsw_outs, &bsw_scratch};
+        std::vector<DevBuf *> v = {&io_pairs, &io_ref, &io_qer, &bsw_jobs, &bsw_outs, &bsw_scratch, &dup_bits};
         for (auto &x : d) v.push_back(&x);
         for (auto &x : bgzf_d) v.push_back(&x);
         for (auto &x : sort_d) v.push_back(&x);
+        for (auto &x : dup_d) v.push_back(&x);
         return v;
     }
     std::vector<HostBuf *> all_host() { std::vector<HostBuf *> v; for (auto &x : h) v.push_back(&x); for (auto &x : bgzf_h) v.push_back(&x); for (auto &x : sort_h) v.push_back(&x); return v; }

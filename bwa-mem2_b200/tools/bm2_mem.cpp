@@ -20,7 +20,9 @@
 //   bm2_sam_pe / bm2_sam_se       worker_sam's arithmetic                                             (src/bwamem.cpp:1262-1336)
 //   bm2_sam_format_ex             mem_aln2sam's text with RG / the -C comment / XR                    (src/bwamem.cpp:1592-1730)
 //     or bm2_bam_format_ex        --bam: the same records as BAM, then bm2_bgzf_compress: BGZF members compressed on the GPU
-//        then bm2_bam_sort_compress  --sort: the records in sorted runs, merged, compressed on the GPU, and the BAI (bam_sort.h)
+//        then bm2_bam_sort_compress_ex  --sort: the records in sorted runs, merged, compressed on the GPU, and the BAI (bam_sort.h)
+//        with bm2_dup_signatures     --markdup: each chunk's templates' entries, resolved by bm2_dup_resolve at the end; the duplicates' records get
+//                                    0x400 in the same sort, which then carries each record's template id (bam_sort.h, markdup_device.cuh)
 // Chunks in flight: the reference's kt_pipeline runs its three steps (read, process, write) on two worker threads so that one chunk's I/O
 // overlaps another's computation (src/fastmap.cpp:952-1003, src/kthread.cpp:122-176).  Here -p workers (default 2) each own a context
 // (bm2_create_sibling: one index in HBM) and take whole chunks off a queue; the GPU interleaves the kernels of the two chunks, the host side of
@@ -75,6 +77,7 @@ struct Shared {
     bm2_sam_text_extra extra{};                                  // -R / -C / -V
     bool copy_comment = false, bam = false;
     BamSortSink *sink = nullptr;                                 // --sort: the records go to the sorted runs instead of the output
+    bool markdup = false; double t_dup_sig = 0;                  // --markdup: device time of the signature kernels
     double t_split = 0;
     long long seq_chunks = 0;                                    // chunks that went through bm2_seq_encode
     size_t in_flight = 0;                                        // bytes of the chunks queued or being aligned
@@ -130,8 +133,10 @@ char *align_and_format(Shared *sh, bm2_ctx *ctx, const bm2_fastq_batch &fq, cons
 }
 
 // -p: the single-end set and the pairs of a chunk as the reference's two mem_process_seqs calls (src/fastmap.cpp:260-285), the reads' lines
-// (or BAM records) merged back into file order (the records of a read are consecutive)
-char *smart_pair_chunk(Shared *sh, bm2_ctx *ctx, const Chunk &ck, int n_reads, const uint8_t *qual_present, int64_t *len, Times &t) {
+// (or BAM records) merged back into file order (the records of a read are consecutive); with read_end, where each read's output ends in
+// the merged text and each read's mate (-1: none)
+char *smart_pair_chunk(Shared *sh, bm2_ctx *ctx, const Chunk &ck, int n_reads, const uint8_t *qual_present, int64_t *len, Times &t,
+                       std::vector<int64_t> *read_end = nullptr, std::vector<int64_t> *mate = nullptr) {
     const double t0 = now_s();
     bm2_fastq_split sp;
     if (bm2_fastq_smart_pair(ctx, &sp)) die("bm2_fastq_smart_pair", ctx);
@@ -156,12 +161,39 @@ char *smart_pair_chunk(Shared *sh, bm2_ctx *ctx, const Chunk &ck, int n_reads, c
         if (s < 0) die("bm2_fastq_smart_pair: a read in neither set", nullptr);
         const char *q = text[s] + ends[s][(size_t) next[s]++];
         memcpy(w, p[s], (size_t) (q - p[s])); w += q - p[s]; p[s] = q;
+        if (read_end) read_end->push_back(w - merged);
+    }
+    if (mate) {
+        mate->assign((size_t) n_reads, -1);
+        for (int j = 0; j + 1 < sp.set[1].n_reads; j += 2) {
+            const int a = sp.read_index[1][j], b = sp.read_index[1][j + 1];
+            (*mate)[(size_t) a] = b; (*mate)[(size_t) b] = a;
+        }
     }
     *w = 0; *len = w - merged;
     bm2_free(text[0]); bm2_free(text[1]);
     std::lock_guard<std::mutex> lk(sh->mu);
     sh->t_split += t_split;
     return merged;
+}
+
+// --markdup: a chunk's templates (a read, or a read and its mate, which follows it) as record ranges from where each read's records end
+// (read_end), each template's id (the global index of its first read) and each record's
+struct ChunkTemplates { std::vector<int64_t> starts, first, id, rec_id; };
+void chunk_templates(const char *text, int64_t len, const std::vector<int64_t> &read_end, const std::vector<int64_t> &mate, long long first_read,
+                     ChunkTemplates &T) {
+    for (int64_t q = 0; q + 4 <= len; q += 4 + *(const int32_t *) (text + q)) T.starts.push_back(q);
+    size_t k = 0;
+    for (size_t i = 0; i < read_end.size(); ++i) {
+        const int64_t m = mate.empty() ? -1 : mate[i];
+        if (m >= 0 && (size_t) m < i) continue;
+        if (m >= 0 && (size_t) m != i + 1) die("--markdup: the mates of a pair are not adjacent in the output", nullptr);
+        const int64_t id = first_read + (long long) i, end = read_end[m >= 0 ? i + 1 : i];
+        T.first.push_back((int64_t) k); T.id.push_back(id);
+        for (; k < T.starts.size() && T.starts[k] < end; ++k) T.rec_id.push_back(id);
+    }
+    T.first.push_back((int64_t) k);
+    if (k != T.starts.size()) die("--markdup: records after the last read", nullptr);
 }
 
 void worker(Shared *sh, bm2_ctx *ctx) {
@@ -183,12 +215,23 @@ void worker(Shared *sh, bm2_ctx *ctx) {
         const double t1 = now_s();
         Times t;
         char *text = nullptr; int64_t len = 0;
-        if (sh->smart) text = smart_pair_chunk(sh, ctx, ck, fq.n_reads, qp, &len, t);
+        std::vector<int64_t> read_end, mate;
+        if (sh->smart) text = smart_pair_chunk(sh, ctx, ck, fq.n_reads, qp, &len, t, sh->markdup ? &read_end : nullptr, sh->markdup ? &mate : nullptr);
         else {
             const int64_t *cb = nullptr; const int32_t *cl = nullptr;
             if (sh->copy_comment && bm2_fastq_comments(ctx, &cb, &cl)) die("bm2_fastq_comments", ctx);
             text = align_and_format(sh, ctx, fq, ck.c1, sh->paired ? ck.c2 : nullptr, cb, cl, qp, sh->paired,
-                                    sh->paired ? ck.first_read >> 1 : ck.first_read, &len, nullptr, t);
+                                    sh->paired ? ck.first_read >> 1 : ck.first_read, &len, sh->markdup ? &read_end : nullptr, t);
+            if (sh->markdup && sh->paired) { mate.resize(read_end.size()); for (size_t i = 0; i < mate.size(); ++i) mate[i] = (int64_t) (i ^ 1); }
+        }
+        ChunkTemplates tpl;
+        const bm2_dup_entry *dp = nullptr, *df = nullptr; int64_t ndp = 0, ndf = 0;
+        double sig_ms = 0;
+        if (sh->markdup) {                                               // the templates' entries, on this worker's context
+            chunk_templates(text, len, read_end, mate, ck.first_read, tpl);
+            if (bm2_dup_signatures(ctx, (const uint8_t *) text, len, tpl.starts.data(), (int64_t) tpl.starts.size(), tpl.first.data(), tpl.id.data(),
+                                   (int64_t) tpl.id.size(), &dp, &ndp, &df, &ndf)) die("bm2_dup_signatures", ctx);
+            bm2_last_dup_stats(ctx, &sig_ms, nullptr);
         }
         const uint8_t *outp = (const uint8_t *) text; int64_t out_len = len;
         double bgzf_ms = 0;
@@ -205,14 +248,17 @@ void worker(Shared *sh, bm2_ctx *ctx) {
             sh->cv_turn.wait(lk, [&] { return sh->next_to_write == ck.index; });
         }
         const double t6 = now_s();
-        if (sh->sink) sh->sink->add(outp, out_len);
+        if (sh->sink) {
+            sh->sink->add(outp, out_len, sh->markdup ? tpl.rec_id.data() : nullptr);
+            if (sh->markdup) sh->sink->add_sigs(dp, ndp, df, ndf);
+        }
         else fwrite(outp, 1, (size_t) out_len, sh->out);
         bm2_free(text);
         const double t7 = now_s();
         {
             std::lock_guard<std::mutex> lk(sh->mu);
             sh->t_enc += t1 - t0; sh->t_aln += t.aln; sh->t_pes += t.pes; sh->t_sam += t.sam; sh->t_fmt += t.fmt; sh->t_turn += t6 - t5; sh->t_write += t7 - t6;
-            sh->t_bam += t.bam; sh->t_bgzf += bgzf_ms / 1e3; sh->bam_bytes += sh->bam ? len : 0; sh->bgzf_bytes += sh->bam && !sh->sink ? out_len : 0;
+            sh->t_bam += t.bam; sh->t_bgzf += bgzf_ms / 1e3; sh->t_dup_sig += sig_ms / 1e3; sh->bam_bytes += sh->bam ? len : 0; sh->bgzf_bytes += sh->bam && !sh->sink ? out_len : 0;
             sh->n_processed += fq.n_reads; sh->seq_chunks += !ck.simple; sh->in_flight -= ck.bytes.size();
             sh->chunk_s.push_back(t7 - t0); sh->chunk_done_s.push_back(t7 - sh->t_loop); sh->chunk_reads.push_back(fq.n_reads);
             ++sh->next_to_write;
@@ -284,6 +330,9 @@ void usage(const bm2_mem_opt_t &o) {
 "              (<out>.tmp.NNNN) or, on standard output, in ${TMPDIR:-/tmp}; the header's @HD line gets SO:coordinate\n"
 "  --sort-mem SIZE  uncompressed BAM bytes per sorted run, with a K, M or G suffix [2G]\n"
 "  --write-index  write the BAI index <out>.bai (needs --sort and -o)\n"
+"  --markdup   mark duplicates (flag 0x400) in the sorted BAM (implies --sort): templates with the same unclipped 5' ends and strands,\n"
+"              the one with the highest sum of base qualities >= 15 kept (ties: the first in the input); Picard MarkDuplicates's\n"
+"              defaults without optical duplicates, not claimed byte-equal to it.  Holds --sort-mem / 8 bytes of signatures on the host\n"
 "  --dump-opt  print the parsed options, the -I values, the read group and the header as JSON, and exit before any GPU work\n"
 "  --dump-chunks  print the chunks the input is cut into (first read, byte ranges, whether bm2_fastq_encode takes them) as JSON lines,\n"
 "              and exit without loading the index\n",
@@ -379,7 +428,7 @@ int main(int argc, char **argv) {
     static const char *const optstring = "51qpaMCSPVYjk:c:v:s:r:t:R:A:B:O:E:U:w:L:d:T:Q:D:m:I:N:W:x:G:h:y:K:X:H:o:f:";
     // this program's own arguments first: `-p N` (worker count), --bam and --dump-opt are taken out of the list, walking it the way getopt will
     // (option arguments skipped, `--` ends the options), so that everything left is parsed as main_mem parses it
-    int workers = 2; bool dump = false, dump_chunks = false, bam = false, sort = false, write_index = false;
+    int workers = 2; bool dump = false, dump_chunks = false, bam = false, sort = false, write_index = false, markdup = false;
     long long sort_mem = 2LL << 30;
     std::vector<char *> av = { argv[0] };
     for (int i = 1; i < argc; ++i) {
@@ -389,6 +438,7 @@ int main(int argc, char **argv) {
         if (!strcmp(s, "--bam")) { bam = true; continue; }
         if (!strcmp(s, "--sort")) { sort = bam = true; continue; }
         if (!strcmp(s, "--write-index")) { write_index = true; continue; }
+        if (!strcmp(s, "--markdup")) { markdup = sort = bam = true; continue; }
         if (!strcmp(s, "--sort-mem")) {
             if (i + 1 >= argc || !parse_size(argv[i + 1], &sort_mem)) {
                 fprintf(stderr, "[E::bm2_mem] --sort-mem takes a positive byte count with an optional K, M or G suffix\n"); return 1;
@@ -607,6 +657,7 @@ int main(int argc, char **argv) {
                have_rg ? json_str(rg_id).c_str() : "null", copy_comment ? "true" : "false", ignore_alt ? "true" : "false", smart ? "true" : "false",
                workers, f2 ? 2 : 1, bam ? "true" : "false");
         if (sort) printf("\"sort\": true, \"sort_mem\": %lld, \"write_index\": %s, ", sort_mem, write_index ? "true" : "false");
+        if (markdup) printf("\"markdup\": true, ");
         printf("\"header\": %s}\n", json_str(header).c_str());
         bm2_index_free(idx);
         return 0;
@@ -627,7 +678,7 @@ int main(int argc, char **argv) {
     if (sort) {
         if (bm2_create_sibling(&sort_ctx, ctxs[0])) { fprintf(stderr, "bm2_mem: %s\n", bm2_last_error(ctxs[0])); return 3; }
         int64_t need = 0, avail = 0;
-        if (bm2_bam_sort_memory(sort_ctx, sort_mem, &need, &avail)) die("bm2_bam_sort_memory", sort_ctx);
+        if (bm2_bam_sort_memory_ex(sort_ctx, sort_mem, markdup ? 1 : 0, &need, &avail)) die("bm2_bam_sort_memory", sort_ctx);
         if (need > avail) {
             fprintf(stderr, "[E::bm2_mem] --sort-mem %lld: one run sort needs %lld bytes of device memory, %lld bytes free\n", sort_mem, (long long) need, (long long) avail);
             return 3;
@@ -656,16 +707,29 @@ int main(int argc, char **argv) {
     }
     BamSortSink sink;
     if (sort) {
-        sink.sort = [sort_ctx](const uint8_t *r, int64_t n, const int64_t *st, int64_t nr, const uint8_t *c, int64_t cl, int last, bm2_sort_out *o,
-                               double *device_s) {
-            const int rc = bm2_bam_sort_compress(sort_ctx, r, n, st, nr, c, cl, last, o);
+        // without --markdup no template ids are passed, and bm2_bam_sort_compress_ex is bm2_bam_sort_compress
+        sink.sort_ex = [sort_ctx](const uint8_t *r, int64_t n, const int64_t *st, int64_t nr, const int64_t *tids, const uint8_t *c, int64_t cl, int last,
+                                  bm2_sort_out *o, const int64_t **tids_out, double *device_s) {
+            const int rc = bm2_bam_sort_compress_ex(sort_ctx, r, n, st, nr, tids, c, cl, last, o, tids_out);
             double ms[4] = { 0, 0, 0, 0 };
             bm2_last_sort_stats(sort_ctx, ms);
             *device_s = (ms[0] + ms[1] + ms[2] + ms[3]) / 1e3;
             return rc;
         };
-        sink.fail = [sort_ctx](const std::string &m) { die(m.c_str(), m == "bm2_bam_sort_compress" ? sort_ctx : nullptr); };
+        sink.fail = [sort_ctx](const std::string &m) { die(m.c_str(), m.compare(0, 4, "bm2_") == 0 ? sort_ctx : nullptr); };
         sink.run_bytes = sort_mem; sink.threads = threads;
+        if (markdup) {
+            sink.dup = [sort_ctx](const bm2_dup_entry *e, int64_t n, int resolve, const bm2_dup_entry **sorted, const int64_t **dups, int64_t *n_dups,
+                                  double *device_s) {
+                const int rc = bm2_dup_resolve(sort_ctx, e, n, resolve, sorted, dups, n_dups);
+                double ms = 0;
+                bm2_last_dup_stats(sort_ctx, nullptr, &ms);
+                *device_s = ms / 1e3;
+                return rc;
+            };
+            sink.dup_set = [sort_ctx](const uint64_t *bits, int64_t n_bits) { return bm2_dup_set(sort_ctx, bits, n_bits); };
+            sink.sig_bytes = sort_mem / 8;
+        }
         if (out_path) sink.tmp_prefix = std::string(out_path) + ".tmp.";
         else {
             const char *td = getenv("TMPDIR");
@@ -674,7 +738,7 @@ int main(int argc, char **argv) {
     }
     Shared sh;
     sh.opt = &opt; sh.idx = idx; sh.cnames = cnames.data(); sh.paired = f2 != nullptr; sh.smart = smart; sh.threads = threads; sh.out = out;
-    sh.pes0 = use_pes ? pes : nullptr; sh.copy_comment = copy_comment; sh.bam = bam; sh.sink = sort ? &sink : nullptr;
+    sh.pes0 = use_pes ? pes : nullptr; sh.copy_comment = copy_comment; sh.bam = bam; sh.sink = sort ? &sink : nullptr; sh.markdup = markdup;
     sh.extra.rg_id = have_rg ? rg_id.c_str() : nullptr; sh.extra.contig_anno = canno.data(); sh.extra.ref_hdr = (opt.flag & 0x100) != 0;
     sh.t_loop = now_s();
     std::vector<std::thread> pool;
@@ -695,6 +759,7 @@ int main(int argc, char **argv) {
     BaiBuilder bai((int) names.size());
     double index_s = 0;
     if (sort) {
+        sink.n_reads = sh.n_processed;
         sink.finish(out, (uint64_t) header_z, write_index ? &bai : nullptr);
         if (write_index) {
             const double t0 = now_s();
@@ -723,6 +788,11 @@ int main(int argc, char **argv) {
     if (sort)
         fprintf(stderr, ", \"sort_runs\": %lld, \"spill_bytes\": %lld, \"sort_s\": %.6f, \"merge_s\": %.6f, \"merge_windows\": %lld, \"index_s\": %.6f",
                 (long long) std::max<size_t>(sink.runs.size(), 1), (long long) sink.spill_bytes, sink.sort_s, sink.merge_s, (long long) sink.merge_windows, index_s);
+    if (markdup)
+        fprintf(stderr, ", \"markdup_s\": %.6f, \"dup_templates\": %lld, \"dup_pair_templates\": %lld, \"dup_fragment_templates\": %lld, \"dup_records\": %lld, "
+                        "\"dup_sig_runs\": %lld, \"dup_sig_bytes\": %lld", sh.t_dup_sig + sink.markdup_s, (long long) sink.dup_templates,
+                (long long) sink.dup_pair_templates, (long long) sink.dup_frag_templates, (long long) sink.dup_records, (long long) sink.dup_sig_runs,
+                (long long) sink.dup_sig_bytes);
     fprintf(stderr, "}\n");
     if (sort_ctx) bm2_destroy(sort_ctx);
     for (int w = workers - 1; w >= 0; --w) bm2_destroy(ctxs[w]);

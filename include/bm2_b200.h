@@ -447,6 +447,47 @@ int  bm2_bam_sort_compress(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const i
 int  bm2_last_sort_stats(const bm2_ctx *ctx, double ms[4]);
 /* Device bytes one bm2_bam_sort_compress call on run_bytes of records of about 300 bytes needs, and the bytes free on ctx's device now. */
 int  bm2_bam_sort_memory(const bm2_ctx *ctx, int64_t run_bytes, int64_t *needed, int64_t *free_bytes);
+/* The same with with_tids != 0: plus the template ids bm2_bam_sort_compress_ex carries (8 bytes per record in, 8 sorted). */
+int  bm2_bam_sort_memory_ex(const bm2_ctx *ctx, int64_t run_bytes, int with_tids, int64_t *needed, int64_t *free_bytes);
+
+/* ---- Duplicate marking (bm2_mem --markdup) ------------------------------------------------------------------------------------------------
+ * The rule (csrc/markdup_device.cuh) follows Picard MarkDuplicates's defaults, SUM_OF_BASE_QUALITIES and no optical duplicates; equality with
+ * Picard or samtools is not claimed.  A template is a read, or both reads of a pair; its id (tid) is the 0-based input-order index of its
+ * first read.  Its primaries (no 0x100 / 0x800) give its entries:
+ *   end    (refID, unclipped 5' coordinate, reverse) packed as refID << 34 | (coord + 2^32) << 1 | reverse (refID < 2^30, |coord| < 2^32):
+ *          forward pos - leading S/H, reverse bam_endpos - 1 + trailing S/H; a CIGAR in CG:B,I is read from there
+ *   score  of a read: min(sum of its qualities >= 15, 16383), 0 for QUAL '*'
+ *   pair entry (kind 0)       both primaries of a pair mapped: k1 = min(endA, endB), k2 = max, score the sum of both
+ *   pair-end entries (kind 2) of such a pair, one per end, in the fragment space: k1 = the end, k2 = 0, score that read's
+ *   fragment entry (kind 1)   one mapped primary (single-end, or its mate unmapped): k1 = its end, k2 = 0, score its read's
+ * Groups are the entries of one space with the same (k1, k2), ordered by score descending then tid.  Pair space: all but the first are
+ * duplicates.  Fragment space: with a pair-end entry in the group every fragment entry is a duplicate, else all fragment entries but the first
+ * are.  Pair-end entries are never duplicates. */
+typedef struct { uint64_t k1, k2; int64_t tid; int32_t score, kind; } bm2_dup_entry;
+/* Signatures of one chunk, one warp per template, on ctx's stream.  recs: n bytes of BAM records (HOST); starts: the n_recs record offsets;
+ * tmpl_first: n_tmpl + 1 record indices, template t owning records [tmpl_first[t], tmpl_first[t+1]); tmpl_id: each template's id.
+ * Out (HOST, owned by the context, valid until its next bm2_dup_signatures call): the pair entries and the fragment-space entries, both in
+ * template order (a pair's two pair-end entries in the order of its primaries). */
+int  bm2_dup_signatures(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int64_t *starts, int64_t n_recs, const int64_t *tmpl_first,
+                        const int64_t *tmpl_id, int64_t n_tmpl, const bm2_dup_entry **pairs, int64_t *n_pairs, const bm2_dup_entry **frags,
+                        int64_t *n_frags);
+/* Entries of one space (HOST, n of them) sorted by (k1, k2, score descending, tid) with a stable radix sort over the bits they use.
+ * resolve == 0: *sorted gets them in that order (for a spilled run).  resolve != 0: every group is taken as whole, and *dups gets the ids of
+ * the duplicate templates in sorted order, *n_dups of them.  Out: HOST, owned by the context, valid until its next bm2_dup_resolve call. */
+int  bm2_dup_resolve(bm2_ctx *ctx, const bm2_dup_entry *entries, int64_t n, int resolve, const bm2_dup_entry **sorted, const int64_t **dups,
+                     int64_t *n_dups);
+/* Device ms (CUDA events) of the context's last bm2_dup_signatures and last bm2_dup_resolve call. */
+int  bm2_last_dup_stats(const bm2_ctx *ctx, double *signatures_ms, double *resolve_ms);
+/* The duplicate templates: bit t of bits (n_bits of them, 1 per input read; word w holds bits 64w..64w+63) set for a duplicate template t.
+ * Copied to ctx's device and kept until the next call (n_bits == 0 clears it).  A bitset larger than the device's free memory is an error
+ * that gives both numbers. */
+int  bm2_dup_set(bm2_ctx *ctx, const uint64_t *bits, int64_t n_bits);
+/* bm2_bam_sort_compress, with one template id per record (tids, NULL: none) carried through the sort: *tids_out (HOST, owned by the context,
+ * valid until its next call; may be NULL) gets them in output order.  When a bitset was given to bm2_dup_set, a record whose template's bit is
+ * set and that lacks 0x4 gets 0x400 in its flag (the uint16 at byte 18 of the record counted from block_size) and in its bm2_sort_rec.flag;
+ * no other byte changes.  Without tids, or with no bitset, the bytes are bm2_bam_sort_compress's. */
+int  bm2_bam_sort_compress_ex(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int64_t *starts, int64_t n_recs, const int64_t *tids,
+                              const uint8_t *carry, int64_t carry_len, int last, bm2_sort_out *out, const int64_t **tids_out);
 
 /* Staged mate rescue inside bm2_sam_pe (same records, other kernels): the windows mem_matesw (src/bwamem_pair.cpp:150-283) can ask for are
  * listed for all pairs of a wave from the regions before any rescue, aligned as one batch with one window per warp (the job shape of
