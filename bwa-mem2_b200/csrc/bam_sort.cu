@@ -92,7 +92,9 @@ __global__ void sort_gather_kernel(const uint8_t *__restrict__ in, const int64_t
 
 enum { SD_IN, SD_STARTS, SD_INFO, SD_LEN, SD_KEYS0, SD_KEYS1, SD_VALS0, SD_VALS1, SD_LENS, SD_OFFS, SD_TEMP, SD_OUT, SD_SINFO, SD_MAX, SD_TIDS,
        SD_STIDS, SD_END };
-static_assert(SD_END <= (int) (sizeof(((bm2_ctx *) nullptr)->sort_d) / sizeof(DevBuf)), "sort buffers");
+enum { SH_OFFS, SH_INFO, SH_END };
+static_assert(SD_END == std::extent<decltype(bm2_ctx::sort_d)>::value, "bm2_ctx::sort_d: one buffer per slot");
+static_assert(SH_END == std::extent<decltype(bm2_ctx::sort_h)>::value, "bm2_ctx::sort_h: one buffer per slot");
 
 int bits_of(uint64_t v) { int b = 0; while (v >> b) ++b; return b; }
 
@@ -139,15 +141,15 @@ static int sort_compress(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int
         ctx->ensure(b[SD_VALS0], (size_t) nr * 4 + 8) || ctx->ensure(b[SD_VALS1], (size_t) nr * 4 + 8) ||
         ctx->ensure(b[SD_LENS], (size_t) nr * 8 + 8) || ctx->ensure(b[SD_OFFS], (size_t) nr * 8 + 8) || ctx->ensure(b[SD_TEMP], temp + 16) ||
         ctx->ensure(b[SD_OUT], (size_t) (carry_len + n) + 16) || ctx->ensure(b[SD_SINFO], (size_t) nr * sizeof(bm2_sort_rec) + 8) ||
-        ctx->ensure(b[SD_MAX], 16) || ctx->ensure_host(ctx->sort_h[0], (size_t) nr * 8 + 16) ||
-        ctx->ensure_host(ctx->sort_h[1], (size_t) nr * sizeof(bm2_sort_rec) + 16)) return 1;
+        ctx->ensure(b[SD_MAX], 16) || ctx->ensure_host(ctx->sort_h[SH_OFFS], (size_t) nr * 8 + 16) ||
+        ctx->ensure_host(ctx->sort_h[SH_INFO], (size_t) nr * sizeof(bm2_sort_rec) + 16)) return 1;
     if (tids && (ctx->ensure(b[SD_TIDS], (size_t) nr * 8 + 8) || ctx->ensure(b[SD_STIDS], (size_t) nr * 8 + 8))) return 1;
     int64_t *d_tids = tids ? (int64_t *) b[SD_TIDS].p : nullptr, *d_stids = tids ? (int64_t *) b[SD_STIDS].p : nullptr;
     ctx->sort_tids.resize(tids ? (size_t) nr : 0);
     for (cudaEvent_t &ev : ctx->sort_ev) if (!ev) BM2_CUDA_OK(cudaEventCreate(&ev));
     if (carry_len) BM2_CUDA_OK(cudaMemcpy(b[SD_OUT].p, carry, (size_t) carry_len, cudaMemcpyHostToDevice));   // carry may be this context's last carry
-    int64_t *h_offs = (int64_t *) ctx->sort_h[0].p;
-    bm2_sort_rec *h_info = (bm2_sort_rec *) ctx->sort_h[1].p;
+    int64_t *h_offs = (int64_t *) ctx->sort_h[SH_OFFS].p;
+    bm2_sort_rec *h_info = (bm2_sort_rec *) ctx->sort_h[SH_INFO].p;
     const uint32_t *ord = (const uint32_t *) b[SD_VALS0].p;
     if (nr) {
         BM2_CUDA_OK(cudaMemcpyAsync(b[SD_IN].p, recs, (size_t) n, cudaMemcpyHostToDevice, st));

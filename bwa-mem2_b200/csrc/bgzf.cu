@@ -143,7 +143,10 @@ __global__ void bgzf_gather_kernel(const uint8_t *__restrict__ slots, const int3
     for (int i = threadIdx.x; i < sizes[b]; i += blockDim.x) o[i] = s[i];
 }
 
-enum { BG_IN, BG_STARTS, BG_ITEMS, BG_SLOTS, BG_SIZES, BG_OFFS, BG_OUT };
+enum { BG_IN, BG_STARTS, BG_ITEMS, BG_SLOTS, BG_SIZES, BG_OFFS, BG_OUT, BG_END };
+enum { BH_SIZES, BH_OUT, BH_END };
+static_assert(BG_END == std::extent<decltype(bm2_ctx::bgzf_d)>::value, "bm2_ctx::bgzf_d: one buffer per slot");
+static_assert(BH_END == std::extent<decltype(bm2_ctx::bgzf_h)>::value, "bm2_ctx::bgzf_h: one buffer per slot");
 
 }  // namespace
 
@@ -162,7 +165,7 @@ int bgzf_compress_device(bm2_ctx *ctx, const uint8_t *d_in, const int64_t *start
     if (ctx->ensure(bg[BG_STARTS], (size_t) (nb + 1) * 8) ||
         ctx->ensure(bg[BG_ITEMS], (size_t) grid * BGZF_BLOCK * 2) || ctx->ensure(bg[BG_SLOTS], (size_t) nb * BGZF_MAX_MEMBER) ||
         ctx->ensure(bg[BG_SIZES], (size_t) nb * 4) || ctx->ensure(bg[BG_OFFS], (size_t) (nb + 1) * 8) ||
-        ctx->ensure_host(ctx->bgzf_h[0], (size_t) (nb + 1) * 8)) return 1;
+        ctx->ensure_host(ctx->bgzf_h[BH_SIZES], (size_t) (nb + 1) * 8)) return 1;
     for (cudaEvent_t &ev : ctx->bgzf_ev) if (!ev) BM2_CUDA_OK(cudaEventCreate(&ev));
     BM2_CUDA_OK(cudaFuncSetAttribute(bgzf_block_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) kSmem));
     BM2_CUDA_OK(cudaMemcpyAsync(bg[BG_STARTS].p, starts, (size_t) (nb + 1) * 8, cudaMemcpyHostToDevice, st));
@@ -171,7 +174,7 @@ int bgzf_compress_device(bm2_ctx *ctx, const uint8_t *d_in, const int64_t *start
                                                      (uint16_t *) bg[BG_ITEMS].p, (uint8_t *) bg[BG_SLOTS].p, (int32_t *) bg[BG_SIZES].p);
     BM2_CUDA_OK(cudaGetLastError());
     BM2_CUDA_OK(cudaEventRecord(ctx->bgzf_ev[1], st));
-    int32_t *hs = (int32_t *) ctx->bgzf_h[0].p;
+    int32_t *hs = (int32_t *) ctx->bgzf_h[BH_SIZES].p;
     BM2_CUDA_OK(cudaMemcpyAsync(hs, bg[BG_SIZES].p, (size_t) nb * 4, cudaMemcpyDeviceToHost, st));
     BM2_CUDA_OK(cudaStreamSynchronize(st));
     std::vector<int64_t> offs((size_t) nb + 1, 0);
@@ -182,20 +185,20 @@ int bgzf_compress_device(bm2_ctx *ctx, const uint8_t *d_in, const int64_t *start
     ctx->bgzf_sizes.assign(hs, hs + nb);
     const int64_t total = offs[(size_t) nb];
     DevBuf &dst = gather ? *gather : bg[BG_OUT];
-    if (ctx->ensure(dst, (size_t) total + 16) || ctx->ensure_host(ctx->bgzf_h[1], (size_t) total + 16)) return 1;
+    if (ctx->ensure(dst, (size_t) total + 16) || ctx->ensure_host(ctx->bgzf_h[BH_OUT], (size_t) total + 16)) return 1;
     BM2_CUDA_OK(cudaMemcpyAsync(bg[BG_OFFS].p, offs.data(), (size_t) (nb + 1) * 8, cudaMemcpyHostToDevice, st));
     BM2_CUDA_OK(cudaEventRecord(ctx->bgzf_ev[2], st));
     bgzf_gather_kernel<<<(unsigned) nb, 256, 0, st>>>((const uint8_t *) bg[BG_SLOTS].p, (const int32_t *) bg[BG_SIZES].p, (const int64_t *) bg[BG_OFFS].p,
                                                       (uint8_t *) dst.p);
     BM2_CUDA_OK(cudaGetLastError());
     BM2_CUDA_OK(cudaEventRecord(ctx->bgzf_ev[3], st));
-    BM2_CUDA_OK(cudaMemcpyAsync(ctx->bgzf_h[1].p, dst.p, (size_t) total, cudaMemcpyDeviceToHost, st));
+    BM2_CUDA_OK(cudaMemcpyAsync(ctx->bgzf_h[BH_OUT].p, dst.p, (size_t) total, cudaMemcpyDeviceToHost, st));
     BM2_CUDA_OK(cudaStreamSynchronize(st));
     float ms0 = 0, ms1 = 0;
     BM2_CUDA_OK(cudaEventElapsedTime(&ms0, ctx->bgzf_ev[0], ctx->bgzf_ev[1]));
     BM2_CUDA_OK(cudaEventElapsedTime(&ms1, ctx->bgzf_ev[2], ctx->bgzf_ev[3]));
     ctx->bgzf_ms = (double) ms0 + ms1; ctx->bgzf_members = nb;
-    *out = (const uint8_t *) ctx->bgzf_h[1].p; *out_len = total;
+    *out = (const uint8_t *) ctx->bgzf_h[BH_OUT].p; *out_len = total;
     return 0;
 }
 

@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <string>
+#include <type_traits>
 #include <vector>
 #include <mutex>
 #include "bm2_b200.h"
@@ -35,9 +36,11 @@ struct bm2_ctx {
     std::vector<void *> idx_allocs;
     // seam 1
     DevBuf io_pairs, io_ref, io_qer, bsw_jobs, bsw_outs, bsw_scratch;
+    // Each x_d / x_h table below holds the scratch and result buffers of one source file, indexed by that file's slot enum; a
+    // static_assert there ties the enum to the size here.  A file's results stay valid while other files run on the same context.
     // seam 2 (pipeline.cu)
-    DevBuf d[144];         // slots: pipeline.cu 0-47, cigar.cu 48-63, sam.cu 64-83 + 90-95, ksw.cu 84-89, fastq.cu 100-126 + 128-143
-    HostBuf h[52];         // slots: pipeline.cu 0-7, cigar.cu 8-15, sam.cu 16-23, fastq.cu 24-51
+    DevBuf pipe_d[39];
+    HostBuf pipe_h[5];
     std::vector<cudaEvent_t> events;
     std::vector<const char *> stage_names;
     std::vector<float> stage_ms;
@@ -52,8 +55,17 @@ struct bm2_ctx {
     // ALU-bound extension stage, so that at any time DIFFERENT kinds of stages overlap instead of four copies of the same
     std::mutex tok_smem, tok_bsw;
     cudaEvent_t ev_entry = nullptr;
-    // seam 4 (sam.cu): staged rescue switch (-1: the BM2_SAM_STAGED environment variable decides, default off), events around the stage's
-    // kernels, and the last call's times (jobs, window alignments, pairs, gather; ms summed over waves) and counters
+    // seam 3 (cigar.cu), the rescue alignments of bm2_ksw_align2 (ksw.cu), the read batches of bm2_fastq_encode / bm2_fastq_smart_pair /
+    // bm2_seq_encode (fastq.cu)
+    DevBuf cigar_d[14];
+    HostBuf cigar_h[3];
+    DevBuf ksw_d[6];
+    DevBuf fq_d[38];
+    HostBuf fq_h[25];
+    // seam 4 (sam.cu): buffers, staged rescue switch (-1: the BM2_SAM_STAGED environment variable decides, default off), events around
+    // the stage's kernels, and the last call's times (jobs, window alignments, pairs, gather; ms summed over waves) and counters
+    DevBuf sam_d[24];
+    HostBuf sam_h[5];
     int sam_staged = -1;
     cudaEvent_t sam_ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
     double sam_ms[4] = {0, 0, 0, 0};
@@ -86,13 +98,16 @@ struct bm2_ctx {
     int ensure_host(HostBuf &b, size_t bytes);
     std::vector<DevBuf *> all_dev() {
         std::vector<DevBuf *> v = {&io_pairs, &io_ref, &io_qer, &bsw_jobs, &bsw_outs, &bsw_scratch, &dup_bits};
-        for (auto &x : d) v.push_back(&x);
-        for (auto &x : bgzf_d) v.push_back(&x);
-        for (auto &x : sort_d) v.push_back(&x);
-        for (auto &x : dup_d) v.push_back(&x);
+        append(v, pipe_d); append(v, cigar_d); append(v, sam_d); append(v, ksw_d); append(v, fq_d);
+        append(v, bgzf_d); append(v, sort_d); append(v, dup_d);
         return v;
     }
-    std::vector<HostBuf *> all_host() { std::vector<HostBuf *> v; for (auto &x : h) v.push_back(&x); for (auto &x : bgzf_h) v.push_back(&x); for (auto &x : sort_h) v.push_back(&x); return v; }
+    std::vector<HostBuf *> all_host() {
+        std::vector<HostBuf *> v;
+        append(v, pipe_h); append(v, cigar_h); append(v, sam_h); append(v, fq_h); append(v, bgzf_h); append(v, sort_h);
+        return v;
+    }
+    template <class B, size_t N> static void append(std::vector<B *> &v, B (&t)[N]) { for (B &x : t) v.push_back(&x); }
 };
 
 // bgzf.cu: the members of the nb blocks [starts[b], starts[b+1]) of the device bytes d_in, on ctx's stream (the body of bm2_bgzf_compress),

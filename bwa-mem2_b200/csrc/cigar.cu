@@ -14,10 +14,10 @@
 #include <cstring>
 
 namespace {
-// bm2_ctx::d[] / h[] slots of this file (pipeline.cu uses d[0..41], h[0..5])
-enum { CB_CODES = 48, CB_OFFS, CB_REQS, CB_CAPOFF, CB_OPS_W, CB_MD_W, CB_RECS, CB_Z, CB_HE, CB_CNT, CB_SCAN, CB_CUB, CB_OPS, CB_MD };
-enum { CH_RECS = 8, CH_OPS, CH_MD };
-static_assert(CB_MD < 64, "bm2_ctx::d[] too small");
+enum { CB_CODES, CB_OFFS, CB_REQS, CB_CAPOFF, CB_OPS_W, CB_MD_W, CB_RECS, CB_Z, CB_HE, CB_CNT, CB_SCAN, CB_CUB, CB_OPS, CB_MD, CB_COUNT_ };
+enum { CH_RECS, CH_OPS, CH_MD, CH_COUNT_ };
+static_assert(CB_COUNT_ == std::extent<decltype(bm2_ctx::cigar_d)>::value, "bm2_ctx::cigar_d: one buffer per slot");
+static_assert(CH_COUNT_ == std::extent<decltype(bm2_ctx::cigar_h)>::value, "bm2_ctx::cigar_h: one buffer per slot");
 
 struct CapOff { int64_t ops, md; };       // start of a request's worst-case stripes
 
@@ -52,7 +52,7 @@ __global__ void cigar_gather_kernel(int64_t n, const CapOff *__restrict__ cap, c
     for (int k = 0; k < o.n_md; ++k) md[o.md_off + k] = md_w[cap[r].md + k];
 }
 
-template <class T> T *P(bm2_ctx *ctx, int b) { return (T *) ctx->d[b].p; }
+template <class T> T *P(bm2_ctx *ctx, int b) { return (T *) ctx->cigar_d[b].p; }
 
 }  // namespace
 
@@ -64,8 +64,8 @@ extern "C" int bm2_gen_cigar(bm2_ctx *ctx, const bm2_read_batch *reads, const bm
     BM2_CUDA_OK(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
     memset(out, 0, sizeof(*out));
-    if (ctx->ensure_host(ctx->h[CH_RECS], sizeof(bm2_cigar_rec)) || ctx->ensure_host(ctx->h[CH_OPS], 16) || ctx->ensure_host(ctx->h[CH_MD], 16)) return 1;
-    out->recs = (const bm2_cigar_rec *) ctx->h[CH_RECS].p; out->cigar = (const uint32_t *) ctx->h[CH_OPS].p; out->md = (const char *) ctx->h[CH_MD].p;
+    if (ctx->ensure_host(ctx->cigar_h[CH_RECS], sizeof(bm2_cigar_rec)) || ctx->ensure_host(ctx->cigar_h[CH_OPS], 16) || ctx->ensure_host(ctx->cigar_h[CH_MD], 16)) return 1;
+    out->recs = (const bm2_cigar_rec *) ctx->cigar_h[CH_RECS].p; out->cigar = (const uint32_t *) ctx->cigar_h[CH_OPS].p; out->md = (const char *) ctx->cigar_h[CH_MD].p;
     if (n == 0) return 0;
     CigarParams p; memcpy(p.mat, ctx->opt.mat, 25); p.o_del = ctx->opt.o_del; p.e_del = ctx->opt.e_del; p.o_ins = ctx->opt.o_ins; p.e_ins = ctx->opt.e_ins;
     if (p.e_del <= 0 || p.e_ins <= 0) { bm2_set_error(ctx, "bm2_gen_cigar: gap extension penalties must be positive"); return 1; }
@@ -98,16 +98,16 @@ extern "C" int bm2_gen_cigar(bm2_ctx *ctx, const bm2_read_batch *reads, const bm
     if (T > t_need) T = t_need;
     const int he_stride = 2 * (max_lq + 1);
     const int64_t total = reads->offsets[nr];
-    if (ctx->ensure(ctx->d[CB_CODES], (size_t) total + 16) || ctx->ensure(ctx->d[CB_OFFS], (size_t) (nr + 1) * 8) ||
-        ctx->ensure(ctx->d[CB_REQS], (size_t) n * sizeof(bm2_cigar_req)) || ctx->ensure(ctx->d[CB_CAPOFF], (size_t) (n + 1) * sizeof(CapOff)) ||
-        ctx->ensure(ctx->d[CB_OPS_W], (size_t) ops_total * 4 + 16) || ctx->ensure(ctx->d[CB_MD_W], (size_t) md_total + 16) ||
-        ctx->ensure(ctx->d[CB_RECS], (size_t) n * sizeof(bm2_cigar_rec)) || ctx->ensure(ctx->d[CB_Z], (size_t) (zcap * T) + 16) ||
-        ctx->ensure(ctx->d[CB_HE], (size_t) T * he_stride * 4) || ctx->ensure(ctx->d[CB_CNT], (size_t) (n + 1) * 16) ||
-        ctx->ensure(ctx->d[CB_SCAN], (size_t) (n + 1) * 16)) return 1;
-    BM2_CUDA_OK(cudaMemcpyAsync(ctx->d[CB_CODES].p, reads->codes, (size_t) total, cudaMemcpyHostToDevice, st));
-    BM2_CUDA_OK(cudaMemcpyAsync(ctx->d[CB_OFFS].p, reads->offsets, (size_t) (nr + 1) * 8, cudaMemcpyHostToDevice, st));
-    BM2_CUDA_OK(cudaMemcpyAsync(ctx->d[CB_REQS].p, reqs, (size_t) n * sizeof(bm2_cigar_req), cudaMemcpyHostToDevice, st));
-    BM2_CUDA_OK(cudaMemcpyAsync(ctx->d[CB_CAPOFF].p, cap.data(), (size_t) (n + 1) * sizeof(CapOff), cudaMemcpyHostToDevice, st));
+    if (ctx->ensure(ctx->cigar_d[CB_CODES], (size_t) total + 16) || ctx->ensure(ctx->cigar_d[CB_OFFS], (size_t) (nr + 1) * 8) ||
+        ctx->ensure(ctx->cigar_d[CB_REQS], (size_t) n * sizeof(bm2_cigar_req)) || ctx->ensure(ctx->cigar_d[CB_CAPOFF], (size_t) (n + 1) * sizeof(CapOff)) ||
+        ctx->ensure(ctx->cigar_d[CB_OPS_W], (size_t) ops_total * 4 + 16) || ctx->ensure(ctx->cigar_d[CB_MD_W], (size_t) md_total + 16) ||
+        ctx->ensure(ctx->cigar_d[CB_RECS], (size_t) n * sizeof(bm2_cigar_rec)) || ctx->ensure(ctx->cigar_d[CB_Z], (size_t) (zcap * T) + 16) ||
+        ctx->ensure(ctx->cigar_d[CB_HE], (size_t) T * he_stride * 4) || ctx->ensure(ctx->cigar_d[CB_CNT], (size_t) (n + 1) * 16) ||
+        ctx->ensure(ctx->cigar_d[CB_SCAN], (size_t) (n + 1) * 16)) return 1;
+    BM2_CUDA_OK(cudaMemcpyAsync(ctx->cigar_d[CB_CODES].p, reads->codes, (size_t) total, cudaMemcpyHostToDevice, st));
+    BM2_CUDA_OK(cudaMemcpyAsync(ctx->cigar_d[CB_OFFS].p, reads->offsets, (size_t) (nr + 1) * 8, cudaMemcpyHostToDevice, st));
+    BM2_CUDA_OK(cudaMemcpyAsync(ctx->cigar_d[CB_REQS].p, reqs, (size_t) n * sizeof(bm2_cigar_req), cudaMemcpyHostToDevice, st));
+    BM2_CUDA_OK(cudaMemcpyAsync(ctx->cigar_d[CB_CAPOFF].p, cap.data(), (size_t) (n + 1) * sizeof(CapOff), cudaMemcpyHostToDevice, st));
     int64_t *cnt_ops = P<int64_t>(ctx, CB_CNT), *cnt_md = cnt_ops + (n + 1), *off_ops = P<int64_t>(ctx, CB_SCAN), *off_md = off_ops + (n + 1);
     BM2_CUDA_OK(cudaMemsetAsync(cnt_ops + n, 0, 8, st));
     BM2_CUDA_OK(cudaMemsetAsync(cnt_md + n, 0, 8, st));
@@ -117,25 +117,25 @@ extern "C" int bm2_gen_cigar(bm2_ctx *ctx, const bm2_read_batch *reads, const bm
                                                       P<int32_t>(ctx, CB_HE), he_stride, cnt_ops, cnt_md);
     size_t cub_bytes = 0;
     cub::DeviceScan::ExclusiveSum(nullptr, cub_bytes, cnt_ops, off_ops, (int) (n + 1));
-    if (ctx->ensure(ctx->d[CB_CUB], cub_bytes)) return 1;
-    BM2_CUDA_OK(cub::DeviceScan::ExclusiveSum(ctx->d[CB_CUB].p, cub_bytes, cnt_ops, off_ops, (int) (n + 1), st));
-    BM2_CUDA_OK(cub::DeviceScan::ExclusiveSum(ctx->d[CB_CUB].p, cub_bytes, cnt_md, off_md, (int) (n + 1), st));
+    if (ctx->ensure(ctx->cigar_d[CB_CUB], cub_bytes)) return 1;
+    BM2_CUDA_OK(cub::DeviceScan::ExclusiveSum(ctx->cigar_d[CB_CUB].p, cub_bytes, cnt_ops, off_ops, (int) (n + 1), st));
+    BM2_CUDA_OK(cub::DeviceScan::ExclusiveSum(ctx->cigar_d[CB_CUB].p, cub_bytes, cnt_md, off_md, (int) (n + 1), st));
     int64_t tot[2] = {0, 0};
     BM2_CUDA_OK(cudaMemcpyAsync(&tot[0], off_ops + n, 8, cudaMemcpyDeviceToHost, st));
     BM2_CUDA_OK(cudaMemcpyAsync(&tot[1], off_md + n, 8, cudaMemcpyDeviceToHost, st));
     BM2_CUDA_OK(cudaStreamSynchronize(st));
-    if (ctx->ensure(ctx->d[CB_OPS], (size_t) tot[0] * 4 + 16) || ctx->ensure(ctx->d[CB_MD], (size_t) tot[1] + 16) ||
-        ctx->ensure_host(ctx->h[CH_RECS], (size_t) n * sizeof(bm2_cigar_rec)) || ctx->ensure_host(ctx->h[CH_OPS], (size_t) tot[0] * 4 + 16) ||
-        ctx->ensure_host(ctx->h[CH_MD], (size_t) tot[1] + 16)) return 1;
+    if (ctx->ensure(ctx->cigar_d[CB_OPS], (size_t) tot[0] * 4 + 16) || ctx->ensure(ctx->cigar_d[CB_MD], (size_t) tot[1] + 16) ||
+        ctx->ensure_host(ctx->cigar_h[CH_RECS], (size_t) n * sizeof(bm2_cigar_rec)) || ctx->ensure_host(ctx->cigar_h[CH_OPS], (size_t) tot[0] * 4 + 16) ||
+        ctx->ensure_host(ctx->cigar_h[CH_MD], (size_t) tot[1] + 16)) return 1;
     cigar_gather_kernel<<<(unsigned) ((n + 127) / 128), 128, 0, st>>>(n, P<CapOff>(ctx, CB_CAPOFF), P<uint32_t>(ctx, CB_OPS_W), P<char>(ctx, CB_MD_W), off_ops,
                                                                       off_md, P<bm2_cigar_rec>(ctx, CB_RECS), P<uint32_t>(ctx, CB_OPS), P<char>(ctx, CB_MD));
-    BM2_CUDA_OK(cudaMemcpyAsync(ctx->h[CH_RECS].p, ctx->d[CB_RECS].p, (size_t) n * sizeof(bm2_cigar_rec), cudaMemcpyDeviceToHost, st));
-    if (tot[0]) BM2_CUDA_OK(cudaMemcpyAsync(ctx->h[CH_OPS].p, ctx->d[CB_OPS].p, (size_t) tot[0] * 4, cudaMemcpyDeviceToHost, st));
-    if (tot[1]) BM2_CUDA_OK(cudaMemcpyAsync(ctx->h[CH_MD].p, ctx->d[CB_MD].p, (size_t) tot[1], cudaMemcpyDeviceToHost, st));
+    BM2_CUDA_OK(cudaMemcpyAsync(ctx->cigar_h[CH_RECS].p, ctx->cigar_d[CB_RECS].p, (size_t) n * sizeof(bm2_cigar_rec), cudaMemcpyDeviceToHost, st));
+    if (tot[0]) BM2_CUDA_OK(cudaMemcpyAsync(ctx->cigar_h[CH_OPS].p, ctx->cigar_d[CB_OPS].p, (size_t) tot[0] * 4, cudaMemcpyDeviceToHost, st));
+    if (tot[1]) BM2_CUDA_OK(cudaMemcpyAsync(ctx->cigar_h[CH_MD].p, ctx->cigar_d[CB_MD].p, (size_t) tot[1], cudaMemcpyDeviceToHost, st));
     BM2_CUDA_OK(cudaStreamSynchronize(st));
     BM2_CUDA_OK(cudaGetLastError());
-    out->n = n; out->recs = (const bm2_cigar_rec *) ctx->h[CH_RECS].p;
-    out->n_ops = tot[0]; out->cigar = (const uint32_t *) ctx->h[CH_OPS].p;
-    out->n_md = tot[1]; out->md = (const char *) ctx->h[CH_MD].p;
+    out->n = n; out->recs = (const bm2_cigar_rec *) ctx->cigar_h[CH_RECS].p;
+    out->n_ops = tot[0]; out->cigar = (const uint32_t *) ctx->cigar_h[CH_OPS].p;
+    out->n_md = tot[1]; out->md = (const char *) ctx->cigar_h[CH_MD].p;
     return 0;
 }

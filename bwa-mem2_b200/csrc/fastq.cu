@@ -116,14 +116,18 @@ __global__ void fastq_gather_kernel(const int32_t *__restrict__ idx, const int64
     }
 }
 
-enum FqBuf { F_RAW0 = 100, F_RAW1, F_NL0, F_NL1, F_SPANS, F_LENS, F_OFFS, F_CODES, F_QUALS, F_TMP, F_MISC };     // slots of bm2_ctx::d[]
-enum FqHost { FH_OFFS = 24, FH_CODES, FH_QUALS, FH_SPANS, FH_NAMEBEG, FH_NAMELEN, FH_CMTBEG, FH_CMTLEN };
-// smart pairing: device slots 112-126; per set s: F_SIDX + s, F_SLEN + s, ... and host slots FH_SPLIT + 8 s + k
-enum FqSplit { F_KEY = 112, F_RUN, F_SFLAG, F_SCNT = F_SFLAG + 2, F_SIDX, F_SLEN = F_SIDX + 2, F_SOFF = F_SLEN + 2, F_SCODES = F_SOFF + 2,
-               F_SQUALS = F_SCODES + 2 };
-enum FqSplitHost { FH_SPLIT = 32 };
-enum { SH_OFFS, SH_CODES, SH_QUALS, SH_NAMEBEG, SH_NAMELEN, SH_CMTBEG, SH_CMTLEN, SH_IDX };
-static_assert(F_SQUALS + 1 < 128, "bm2_ctx::d[] slots");
+// slots of bm2_ctx::fq_d: the read batch (buffer b: F_RAW0 + b, F_NL0 + b); smart pairing (set s: F_SFLAG + s, F_SIDX + s, ...);
+// bm2_seq_encode (buffer b: S_HP0 + b, S_REC0 + b)
+enum FqBuf { F_RAW0, F_RAW1, F_NL0, F_NL1, F_SPANS, F_LENS, F_OFFS, F_CODES, F_QUALS, F_TMP, F_MISC,
+             F_KEY, F_RUN, F_SFLAG, F_SCNT = F_SFLAG + 2, F_SIDX, F_SLEN = F_SIDX + 2, F_SOFF = F_SLEN + 2, F_SCODES = F_SOFF + 2,
+             F_SQUALS = F_SCODES + 2,
+             S_HP0 = F_SQUALS + 2, S_HP1, S_CAND, S_CANDU, S_INFO, S_JUMP, S_MARK, S_FLAG, S_REC0, S_REC1, S_QP, S_CNT, F_COUNT_ };
+// the host buffers of one smart-pairing set
+enum { SH_OFFS, SH_CODES, SH_QUALS, SH_NAMEBEG, SH_NAMELEN, SH_CMTBEG, SH_CMTLEN, SH_IDX, SH_COUNT_ };
+// slots of bm2_ctx::fq_h: the read batch; smart pairing (set s: FH_SPLIT + SH_COUNT_ * s + k); bm2_seq_encode
+enum FqHost { FH_OFFS, FH_CODES, FH_QUALS, FH_SPANS, FH_NAMEBEG, FH_NAMELEN, FH_CMTBEG, FH_CMTLEN, FH_SPLIT, FH_QP = FH_SPLIT + 2 * SH_COUNT_, FH_COUNT_ };
+static_assert(F_COUNT_ == std::extent<decltype(bm2_ctx::fq_d)>::value, "bm2_ctx::fq_d: one buffer per slot");
+static_assert(FH_COUNT_ == std::extent<decltype(bm2_ctx::fq_h)>::value, "bm2_ctx::fq_h: one buffer per slot");
 
 }  // namespace
 
@@ -137,32 +141,32 @@ extern "C" int bm2_fastq_encode(bm2_ctx *ctx, const char *buf1, int64_t n1, cons
     const int nbuf = buf2 ? 2 : 1;
     const char *hb[2] = { buf1, buf2 }; const int64_t hn[2] = { n1, buf2 ? n2 : 0 };
     int n_rec[2] = { 0, 0 };
-    if (ctx->ensure(ctx->d[F_MISC], 64)) return 1;
-    int *d_misc = (int *) ctx->d[F_MISC].p;            // [0], [1]: newline counts; [2]: error flag
+    if (ctx->ensure(ctx->fq_d[F_MISC], 64)) return 1;
+    int *d_misc = (int *) ctx->fq_d[F_MISC].p;            // [0], [1]: newline counts; [2]: error flag
     BM2_CUDA_OK(cudaMemsetAsync(d_misc, 0, 64, st));
     for (int b = 0; b < nbuf; ++b) {
-        if (ctx->ensure(ctx->d[F_RAW0 + b], (size_t) hn[b] + 16) || ctx->ensure(ctx->d[F_NL0 + b], ((size_t) hn[b] / 2 + 16) * 4)) return 1;
-        if (hn[b]) BM2_CUDA_OK(cudaMemcpyAsync(ctx->d[F_RAW0 + b].p, hb[b], (size_t) hn[b], cudaMemcpyHostToDevice, st));
+        if (ctx->ensure(ctx->fq_d[F_RAW0 + b], (size_t) hn[b] + 16) || ctx->ensure(ctx->fq_d[F_NL0 + b], ((size_t) hn[b] / 2 + 16) * 4)) return 1;
+        if (hn[b]) BM2_CUDA_OK(cudaMemcpyAsync(ctx->fq_d[F_RAW0 + b].p, hb[b], (size_t) hn[b], cudaMemcpyHostToDevice, st));
         if (hn[b]) {
             size_t tmp = 0;
             cub::CountingInputIterator<int> it(0);
-            IsNewline pred = { (const char *) ctx->d[F_RAW0 + b].p };
+            IsNewline pred = { (const char *) ctx->fq_d[F_RAW0 + b].p };
             {   // the position array holds n / 2 + 16 entries (a four-line record has at most one newline per two bytes): count first,
                 // so that malformed input is an error and not a write past the array
-                NewlineAsInt conv = { (const char *) ctx->d[F_RAW0 + b].p };
+                NewlineAsInt conv = { (const char *) ctx->fq_d[F_RAW0 + b].p };
                 cub::TransformInputIterator<int, NewlineAsInt, cub::CountingInputIterator<int>> cnt_it(it, conv);
                 cub::DeviceReduce::Sum(nullptr, tmp, cnt_it, d_misc + 4 + b, (int) hn[b], st);
-                if (ctx->ensure(ctx->d[F_TMP], tmp)) return 1;
-                BM2_CUDA_OK(cub::DeviceReduce::Sum(ctx->d[F_TMP].p, tmp, cnt_it, d_misc + 4 + b, (int) hn[b], st));
+                if (ctx->ensure(ctx->fq_d[F_TMP], tmp)) return 1;
+                BM2_CUDA_OK(cub::DeviceReduce::Sum(ctx->fq_d[F_TMP].p, tmp, cnt_it, d_misc + 4 + b, (int) hn[b], st));
                 int h_n = 0;
                 BM2_CUDA_OK(cudaMemcpyAsync(&h_n, d_misc + 4 + b, 4, cudaMemcpyDeviceToHost, st));
                 BM2_CUDA_OK(cudaStreamSynchronize(st));
                 if ((int64_t) h_n > hn[b] / 2 + 8) { bm2_set_error(ctx, "bm2_fastq_encode: too many line ends for FASTQ records"); return 2; }
                 tmp = 0;
             }
-            cub::DeviceSelect::If(nullptr, tmp, it, (int32_t *) ctx->d[F_NL0 + b].p, d_misc + b, (int) hn[b], pred, st);
-            if (ctx->ensure(ctx->d[F_TMP], tmp)) return 1;
-            BM2_CUDA_OK(cub::DeviceSelect::If(ctx->d[F_TMP].p, tmp, it, (int32_t *) ctx->d[F_NL0 + b].p, d_misc + b, (int) hn[b], pred, st));
+            cub::DeviceSelect::If(nullptr, tmp, it, (int32_t *) ctx->fq_d[F_NL0 + b].p, d_misc + b, (int) hn[b], pred, st);
+            if (ctx->ensure(ctx->fq_d[F_TMP], tmp)) return 1;
+            BM2_CUDA_OK(cub::DeviceSelect::If(ctx->fq_d[F_TMP].p, tmp, it, (int32_t *) ctx->fq_d[F_NL0 + b].p, d_misc + b, (int) hn[b], pred, st));
         }
     }
     int h_cnt[2] = { 0, 0 };
@@ -172,7 +176,7 @@ extern "C" int bm2_fastq_encode(bm2_ctx *ctx, const char *buf1, int64_t n1, cons
         int lines = h_cnt[b];
         if (hn[b] > 0 && hb[b][hn[b] - 1] != '\n') {      // last line without a newline: a virtual one at the end of the buffer
             const int32_t endpos = (int32_t) hn[b];
-            BM2_CUDA_OK(cudaMemcpyAsync((int32_t *) ctx->d[F_NL0 + b].p + lines, &endpos, 4, cudaMemcpyHostToDevice, st));
+            BM2_CUDA_OK(cudaMemcpyAsync((int32_t *) ctx->fq_d[F_NL0 + b].p + lines, &endpos, 4, cudaMemcpyHostToDevice, st));
             BM2_CUDA_OK(cudaStreamSynchronize(st));
             ++lines;
         }
@@ -182,46 +186,46 @@ extern "C" int bm2_fastq_encode(bm2_ctx *ctx, const char *buf1, int64_t n1, cons
     if (nbuf == 2 && n_rec[0] != n_rec[1]) { bm2_set_error(ctx, "bm2_fastq_encode: the two files hold different numbers of records"); return 2; }
     const int n_reads = n_rec[0] * nbuf;
     out->n_reads = n_reads;
-    if (ctx->ensure(ctx->d[F_SPANS], (size_t) (n_reads + 1) * sizeof(Span)) || ctx->ensure(ctx->d[F_LENS], (size_t) (n_reads + 2) * 8) ||
-        ctx->ensure(ctx->d[F_OFFS], (size_t) (n_reads + 2) * 8)) return 1;
-    Span *d_spans = (Span *) ctx->d[F_SPANS].p; int64_t *d_lens = (int64_t *) ctx->d[F_LENS].p, *d_offs = (int64_t *) ctx->d[F_OFFS].p;
+    if (ctx->ensure(ctx->fq_d[F_SPANS], (size_t) (n_reads + 1) * sizeof(Span)) || ctx->ensure(ctx->fq_d[F_LENS], (size_t) (n_reads + 2) * 8) ||
+        ctx->ensure(ctx->fq_d[F_OFFS], (size_t) (n_reads + 2) * 8)) return 1;
+    Span *d_spans = (Span *) ctx->fq_d[F_SPANS].p; int64_t *d_lens = (int64_t *) ctx->fq_d[F_LENS].p, *d_offs = (int64_t *) ctx->fq_d[F_OFFS].p;
     BM2_CUDA_OK(cudaMemsetAsync(d_lens + n_reads, 0, 8, st));
     for (int b = 0; b < nbuf && n_rec[b] > 0; ++b)
-        fastq_spans_kernel<<<(n_rec[b] + 255) / 256, 256, 0, st>>>((const char *) ctx->d[F_RAW0 + b].p, (const int32_t *) ctx->d[F_NL0 + b].p, n_rec[b], b, nbuf,
+        fastq_spans_kernel<<<(n_rec[b] + 255) / 256, 256, 0, st>>>((const char *) ctx->fq_d[F_RAW0 + b].p, (const int32_t *) ctx->fq_d[F_NL0 + b].p, n_rec[b], b, nbuf,
                                                                       d_spans, d_lens, d_misc + 2);
     {
         size_t tmp = 0;
         cub::DeviceScan::ExclusiveSum(nullptr, tmp, d_lens, d_offs, n_reads + 1, st);
-        if (ctx->ensure(ctx->d[F_TMP], tmp)) return 1;
-        BM2_CUDA_OK(cub::DeviceScan::ExclusiveSum(ctx->d[F_TMP].p, tmp, d_lens, d_offs, n_reads + 1, st));
+        if (ctx->ensure(ctx->fq_d[F_TMP], tmp)) return 1;
+        BM2_CUDA_OK(cub::DeviceScan::ExclusiveSum(ctx->fq_d[F_TMP].p, tmp, d_lens, d_offs, n_reads + 1, st));
     }
     int64_t total = 0; int h_err = 0;
     BM2_CUDA_OK(cudaMemcpyAsync(&total, d_offs + n_reads, 8, cudaMemcpyDeviceToHost, st));
     BM2_CUDA_OK(cudaMemcpyAsync(&h_err, d_misc + 2, 4, cudaMemcpyDeviceToHost, st));
     BM2_CUDA_OK(cudaStreamSynchronize(st));
     if (h_err) { bm2_set_error(ctx, "bm2_fastq_encode: malformed record " + std::to_string(h_err - 1) + " (expected @name / sequence / + / qualities of the same length)"); return 2; }
-    if (ctx->ensure(ctx->d[F_CODES], (size_t) total + 16) || ctx->ensure(ctx->d[F_QUALS], (size_t) total + 16)) return 1;
+    if (ctx->ensure(ctx->fq_d[F_CODES], (size_t) total + 16) || ctx->ensure(ctx->fq_d[F_QUALS], (size_t) total + 16)) return 1;
     if (n_reads > 0) {
         int blocks = (n_reads + 7) / 8; if (blocks > ctx->n_sm * 16) blocks = ctx->n_sm * 16;
-        fastq_encode_kernel<<<blocks, 256, 0, st>>>((const char *) ctx->d[F_RAW0].p, (const char *) ctx->d[F_RAW1].p, d_spans, d_offs, n_reads, nbuf,
-                                                     (uint8_t *) ctx->d[F_CODES].p, (char *) ctx->d[F_QUALS].p);
+        fastq_encode_kernel<<<blocks, 256, 0, st>>>((const char *) ctx->fq_d[F_RAW0].p, (const char *) ctx->fq_d[F_RAW1].p, d_spans, d_offs, n_reads, nbuf,
+                                                     (uint8_t *) ctx->fq_d[F_CODES].p, (char *) ctx->fq_d[F_QUALS].p);
     }
     // host copies: offsets, codes, qualities (the SAM stage and the formatter read them), name positions
-    if (ctx->ensure_host(ctx->h[FH_OFFS], (size_t) (n_reads + 1) * 8) || ctx->ensure_host(ctx->h[FH_CODES], (size_t) total + 16) ||
-        ctx->ensure_host(ctx->h[FH_QUALS], (size_t) total + 16) || ctx->ensure_host(ctx->h[FH_SPANS], (size_t) (n_reads + 1) * sizeof(Span)) ||
-        ctx->ensure_host(ctx->h[FH_NAMEBEG], (size_t) (n_reads + 1) * 8) || ctx->ensure_host(ctx->h[FH_NAMELEN], (size_t) (n_reads + 1) * 4)) return 1;
-    BM2_CUDA_OK(cudaMemcpyAsync(ctx->h[FH_OFFS].p, d_offs, (size_t) (n_reads + 1) * 8, cudaMemcpyDeviceToHost, st));
-    if (total) BM2_CUDA_OK(cudaMemcpyAsync(ctx->h[FH_CODES].p, ctx->d[F_CODES].p, (size_t) total, cudaMemcpyDeviceToHost, st));
-    if (total) BM2_CUDA_OK(cudaMemcpyAsync(ctx->h[FH_QUALS].p, ctx->d[F_QUALS].p, (size_t) total, cudaMemcpyDeviceToHost, st));
-    if (n_reads) BM2_CUDA_OK(cudaMemcpyAsync(ctx->h[FH_SPANS].p, d_spans, (size_t) n_reads * sizeof(Span), cudaMemcpyDeviceToHost, st));
+    if (ctx->ensure_host(ctx->fq_h[FH_OFFS], (size_t) (n_reads + 1) * 8) || ctx->ensure_host(ctx->fq_h[FH_CODES], (size_t) total + 16) ||
+        ctx->ensure_host(ctx->fq_h[FH_QUALS], (size_t) total + 16) || ctx->ensure_host(ctx->fq_h[FH_SPANS], (size_t) (n_reads + 1) * sizeof(Span)) ||
+        ctx->ensure_host(ctx->fq_h[FH_NAMEBEG], (size_t) (n_reads + 1) * 8) || ctx->ensure_host(ctx->fq_h[FH_NAMELEN], (size_t) (n_reads + 1) * 4)) return 1;
+    BM2_CUDA_OK(cudaMemcpyAsync(ctx->fq_h[FH_OFFS].p, d_offs, (size_t) (n_reads + 1) * 8, cudaMemcpyDeviceToHost, st));
+    if (total) BM2_CUDA_OK(cudaMemcpyAsync(ctx->fq_h[FH_CODES].p, ctx->fq_d[F_CODES].p, (size_t) total, cudaMemcpyDeviceToHost, st));
+    if (total) BM2_CUDA_OK(cudaMemcpyAsync(ctx->fq_h[FH_QUALS].p, ctx->fq_d[F_QUALS].p, (size_t) total, cudaMemcpyDeviceToHost, st));
+    if (n_reads) BM2_CUDA_OK(cudaMemcpyAsync(ctx->fq_h[FH_SPANS].p, d_spans, (size_t) n_reads * sizeof(Span), cudaMemcpyDeviceToHost, st));
     BM2_CUDA_OK(cudaStreamSynchronize(st));
     BM2_CUDA_OK(cudaGetLastError());
-    const Span *hs = (const Span *) ctx->h[FH_SPANS].p;
-    int64_t *nb = (int64_t *) ctx->h[FH_NAMEBEG].p; int32_t *nlv = (int32_t *) ctx->h[FH_NAMELEN].p;
+    const Span *hs = (const Span *) ctx->fq_h[FH_SPANS].p;
+    int64_t *nb = (int64_t *) ctx->fq_h[FH_NAMEBEG].p; int32_t *nlv = (int32_t *) ctx->fq_h[FH_NAMELEN].p;
     for (int r = 0; r < n_reads; ++r) { nb[r] = hs[r].name_beg; nlv[r] = hs[r].name_len; }
-    out->d_codes = (const uint8_t *) ctx->d[F_CODES].p; out->d_offsets = d_offs;
-    out->codes = (const uint8_t *) ctx->h[FH_CODES].p; out->offsets = (const int64_t *) ctx->h[FH_OFFS].p;
-    out->quals = (const char *) ctx->h[FH_QUALS].p; out->name_beg = nb; out->name_len = nlv;
+    out->d_codes = (const uint8_t *) ctx->fq_d[F_CODES].p; out->d_offsets = d_offs;
+    out->codes = (const uint8_t *) ctx->fq_h[FH_CODES].p; out->offsets = (const int64_t *) ctx->fq_h[FH_OFFS].p;
+    out->quals = (const char *) ctx->fq_h[FH_QUALS].p; out->name_beg = nb; out->name_len = nlv;
     ctx->fq_n_reads = n_reads; ctx->fq_n_bufs = nbuf;
     return 0;
 }
@@ -229,9 +233,9 @@ extern "C" int bm2_fastq_encode(bm2_ctx *ctx, const char *buf1, int64_t n1, cons
 extern "C" int bm2_fastq_comments(bm2_ctx *ctx, const int64_t **beg, const int32_t **len) {
     if (!ctx || !beg || !len) { if (ctx) bm2_set_error(ctx, "bm2_fastq_comments: bad arguments"); return 1; }
     const int n = ctx->fq_n_reads;
-    if (ctx->ensure_host(ctx->h[FH_CMTBEG], (size_t) (n + 1) * 8) || ctx->ensure_host(ctx->h[FH_CMTLEN], (size_t) (n + 1) * 4)) return 1;
-    const Span *hs = (const Span *) ctx->h[FH_SPANS].p;
-    int64_t *cb = (int64_t *) ctx->h[FH_CMTBEG].p; int32_t *cl = (int32_t *) ctx->h[FH_CMTLEN].p;
+    if (ctx->ensure_host(ctx->fq_h[FH_CMTBEG], (size_t) (n + 1) * 8) || ctx->ensure_host(ctx->fq_h[FH_CMTLEN], (size_t) (n + 1) * 4)) return 1;
+    const Span *hs = (const Span *) ctx->fq_h[FH_SPANS].p;
+    int64_t *cb = (int64_t *) ctx->fq_h[FH_CMTBEG].p; int32_t *cl = (int32_t *) ctx->fq_h[FH_CMTLEN].p;
     for (int r = 0; r < n; ++r) { cb[r] = hs[r].cmt_beg; cl[r] = hs[r].cmt_len; }
     *beg = cb; *len = cl;
     return 0;
@@ -245,60 +249,60 @@ extern "C" int bm2_fastq_smart_pair(bm2_ctx *ctx, bm2_fastq_split *out) {
     cudaStream_t st = ctx->stream;
     const int n = ctx->fq_n_reads;
     memset(out, 0, sizeof *out);
-    if (ctx->ensure(ctx->d[F_KEY], (size_t) (n + 1) * 4) || ctx->ensure(ctx->d[F_RUN], (size_t) (n + 1) * 4) || ctx->ensure(ctx->d[F_SCNT], 16)) return 1;
+    if (ctx->ensure(ctx->fq_d[F_KEY], (size_t) (n + 1) * 4) || ctx->ensure(ctx->fq_d[F_RUN], (size_t) (n + 1) * 4) || ctx->ensure(ctx->fq_d[F_SCNT], 16)) return 1;
     for (int s = 0; s < 2; ++s)
-        if (ctx->ensure(ctx->d[F_SFLAG + s], (size_t) n + 16) || ctx->ensure(ctx->d[F_SIDX + s], (size_t) (n + 1) * 4) ||
-            ctx->ensure(ctx->d[F_SLEN + s], (size_t) (n + 2) * 8) || ctx->ensure(ctx->d[F_SOFF + s], (size_t) (n + 2) * 8)) return 1;
-    const Span *d_spans = (const Span *) ctx->d[F_SPANS].p;
-    const int64_t *d_offs = (const int64_t *) ctx->d[F_OFFS].p;
-    int *d_key = (int *) ctx->d[F_KEY].p, *d_run = (int *) ctx->d[F_RUN].p, *d_cnt = (int *) ctx->d[F_SCNT].p;
+        if (ctx->ensure(ctx->fq_d[F_SFLAG + s], (size_t) n + 16) || ctx->ensure(ctx->fq_d[F_SIDX + s], (size_t) (n + 1) * 4) ||
+            ctx->ensure(ctx->fq_d[F_SLEN + s], (size_t) (n + 2) * 8) || ctx->ensure(ctx->fq_d[F_SOFF + s], (size_t) (n + 2) * 8)) return 1;
+    const Span *d_spans = (const Span *) ctx->fq_d[F_SPANS].p;
+    const int64_t *d_offs = (const int64_t *) ctx->fq_d[F_OFFS].p;
+    int *d_key = (int *) ctx->fq_d[F_KEY].p, *d_run = (int *) ctx->fq_d[F_RUN].p, *d_cnt = (int *) ctx->fq_d[F_SCNT].p;
     int h_cnt[2] = { 0, 0 };
     if (n > 0) {
         const int blocks = (n + 255) / 256;
-        fastq_link_kernel<<<blocks, 256, 0, st>>>((const char *) ctx->d[F_RAW0].p, d_spans, n, d_key);
+        fastq_link_kernel<<<blocks, 256, 0, st>>>((const char *) ctx->fq_d[F_RAW0].p, d_spans, n, d_key);
         size_t tmp = 0;
         cub::DeviceScan::InclusiveScan(nullptr, tmp, d_key, d_run, cub::Max(), n, st);
-        if (ctx->ensure(ctx->d[F_TMP], tmp)) return 1;
-        BM2_CUDA_OK(cub::DeviceScan::InclusiveScan(ctx->d[F_TMP].p, tmp, d_key, d_run, cub::Max(), n, st));
-        fastq_classify_kernel<<<blocks, 256, 0, st>>>(d_run, n, (uint8_t *) ctx->d[F_SFLAG].p, (uint8_t *) ctx->d[F_SFLAG + 1].p);
+        if (ctx->ensure(ctx->fq_d[F_TMP], tmp)) return 1;
+        BM2_CUDA_OK(cub::DeviceScan::InclusiveScan(ctx->fq_d[F_TMP].p, tmp, d_key, d_run, cub::Max(), n, st));
+        fastq_classify_kernel<<<blocks, 256, 0, st>>>(d_run, n, (uint8_t *) ctx->fq_d[F_SFLAG].p, (uint8_t *) ctx->fq_d[F_SFLAG + 1].p);
         cub::CountingInputIterator<int32_t> it(0);
         for (int s = 0; s < 2; ++s) {       // stable compaction: the reads of each set in file order
             tmp = 0;
-            cub::DeviceSelect::Flagged(nullptr, tmp, it, (const uint8_t *) ctx->d[F_SFLAG + s].p, (int32_t *) ctx->d[F_SIDX + s].p, d_cnt + s, n, st);
-            if (ctx->ensure(ctx->d[F_TMP], tmp)) return 1;
-            BM2_CUDA_OK(cub::DeviceSelect::Flagged(ctx->d[F_TMP].p, tmp, it, (const uint8_t *) ctx->d[F_SFLAG + s].p, (int32_t *) ctx->d[F_SIDX + s].p,
+            cub::DeviceSelect::Flagged(nullptr, tmp, it, (const uint8_t *) ctx->fq_d[F_SFLAG + s].p, (int32_t *) ctx->fq_d[F_SIDX + s].p, d_cnt + s, n, st);
+            if (ctx->ensure(ctx->fq_d[F_TMP], tmp)) return 1;
+            BM2_CUDA_OK(cub::DeviceSelect::Flagged(ctx->fq_d[F_TMP].p, tmp, it, (const uint8_t *) ctx->fq_d[F_SFLAG + s].p, (int32_t *) ctx->fq_d[F_SIDX + s].p,
                                                    d_cnt + s, n, st));
         }
         BM2_CUDA_OK(cudaMemcpyAsync(h_cnt, d_cnt, 8, cudaMemcpyDeviceToHost, st));
         BM2_CUDA_OK(cudaStreamSynchronize(st));
     }
-    const Span *hs = (const Span *) ctx->h[FH_SPANS].p;
+    const Span *hs = (const Span *) ctx->fq_h[FH_SPANS].p;
     for (int s = 0; s < 2; ++s) {
         const int m = h_cnt[s];
-        const int32_t *d_idx = (const int32_t *) ctx->d[F_SIDX + s].p;
-        int64_t *d_len = (int64_t *) ctx->d[F_SLEN + s].p, *d_soff = (int64_t *) ctx->d[F_SOFF + s].p;
+        const int32_t *d_idx = (const int32_t *) ctx->fq_d[F_SIDX + s].p;
+        int64_t *d_len = (int64_t *) ctx->fq_d[F_SLEN + s].p, *d_soff = (int64_t *) ctx->fq_d[F_SOFF + s].p;
         fastq_gather_lens_kernel<<<(m + 1 + 255) / 256, 256, 0, st>>>(d_idx, d_offs, m, d_len);
         size_t tmp = 0;
         cub::DeviceScan::ExclusiveSum(nullptr, tmp, d_len, d_soff, m + 1, st);
-        if (ctx->ensure(ctx->d[F_TMP], tmp)) return 1;
-        BM2_CUDA_OK(cub::DeviceScan::ExclusiveSum(ctx->d[F_TMP].p, tmp, d_len, d_soff, m + 1, st));
+        if (ctx->ensure(ctx->fq_d[F_TMP], tmp)) return 1;
+        BM2_CUDA_OK(cub::DeviceScan::ExclusiveSum(ctx->fq_d[F_TMP].p, tmp, d_len, d_soff, m + 1, st));
         int64_t total = 0;
         BM2_CUDA_OK(cudaMemcpyAsync(&total, d_soff + m, 8, cudaMemcpyDeviceToHost, st));
         BM2_CUDA_OK(cudaStreamSynchronize(st));
-        if (ctx->ensure(ctx->d[F_SCODES + s], (size_t) total + 16) || ctx->ensure(ctx->d[F_SQUALS + s], (size_t) total + 16)) return 1;
+        if (ctx->ensure(ctx->fq_d[F_SCODES + s], (size_t) total + 16) || ctx->ensure(ctx->fq_d[F_SQUALS + s], (size_t) total + 16)) return 1;
         if (m > 0) {
             int blocks = (m + 7) / 8; if (blocks > ctx->n_sm * 16) blocks = ctx->n_sm * 16;
-            fastq_gather_kernel<<<blocks, 256, 0, st>>>(d_idx, d_offs, d_soff, m, (const uint8_t *) ctx->d[F_CODES].p, (const char *) ctx->d[F_QUALS].p,
-                                                        (uint8_t *) ctx->d[F_SCODES + s].p, (char *) ctx->d[F_SQUALS + s].p);
+            fastq_gather_kernel<<<blocks, 256, 0, st>>>(d_idx, d_offs, d_soff, m, (const uint8_t *) ctx->fq_d[F_CODES].p, (const char *) ctx->fq_d[F_QUALS].p,
+                                                        (uint8_t *) ctx->fq_d[F_SCODES + s].p, (char *) ctx->fq_d[F_SQUALS + s].p);
         }
-        HostBuf *h = ctx->h + FH_SPLIT + 8 * s;
+        HostBuf *h = ctx->fq_h + FH_SPLIT + SH_COUNT_ * s;
         if (ctx->ensure_host(h[SH_OFFS], (size_t) (m + 1) * 8) || ctx->ensure_host(h[SH_CODES], (size_t) total + 16) ||
             ctx->ensure_host(h[SH_QUALS], (size_t) total + 16) || ctx->ensure_host(h[SH_NAMEBEG], (size_t) (m + 1) * 8) ||
             ctx->ensure_host(h[SH_NAMELEN], (size_t) (m + 1) * 4) || ctx->ensure_host(h[SH_CMTBEG], (size_t) (m + 1) * 8) ||
             ctx->ensure_host(h[SH_CMTLEN], (size_t) (m + 1) * 4) || ctx->ensure_host(h[SH_IDX], (size_t) (m + 1) * 4)) return 1;
         BM2_CUDA_OK(cudaMemcpyAsync(h[SH_OFFS].p, d_soff, (size_t) (m + 1) * 8, cudaMemcpyDeviceToHost, st));
-        if (total) BM2_CUDA_OK(cudaMemcpyAsync(h[SH_CODES].p, ctx->d[F_SCODES + s].p, (size_t) total, cudaMemcpyDeviceToHost, st));
-        if (total) BM2_CUDA_OK(cudaMemcpyAsync(h[SH_QUALS].p, ctx->d[F_SQUALS + s].p, (size_t) total, cudaMemcpyDeviceToHost, st));
+        if (total) BM2_CUDA_OK(cudaMemcpyAsync(h[SH_CODES].p, ctx->fq_d[F_SCODES + s].p, (size_t) total, cudaMemcpyDeviceToHost, st));
+        if (total) BM2_CUDA_OK(cudaMemcpyAsync(h[SH_QUALS].p, ctx->fq_d[F_SQUALS + s].p, (size_t) total, cudaMemcpyDeviceToHost, st));
         if (m) BM2_CUDA_OK(cudaMemcpyAsync(h[SH_IDX].p, d_idx, (size_t) m * 4, cudaMemcpyDeviceToHost, st));
         BM2_CUDA_OK(cudaStreamSynchronize(st));
         BM2_CUDA_OK(cudaGetLastError());
@@ -308,7 +312,7 @@ extern "C" int bm2_fastq_smart_pair(bm2_ctx *ctx, bm2_fastq_split *out) {
         for (int j = 0; j < m; ++j) { const Span &sp = hs[idx[j]]; nb[j] = sp.name_beg; nlv[j] = sp.name_len; cb[j] = sp.cmt_beg; cl[j] = sp.cmt_len; }
         bm2_fastq_batch &b = out->set[s];
         b.n_reads = m;
-        b.d_codes = (const uint8_t *) ctx->d[F_SCODES + s].p; b.d_offsets = d_soff;
+        b.d_codes = (const uint8_t *) ctx->fq_d[F_SCODES + s].p; b.d_offsets = d_soff;
         b.codes = (const uint8_t *) h[SH_CODES].p; b.offsets = (const int64_t *) h[SH_OFFS].p; b.quals = (const char *) h[SH_QUALS].p;
         b.name_beg = nb; b.name_len = nlv;
         out->comment_beg[s] = cb; out->comment_len[s] = cl; out->read_index[s] = idx;
@@ -416,10 +420,6 @@ __global__ void seq_gather_kernel(SeqTableSrc s0, SeqTableSrc s1, const Span *__
     }
 }
 
-enum SeqBuf { S_HP0 = 128, S_HP1, S_CAND, S_CANDU, S_INFO, S_JUMP, S_MARK, S_FLAG, S_REC0, S_REC1, S_QP, S_CNT };
-enum SeqHost { FH_QP = 48 };
-static_assert(S_CNT < 144, "bm2_ctx::d[] slots");
-
 }  // namespace
 
 extern "C" int bm2_seq_encode(bm2_ctx *ctx, const char *buf1, int64_t n1, const char *buf2, int64_t n2, bm2_fastq_batch *out, const uint8_t **qual_present) {
@@ -434,63 +434,63 @@ extern "C" int bm2_seq_encode(bm2_ctx *ctx, const char *buf1, int64_t n1, const 
     int n_rec[2] = { 0, 0 };
     SeqTableSrc src[2] = {};
     int bad[2] = { -1, -1 };                                       // per buffer: index of the malformed record, -1: none
-    if (ctx->ensure(ctx->d[S_CNT], 64)) return 1;
-    int *d_cnt = (int *) ctx->d[S_CNT].p;
+    if (ctx->ensure(ctx->fq_d[S_CNT], 64)) return 1;
+    int *d_cnt = (int *) ctx->fq_d[S_CNT].p;
     // compaction of the positions i < n where pred(raw[i]) into slot `dst` (counted first to size it)
     auto positions = [&](int b, int slot, bool newline, int *count) -> int {
-        const char *d_raw = (const char *) ctx->d[F_RAW0 + b].p;
+        const char *d_raw = (const char *) ctx->fq_d[F_RAW0 + b].p;
         cub::CountingInputIterator<int> it(0);
         size_t tmp = 0;
         int h_n = 0;
         if (newline) {
             cub::TransformInputIterator<int, NewlineAsInt, cub::CountingInputIterator<int>> cnt_it(it, NewlineAsInt{ d_raw });
             cub::DeviceReduce::Sum(nullptr, tmp, cnt_it, d_cnt, (int) hn[b], st);
-            if (ctx->ensure(ctx->d[F_TMP], tmp)) return 1;
-            BM2_CUDA_OK(cub::DeviceReduce::Sum(ctx->d[F_TMP].p, tmp, cnt_it, d_cnt, (int) hn[b], st));
+            if (ctx->ensure(ctx->fq_d[F_TMP], tmp)) return 1;
+            BM2_CUDA_OK(cub::DeviceReduce::Sum(ctx->fq_d[F_TMP].p, tmp, cnt_it, d_cnt, (int) hn[b], st));
         } else {
             cub::TransformInputIterator<int, HeaderCharAsInt, cub::CountingInputIterator<int>> cnt_it(it, HeaderCharAsInt{ d_raw });
             cub::DeviceReduce::Sum(nullptr, tmp, cnt_it, d_cnt, (int) hn[b], st);
-            if (ctx->ensure(ctx->d[F_TMP], tmp)) return 1;
-            BM2_CUDA_OK(cub::DeviceReduce::Sum(ctx->d[F_TMP].p, tmp, cnt_it, d_cnt, (int) hn[b], st));
+            if (ctx->ensure(ctx->fq_d[F_TMP], tmp)) return 1;
+            BM2_CUDA_OK(cub::DeviceReduce::Sum(ctx->fq_d[F_TMP].p, tmp, cnt_it, d_cnt, (int) hn[b], st));
         }
         BM2_CUDA_OK(cudaMemcpyAsync(&h_n, d_cnt, 4, cudaMemcpyDeviceToHost, st));
         BM2_CUDA_OK(cudaStreamSynchronize(st));
-        if (ctx->ensure(ctx->d[slot], ((size_t) h_n + 16) * 4)) return 1;
+        if (ctx->ensure(ctx->fq_d[slot], ((size_t) h_n + 16) * 4)) return 1;
         tmp = 0;
         if (newline) {
             IsNewline pred = { d_raw };
-            cub::DeviceSelect::If(nullptr, tmp, it, (int32_t *) ctx->d[slot].p, d_cnt, (int) hn[b], pred, st);
-            if (ctx->ensure(ctx->d[F_TMP], tmp)) return 1;
-            BM2_CUDA_OK(cub::DeviceSelect::If(ctx->d[F_TMP].p, tmp, it, (int32_t *) ctx->d[slot].p, d_cnt, (int) hn[b], pred, st));
+            cub::DeviceSelect::If(nullptr, tmp, it, (int32_t *) ctx->fq_d[slot].p, d_cnt, (int) hn[b], pred, st);
+            if (ctx->ensure(ctx->fq_d[F_TMP], tmp)) return 1;
+            BM2_CUDA_OK(cub::DeviceSelect::If(ctx->fq_d[F_TMP].p, tmp, it, (int32_t *) ctx->fq_d[slot].p, d_cnt, (int) hn[b], pred, st));
         } else {
             IsHeaderChar pred = { d_raw };
-            cub::DeviceSelect::If(nullptr, tmp, it, (int32_t *) ctx->d[slot].p, d_cnt, (int) hn[b], pred, st);
-            if (ctx->ensure(ctx->d[F_TMP], tmp)) return 1;
-            BM2_CUDA_OK(cub::DeviceSelect::If(ctx->d[F_TMP].p, tmp, it, (int32_t *) ctx->d[slot].p, d_cnt, (int) hn[b], pred, st));
+            cub::DeviceSelect::If(nullptr, tmp, it, (int32_t *) ctx->fq_d[slot].p, d_cnt, (int) hn[b], pred, st);
+            if (ctx->ensure(ctx->fq_d[F_TMP], tmp)) return 1;
+            BM2_CUDA_OK(cub::DeviceSelect::If(ctx->fq_d[F_TMP].p, tmp, it, (int32_t *) ctx->fq_d[slot].p, d_cnt, (int) hn[b], pred, st));
         }
         *count = h_n;
         return 0;
     };
     for (int b = 0; b < nbuf; ++b) {
-        if (ctx->ensure(ctx->d[F_RAW0 + b], (size_t) hn[b] + 16)) return 1;
-        if (hn[b]) BM2_CUDA_OK(cudaMemcpyAsync(ctx->d[F_RAW0 + b].p, hb[b], (size_t) hn[b], cudaMemcpyHostToDevice, st));
+        if (ctx->ensure(ctx->fq_d[F_RAW0 + b], (size_t) hn[b] + 16)) return 1;
+        if (hn[b]) BM2_CUDA_OK(cudaMemcpyAsync(ctx->fq_d[F_RAW0 + b].p, hb[b], (size_t) hn[b], cudaMemcpyHostToDevice, st));
         int n_nl = 0, n_hp = 0;
         if (hn[b] && (positions(b, F_NL0 + b, true, &n_nl) || positions(b, S_HP0 + b, false, &n_hp))) return 1;
-        if (!hn[b] && (ctx->ensure(ctx->d[F_NL0 + b], 64) || ctx->ensure(ctx->d[S_HP0 + b], 64))) return 1;
+        if (!hn[b] && (ctx->ensure(ctx->fq_d[F_NL0 + b], 64) || ctx->ensure(ctx->fq_d[S_HP0 + b], 64))) return 1;
         SeqTableSrc &s = src[b];
-        s.raw = (const char *) ctx->d[F_RAW0 + b].p; s.n = hn[b]; s.nl = (const int32_t *) ctx->d[F_NL0 + b].p; s.n_nl = n_nl;
-        s.hp = (const int32_t *) ctx->d[S_HP0 + b].p; s.n_hp = n_hp; s.k = 0;
-        if (n_hp == 0) { n_rec[b] = 0; if (ctx->ensure(ctx->d[S_REC0 + b], 64)) return 1; continue; }
+        s.raw = (const char *) ctx->fq_d[F_RAW0 + b].p; s.n = hn[b]; s.nl = (const int32_t *) ctx->fq_d[F_NL0 + b].p; s.n_nl = n_nl;
+        s.hp = (const int32_t *) ctx->fq_d[S_HP0 + b].p; s.n_hp = n_hp; s.k = 0;
+        if (n_hp == 0) { n_rec[b] = 0; if (ctx->ensure(ctx->fq_d[S_REC0 + b], 64)) return 1; continue; }
         // candidates: the first header character at or after each line start, deduplicated (non-decreasing in the line index)
         const int n_ls = n_nl + 1;
-        if (ctx->ensure(ctx->d[S_CAND], (size_t) (n_ls + 16) * 4) || ctx->ensure(ctx->d[S_CANDU], (size_t) (n_ls + 16) * 4)) return 1;
-        int32_t *d_cand = (int32_t *) ctx->d[S_CAND].p, *d_cu = (int32_t *) ctx->d[S_CANDU].p;
+        if (ctx->ensure(ctx->fq_d[S_CAND], (size_t) (n_ls + 16) * 4) || ctx->ensure(ctx->fq_d[S_CANDU], (size_t) (n_ls + 16) * 4)) return 1;
+        int32_t *d_cand = (int32_t *) ctx->fq_d[S_CAND].p, *d_cu = (int32_t *) ctx->fq_d[S_CANDU].p;
         seq_cand_kernel<<<(n_ls + 255) / 256, 256, 0, st>>>(s, d_cand);
         {
             size_t tmp = 0;
             cub::DeviceSelect::Unique(nullptr, tmp, d_cand, d_cu, d_cnt, n_ls, st);
-            if (ctx->ensure(ctx->d[F_TMP], tmp)) return 1;
-            BM2_CUDA_OK(cub::DeviceSelect::Unique(ctx->d[F_TMP].p, tmp, d_cand, d_cu, d_cnt, n_ls, st));
+            if (ctx->ensure(ctx->fq_d[F_TMP], tmp)) return 1;
+            BM2_CUDA_OK(cub::DeviceSelect::Unique(ctx->fq_d[F_TMP].p, tmp, d_cand, d_cu, d_cnt, n_ls, st));
         }
         int K = 0;
         BM2_CUDA_OK(cudaMemcpyAsync(&K, d_cnt, 4, cudaMemcpyDeviceToHost, st));
@@ -501,12 +501,12 @@ extern "C" int bm2_seq_encode(bm2_ctx *ctx, const char *buf1, int64_t n1, const 
         if (last >= hn[b]) --K;                         // "no header character after this line"
         // next() of every candidate, then the jump tables J_t = next^(2^t), t < T with 2^T > K
         int T = 1; while ((1LL << T) <= K) ++T;
-        if (ctx->ensure(ctx->d[S_INFO], (size_t) (K + 1) * sizeof(SeqCand)) || ctx->ensure(ctx->d[S_JUMP], (size_t) T * (K + 1) * 4) ||
-            ctx->ensure(ctx->d[S_MARK], (size_t) K + 16) || ctx->ensure(ctx->d[S_FLAG], (size_t) K + 16) ||
-            ctx->ensure(ctx->d[S_REC0 + b], (size_t) (K + 1) * sizeof(SeqCand))) return 1;
-        int32_t *d_jump = (int32_t *) ctx->d[S_JUMP].p;
-        SeqCand *d_info = (SeqCand *) ctx->d[S_INFO].p;
-        uint8_t *d_mark = (uint8_t *) ctx->d[S_MARK].p, *d_flag = (uint8_t *) ctx->d[S_FLAG].p;
+        if (ctx->ensure(ctx->fq_d[S_INFO], (size_t) (K + 1) * sizeof(SeqCand)) || ctx->ensure(ctx->fq_d[S_JUMP], (size_t) T * (K + 1) * 4) ||
+            ctx->ensure(ctx->fq_d[S_MARK], (size_t) K + 16) || ctx->ensure(ctx->fq_d[S_FLAG], (size_t) K + 16) ||
+            ctx->ensure(ctx->fq_d[S_REC0 + b], (size_t) (K + 1) * sizeof(SeqCand))) return 1;
+        int32_t *d_jump = (int32_t *) ctx->fq_d[S_JUMP].p;
+        SeqCand *d_info = (SeqCand *) ctx->fq_d[S_INFO].p;
+        uint8_t *d_mark = (uint8_t *) ctx->fq_d[S_MARK].p, *d_flag = (uint8_t *) ctx->fq_d[S_FLAG].p;
         const int gK = (K + 1 + 255) / 256;
         seq_walk_kernel<<<gK, 256, 0, st>>>(s, d_cu, K, d_jump, d_info);
         for (int t = 1; t < T; ++t) seq_jump_kernel<<<gK, 256, 0, st>>>(d_jump + (size_t) (t - 1) * (K + 1), K, d_jump + (size_t) t * (K + 1));
@@ -516,16 +516,16 @@ extern "C" int bm2_seq_encode(bm2_ctx *ctx, const char *buf1, int64_t n1, const 
         seq_flag_kernel<<<gK, 256, 0, st>>>(d_mark, d_info, K, d_flag);
         {
             size_t tmp = 0;
-            cub::DeviceSelect::Flagged(nullptr, tmp, d_info, d_flag, (SeqCand *) ctx->d[S_REC0 + b].p, d_cnt, K, st);
-            if (ctx->ensure(ctx->d[F_TMP], tmp)) return 1;
-            BM2_CUDA_OK(cub::DeviceSelect::Flagged(ctx->d[F_TMP].p, tmp, d_info, d_flag, (SeqCand *) ctx->d[S_REC0 + b].p, d_cnt, K, st));
+            cub::DeviceSelect::Flagged(nullptr, tmp, d_info, d_flag, (SeqCand *) ctx->fq_d[S_REC0 + b].p, d_cnt, K, st);
+            if (ctx->ensure(ctx->fq_d[F_TMP], tmp)) return 1;
+            BM2_CUDA_OK(cub::DeviceSelect::Flagged(ctx->fq_d[F_TMP].p, tmp, d_info, d_flag, (SeqCand *) ctx->fq_d[S_REC0 + b].p, d_cnt, K, st));
         }
         BM2_CUDA_OK(cudaMemcpyAsync(&n_rec[b], d_cnt, 4, cudaMemcpyDeviceToHost, st));
         BM2_CUDA_OK(cudaStreamSynchronize(st));
         // a malformed record ends its chain (its next() is K), so only the last record of the buffer can be one
         if (n_rec[b] > 0) {
             SeqCand lastc;
-            BM2_CUDA_OK(cudaMemcpyAsync(&lastc, (const SeqCand *) ctx->d[S_REC0 + b].p + n_rec[b] - 1, sizeof lastc, cudaMemcpyDeviceToHost, st));
+            BM2_CUDA_OK(cudaMemcpyAsync(&lastc, (const SeqCand *) ctx->fq_d[S_REC0 + b].p + n_rec[b] - 1, sizeof lastc, cudaMemcpyDeviceToHost, st));
             BM2_CUDA_OK(cudaStreamSynchronize(st));
             if (lastc.status == SEQ_BAD) bad[b] = n_rec[b] - 1;
         }
@@ -539,46 +539,46 @@ extern "C" int bm2_seq_encode(bm2_ctx *ctx, const char *buf1, int64_t n1, const 
     if (nbuf == 2 && n_rec[0] != n_rec[1]) { bm2_set_error(ctx, "bm2_seq_encode: the two files hold different numbers of records"); return 2; }
     const int n_reads = n_rec[0] * nbuf;
     out->n_reads = n_reads;
-    if (ctx->ensure(ctx->d[F_SPANS], (size_t) (n_reads + 1) * sizeof(Span)) || ctx->ensure(ctx->d[F_LENS], (size_t) (n_reads + 2) * 8) ||
-        ctx->ensure(ctx->d[F_OFFS], (size_t) (n_reads + 2) * 8) || ctx->ensure(ctx->d[S_QP], (size_t) n_reads + 16)) return 1;
-    Span *d_spans = (Span *) ctx->d[F_SPANS].p; int64_t *d_lens = (int64_t *) ctx->d[F_LENS].p, *d_offs = (int64_t *) ctx->d[F_OFFS].p;
-    uint8_t *d_qp = (uint8_t *) ctx->d[S_QP].p;
+    if (ctx->ensure(ctx->fq_d[F_SPANS], (size_t) (n_reads + 1) * sizeof(Span)) || ctx->ensure(ctx->fq_d[F_LENS], (size_t) (n_reads + 2) * 8) ||
+        ctx->ensure(ctx->fq_d[F_OFFS], (size_t) (n_reads + 2) * 8) || ctx->ensure(ctx->fq_d[S_QP], (size_t) n_reads + 16)) return 1;
+    Span *d_spans = (Span *) ctx->fq_d[F_SPANS].p; int64_t *d_lens = (int64_t *) ctx->fq_d[F_LENS].p, *d_offs = (int64_t *) ctx->fq_d[F_OFFS].p;
+    uint8_t *d_qp = (uint8_t *) ctx->fq_d[S_QP].p;
     BM2_CUDA_OK(cudaMemsetAsync(d_lens + n_reads, 0, 8, st));
     for (int b = 0; b < nbuf && n_rec[b] > 0; ++b)
-        seq_span_kernel<<<(n_rec[b] + 255) / 256, 256, 0, st>>>((const SeqCand *) ctx->d[S_REC0 + b].p, n_rec[b], b, nbuf, d_spans, d_lens, d_qp);
+        seq_span_kernel<<<(n_rec[b] + 255) / 256, 256, 0, st>>>((const SeqCand *) ctx->fq_d[S_REC0 + b].p, n_rec[b], b, nbuf, d_spans, d_lens, d_qp);
     {
         size_t tmp = 0;
         cub::DeviceScan::ExclusiveSum(nullptr, tmp, d_lens, d_offs, n_reads + 1, st);
-        if (ctx->ensure(ctx->d[F_TMP], tmp)) return 1;
-        BM2_CUDA_OK(cub::DeviceScan::ExclusiveSum(ctx->d[F_TMP].p, tmp, d_lens, d_offs, n_reads + 1, st));
+        if (ctx->ensure(ctx->fq_d[F_TMP], tmp)) return 1;
+        BM2_CUDA_OK(cub::DeviceScan::ExclusiveSum(ctx->fq_d[F_TMP].p, tmp, d_lens, d_offs, n_reads + 1, st));
     }
     int64_t total = 0;
     BM2_CUDA_OK(cudaMemcpyAsync(&total, d_offs + n_reads, 8, cudaMemcpyDeviceToHost, st));
     BM2_CUDA_OK(cudaStreamSynchronize(st));
-    if (ctx->ensure(ctx->d[F_CODES], (size_t) total + 16) || ctx->ensure(ctx->d[F_QUALS], (size_t) total + 16)) return 1;
+    if (ctx->ensure(ctx->fq_d[F_CODES], (size_t) total + 16) || ctx->ensure(ctx->fq_d[F_QUALS], (size_t) total + 16)) return 1;
     if (n_reads > 0) {
         int blocks = (n_reads + 7) / 8; if (blocks > ctx->n_sm * 16) blocks = ctx->n_sm * 16;
-        seq_gather_kernel<<<blocks, 256, 0, st>>>(src[0], nbuf == 2 ? src[1] : src[0], d_spans, d_offs, n_reads, nbuf, (uint8_t *) ctx->d[F_CODES].p,
-                                                  (char *) ctx->d[F_QUALS].p);
+        seq_gather_kernel<<<blocks, 256, 0, st>>>(src[0], nbuf == 2 ? src[1] : src[0], d_spans, d_offs, n_reads, nbuf, (uint8_t *) ctx->fq_d[F_CODES].p,
+                                                  (char *) ctx->fq_d[F_QUALS].p);
     }
-    if (ctx->ensure_host(ctx->h[FH_OFFS], (size_t) (n_reads + 1) * 8) || ctx->ensure_host(ctx->h[FH_CODES], (size_t) total + 16) ||
-        ctx->ensure_host(ctx->h[FH_QUALS], (size_t) total + 16) || ctx->ensure_host(ctx->h[FH_SPANS], (size_t) (n_reads + 1) * sizeof(Span)) ||
-        ctx->ensure_host(ctx->h[FH_NAMEBEG], (size_t) (n_reads + 1) * 8) || ctx->ensure_host(ctx->h[FH_NAMELEN], (size_t) (n_reads + 1) * 4) ||
-        ctx->ensure_host(ctx->h[FH_QP], (size_t) n_reads + 16)) return 1;
-    BM2_CUDA_OK(cudaMemcpyAsync(ctx->h[FH_OFFS].p, d_offs, (size_t) (n_reads + 1) * 8, cudaMemcpyDeviceToHost, st));
-    if (total) BM2_CUDA_OK(cudaMemcpyAsync(ctx->h[FH_CODES].p, ctx->d[F_CODES].p, (size_t) total, cudaMemcpyDeviceToHost, st));
-    if (total) BM2_CUDA_OK(cudaMemcpyAsync(ctx->h[FH_QUALS].p, ctx->d[F_QUALS].p, (size_t) total, cudaMemcpyDeviceToHost, st));
-    if (n_reads) BM2_CUDA_OK(cudaMemcpyAsync(ctx->h[FH_SPANS].p, d_spans, (size_t) n_reads * sizeof(Span), cudaMemcpyDeviceToHost, st));
-    if (n_reads) BM2_CUDA_OK(cudaMemcpyAsync(ctx->h[FH_QP].p, d_qp, (size_t) n_reads, cudaMemcpyDeviceToHost, st));
+    if (ctx->ensure_host(ctx->fq_h[FH_OFFS], (size_t) (n_reads + 1) * 8) || ctx->ensure_host(ctx->fq_h[FH_CODES], (size_t) total + 16) ||
+        ctx->ensure_host(ctx->fq_h[FH_QUALS], (size_t) total + 16) || ctx->ensure_host(ctx->fq_h[FH_SPANS], (size_t) (n_reads + 1) * sizeof(Span)) ||
+        ctx->ensure_host(ctx->fq_h[FH_NAMEBEG], (size_t) (n_reads + 1) * 8) || ctx->ensure_host(ctx->fq_h[FH_NAMELEN], (size_t) (n_reads + 1) * 4) ||
+        ctx->ensure_host(ctx->fq_h[FH_QP], (size_t) n_reads + 16)) return 1;
+    BM2_CUDA_OK(cudaMemcpyAsync(ctx->fq_h[FH_OFFS].p, d_offs, (size_t) (n_reads + 1) * 8, cudaMemcpyDeviceToHost, st));
+    if (total) BM2_CUDA_OK(cudaMemcpyAsync(ctx->fq_h[FH_CODES].p, ctx->fq_d[F_CODES].p, (size_t) total, cudaMemcpyDeviceToHost, st));
+    if (total) BM2_CUDA_OK(cudaMemcpyAsync(ctx->fq_h[FH_QUALS].p, ctx->fq_d[F_QUALS].p, (size_t) total, cudaMemcpyDeviceToHost, st));
+    if (n_reads) BM2_CUDA_OK(cudaMemcpyAsync(ctx->fq_h[FH_SPANS].p, d_spans, (size_t) n_reads * sizeof(Span), cudaMemcpyDeviceToHost, st));
+    if (n_reads) BM2_CUDA_OK(cudaMemcpyAsync(ctx->fq_h[FH_QP].p, d_qp, (size_t) n_reads, cudaMemcpyDeviceToHost, st));
     BM2_CUDA_OK(cudaStreamSynchronize(st));
     BM2_CUDA_OK(cudaGetLastError());
-    const Span *hs = (const Span *) ctx->h[FH_SPANS].p;
-    int64_t *nb = (int64_t *) ctx->h[FH_NAMEBEG].p; int32_t *nlv = (int32_t *) ctx->h[FH_NAMELEN].p;
+    const Span *hs = (const Span *) ctx->fq_h[FH_SPANS].p;
+    int64_t *nb = (int64_t *) ctx->fq_h[FH_NAMEBEG].p; int32_t *nlv = (int32_t *) ctx->fq_h[FH_NAMELEN].p;
     for (int r = 0; r < n_reads; ++r) { nb[r] = hs[r].name_beg; nlv[r] = hs[r].name_len; }
-    out->d_codes = (const uint8_t *) ctx->d[F_CODES].p; out->d_offsets = d_offs;
-    out->codes = (const uint8_t *) ctx->h[FH_CODES].p; out->offsets = (const int64_t *) ctx->h[FH_OFFS].p;
-    out->quals = (const char *) ctx->h[FH_QUALS].p; out->name_beg = nb; out->name_len = nlv;
-    if (qual_present) *qual_present = (const uint8_t *) ctx->h[FH_QP].p;
+    out->d_codes = (const uint8_t *) ctx->fq_d[F_CODES].p; out->d_offsets = d_offs;
+    out->codes = (const uint8_t *) ctx->fq_h[FH_CODES].p; out->offsets = (const int64_t *) ctx->fq_h[FH_OFFS].p;
+    out->quals = (const char *) ctx->fq_h[FH_QUALS].p; out->name_beg = nb; out->name_len = nlv;
+    if (qual_present) *qual_present = (const uint8_t *) ctx->fq_h[FH_QP].p;
     ctx->fq_n_reads = n_reads; ctx->fq_n_bufs = nbuf;
     return 0;
 }

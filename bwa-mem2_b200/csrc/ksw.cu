@@ -13,8 +13,8 @@
 #include <cstring>
 
 namespace {
-enum { KB_SEQ = 84, KB_REQ, KB_LISTOFF, KB_LIST, KB_RES, KB_OVF };
-static_assert(KB_OVF < 96, "bm2_ctx::d[] too small");
+enum { KB_SEQ, KB_REQ, KB_LISTOFF, KB_LIST, KB_RES, KB_OVF, KB_COUNT_ };
+static_assert(KB_COUNT_ == std::extent<decltype(bm2_ctx::ksw_d)>::value, "bm2_ctx::ksw_d: one buffer per slot");
 struct KswMat { int8_t m[25]; };
 
 template <int TMAX>
@@ -41,7 +41,7 @@ ksw_warp_kernel(KswMat mat, int o_del, int e_del, int o_ins, int e_ins, const ui
         __syncwarp(0xffffffffu);
     }
 }
-template <class T> T *P(bm2_ctx *ctx, int b) { return (T *) ctx->d[b].p; }
+template <class T> T *P(bm2_ctx *ctx, int b) { return (T *) ctx->ksw_d[b].p; }
 }  // namespace
 
 extern "C" int bm2_ksw_align2(bm2_ctx *ctx, const uint8_t *seqs, int64_t n_seq_bytes, const bm2_ksw_req *reqs, int64_t n, bm2_ksw_res *out)
@@ -68,13 +68,13 @@ extern "C" int bm2_ksw_align2(bm2_ctx *ctx, const uint8_t *seqs, int64_t n_seq_b
         tot += 2 * ((int64_t) q.tlen / 2 + 2);
     }
     list_off[(size_t) n] = tot;
-    if (ctx->ensure(ctx->d[KB_SEQ], (size_t) n_seq_bytes + 16) || ctx->ensure(ctx->d[KB_REQ], (size_t) n * sizeof(bm2_ksw_req)) ||
-        ctx->ensure(ctx->d[KB_LISTOFF], (size_t) (n + 1) * 8) || ctx->ensure(ctx->d[KB_LIST], (size_t) tot * 4 + 16) ||
-        ctx->ensure(ctx->d[KB_RES], (size_t) n * sizeof(bm2_ksw_res)) || ctx->ensure(ctx->d[KB_OVF], 16)) return 1;
-    BM2_CUDA_OK(cudaMemcpyAsync(ctx->d[KB_SEQ].p, seqs, (size_t) n_seq_bytes, cudaMemcpyHostToDevice, st));
-    BM2_CUDA_OK(cudaMemcpyAsync(ctx->d[KB_REQ].p, reqs, (size_t) n * sizeof(bm2_ksw_req), cudaMemcpyHostToDevice, st));
-    BM2_CUDA_OK(cudaMemcpyAsync(ctx->d[KB_LISTOFF].p, list_off.data(), (size_t) (n + 1) * 8, cudaMemcpyHostToDevice, st));
-    BM2_CUDA_OK(cudaMemsetAsync(ctx->d[KB_OVF].p, 0, 4, st));
+    if (ctx->ensure(ctx->ksw_d[KB_SEQ], (size_t) n_seq_bytes + 16) || ctx->ensure(ctx->ksw_d[KB_REQ], (size_t) n * sizeof(bm2_ksw_req)) ||
+        ctx->ensure(ctx->ksw_d[KB_LISTOFF], (size_t) (n + 1) * 8) || ctx->ensure(ctx->ksw_d[KB_LIST], (size_t) tot * 4 + 16) ||
+        ctx->ensure(ctx->ksw_d[KB_RES], (size_t) n * sizeof(bm2_ksw_res)) || ctx->ensure(ctx->ksw_d[KB_OVF], 16)) return 1;
+    BM2_CUDA_OK(cudaMemcpyAsync(ctx->ksw_d[KB_SEQ].p, seqs, (size_t) n_seq_bytes, cudaMemcpyHostToDevice, st));
+    BM2_CUDA_OK(cudaMemcpyAsync(ctx->ksw_d[KB_REQ].p, reqs, (size_t) n * sizeof(bm2_ksw_req), cudaMemcpyHostToDevice, st));
+    BM2_CUDA_OK(cudaMemcpyAsync(ctx->ksw_d[KB_LISTOFF].p, list_off.data(), (size_t) (n + 1) * 8, cudaMemcpyHostToDevice, st));
+    BM2_CUDA_OK(cudaMemsetAsync(ctx->ksw_d[KB_OVF].p, 0, 4, st));
     KswMat mat; memcpy(mat.m, o.mat, 25);
     const int64_t blocks_need = (n + 3) / 4, blocks_max = (int64_t) ctx->n_sm * 8;
     const unsigned grid = (unsigned) (blocks_need < blocks_max ? blocks_need : blocks_max);
@@ -89,8 +89,8 @@ extern "C" int bm2_ksw_align2(bm2_ctx *ctx, const uint8_t *seqs, int64_t n_seq_b
 #undef BM2_KSW_LAUNCH
     BM2_CUDA_OK(cudaGetLastError());
     int ovf = 0;
-    BM2_CUDA_OK(cudaMemcpyAsync(out, ctx->d[KB_RES].p, (size_t) n * sizeof(bm2_ksw_res), cudaMemcpyDeviceToHost, st));
-    BM2_CUDA_OK(cudaMemcpyAsync(&ovf, ctx->d[KB_OVF].p, 4, cudaMemcpyDeviceToHost, st));
+    BM2_CUDA_OK(cudaMemcpyAsync(out, ctx->ksw_d[KB_RES].p, (size_t) n * sizeof(bm2_ksw_res), cudaMemcpyDeviceToHost, st));
+    BM2_CUDA_OK(cudaMemcpyAsync(&ovf, ctx->ksw_d[KB_OVF].p, 4, cudaMemcpyDeviceToHost, st));
     BM2_CUDA_OK(cudaStreamSynchronize(st));
     if (ovf) { bm2_set_error(ctx, "bm2_ksw_align2: score-2 list overflow (internal)"); return 1; }
     return 0;

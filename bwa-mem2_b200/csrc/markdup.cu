@@ -110,7 +110,7 @@ __global__ void dup_mark_kernel(const bm2_dup_entry *__restrict__ s, const int32
 }
 
 enum { DD_IN, DD_STARTS, DD_TFIRST, DD_TID, DD_PAIR, DD_FRAG, DD_OUT, DD_CNT, DD_TEMP, DD_KEYS0, DD_KEYS1, DD_ORD0, DD_ORD1, DD_SORTED, DD_END };
-static_assert(DD_END <= (int) (sizeof(((bm2_ctx *) nullptr)->dup_d) / sizeof(DevBuf)), "markdup buffers");
+static_assert(DD_END == std::extent<decltype(bm2_ctx::dup_d)>::value, "bm2_ctx::dup_d: one buffer per slot");
 // bm2_dup_resolve reuses the signature slots: entries in DD_PAIR, group numbers / flags / ids in DD_IN / DD_STARTS / DD_TFIRST / DD_TID / DD_FRAG
 
 int bits_of(uint64_t v) { int b = 0; while (b < 64 && (v >> b)) ++b; return b; }

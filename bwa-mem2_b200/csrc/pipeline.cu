@@ -833,12 +833,13 @@ __global__ void widen_kernel(const int32_t *in, int n, int64_t *out) {
 // ------------------------------------------------------------------------------------------------
 namespace {
 enum Buf {
-    B_CODES, B_OFFS, B_CNT, B_PREV, B_RESEED, B_SMEM_RAW, B_KEYS_IN, B_KEYS_OUT, B_VALS_IN, B_VALS_OUT, B_CUB, B_SMEM, B_SLOT_CNT,
+    B_CODES, B_OFFS, B_CNT, B_PREV, B_SMEM_RAW, B_KEYS_IN, B_KEYS_OUT, B_VALS_IN, B_VALS_OUT, B_CUB, B_SMEM, B_SLOT_CNT,
     B_SLOT_OFF, B_READ_SMEM_OFF, B_SA, B_WSEED, B_WCHAIN, B_ORD, B_SRT, B_KV, B_FIN_CHAIN, B_FIN_SEED, B_PER_READ, B_SCAN, B_CHAINS,
     B_SEEDS, B_REGS, B_REG_AUX, B_JOBS, B_NW, B_OUT, B_PERM, B_ORDPOS, B_FLT, B_MINHSP, B_OWNER, B_POOL, B_TASKS, B_RTASKS, B_COUNT_
 };
-static_assert(B_COUNT_ <= 64, "bm2_ctx::d[] too small");
-enum HBuf { H_OUT_REGS, H_OUT_OFF, H_SMEM, H_CHAINS, H_SEEDS, H_MISC };
+enum HBuf { H_OUT_REGS, H_OUT_OFF, H_SMEM, H_CHAINS, H_SEEDS, H_COUNT_ };
+static_assert(B_COUNT_ == std::extent<decltype(bm2_ctx::pipe_d)>::value, "bm2_ctx::pipe_d: one buffer per slot");
+static_assert(H_COUNT_ == std::extent<decltype(bm2_ctx::pipe_h)>::value, "bm2_ctx::pipe_h: one buffer per slot");
 
 struct Stages {
     bm2_ctx *ctx; std::vector<cudaEvent_t> &ev; std::vector<const char *> &names;
@@ -853,7 +854,7 @@ struct Stages {
     }
 };
 
-template <class T> T *P(bm2_ctx *ctx, int b) { return (T *) ctx->d[b].p; }
+template <class T> T *P(bm2_ctx *ctx, int b) { return (T *) ctx->pipe_d[b].p; }
 
 }  // namespace
 
@@ -893,8 +894,8 @@ int scan64(bm2_ctx *ctx, const int64_t *in, int64_t *out, int64_t n) {
     bm2_ctx *ctx_for_error = ctx;
     size_t bytes = 0;
     cub::DeviceScan::ExclusiveSum(nullptr, bytes, in, out, (int) (n + 1));
-    if (ctx->ensure(ctx->d[B_CUB], bytes)) return 1;
-    BM2_CUDA_OK(cub::DeviceScan::ExclusiveSum(ctx->d[B_CUB].p, bytes, in, out, (int) (n + 1), ctx->stream));
+    if (ctx->ensure(ctx->pipe_d[B_CUB], bytes)) return 1;
+    BM2_CUDA_OK(cub::DeviceScan::ExclusiveSum(ctx->pipe_d[B_CUB].p, bytes, in, out, (int) (n + 1), ctx->stream));
     return 0;
 }
 
@@ -912,8 +913,8 @@ int sort_work(bm2_ctx *ctx, uint32_t *keys_in, uint32_t *keys_out, int32_t *vals
     }
     size_t bytes = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, bytes, keys_in, keys_out, vals_in, vals_out, n);
-    if (ctx->ensure(ctx->d[B_CUB], bytes)) return 1;
-    BM2_CUDA_OK(cub::DeviceRadixSort::SortPairs(ctx->d[B_CUB].p, bytes, keys_in, keys_out, vals_in, vals_out, n, 0, 32, ctx->stream));
+    if (ctx->ensure(ctx->pipe_d[B_CUB], bytes)) return 1;
+    BM2_CUDA_OK(cub::DeviceRadixSort::SortPairs(ctx->pipe_d[B_CUB].p, bytes, keys_in, keys_out, vals_in, vals_out, n, 0, 32, ctx->stream));
     return 0;
 }
 
@@ -971,23 +972,23 @@ int run_pipeline(bm2_ctx *ctx, const bm2_read_batch *rb, UpTo upto, BatchState &
     Stages sg = { ctx, ctx->events, ctx->stage_names };
     if (sg.mark("h2d")) return 1;
 
-    if (ctx->ensure(ctx->d[B_CNT], sizeof(Counters))) return 1;
+    if (ctx->ensure(ctx->pipe_d[B_CNT], sizeof(Counters))) return 1;
     const uint8_t *d_codes = ext_codes; const int64_t *d_offs = ext_offs;
     if (!ext_codes) {
-        if (ctx->ensure(ctx->d[B_CODES], (size_t) total + 16)) return 1;
-        BM2_CUDA_OK(cudaMemcpyAsync(ctx->d[B_CODES].p, rb->codes, (size_t) total, cudaMemcpyHostToDevice, st));
+        if (ctx->ensure(ctx->pipe_d[B_CODES], (size_t) total + 16)) return 1;
+        BM2_CUDA_OK(cudaMemcpyAsync(ctx->pipe_d[B_CODES].p, rb->codes, (size_t) total, cudaMemcpyHostToDevice, st));
         d_codes = P<uint8_t>(ctx, B_CODES);
     }
     if (!ext_offs) {     // (a sub-batch of a device-resident batch brings its codes pointer but re-based offsets from the host)
-        if (ctx->ensure(ctx->d[B_OFFS], (size_t) (n + 1) * 8)) return 1;
-        BM2_CUDA_OK(cudaMemcpyAsync(ctx->d[B_OFFS].p, rb->offsets, (size_t) (n + 1) * 8, cudaMemcpyHostToDevice, st));
+        if (ctx->ensure(ctx->pipe_d[B_OFFS], (size_t) (n + 1) * 8)) return 1;
+        BM2_CUDA_OK(cudaMemcpyAsync(ctx->pipe_d[B_OFFS].p, rb->offsets, (size_t) (n + 1) * 8, cudaMemcpyHostToDevice, st));
         d_offs = P<int64_t>(ctx, B_OFFS);
     }
     if (any_flt) {
-        if (ctx->ensure(ctx->d[B_MINHSP], (size_t) n * 4)) return 1;
-        BM2_CUDA_OK(cudaMemcpyAsync(ctx->d[B_MINHSP].p, min_hsp_host.data(), (size_t) n * 4, cudaMemcpyHostToDevice, st));
+        if (ctx->ensure(ctx->pipe_d[B_MINHSP], (size_t) n * 4)) return 1;
+        BM2_CUDA_OK(cudaMemcpyAsync(ctx->pipe_d[B_MINHSP].p, min_hsp_host.data(), (size_t) n * 4, cudaMemcpyHostToDevice, st));
     }
-    BM2_CUDA_OK(cudaMemsetAsync(ctx->d[B_CNT].p, 0, sizeof(Counters), st));
+    BM2_CUDA_OK(cudaMemsetAsync(ctx->pipe_d[B_CNT].p, 0, sizeof(Counters), st));
     Counters *d_cnt = P<Counters>(ctx, B_CNT);
     Counters h_cnt;
 
@@ -1009,7 +1010,7 @@ int run_pipeline(bm2_ctx *ctx, const bm2_read_batch *rb, UpTo upto, BatchState &
     }
     if (blocks_a > max_blocks_a) blocks_a = max_blocks_a;
     const size_t thr_a = (size_t) blocks_a * 128;
-    if (ctx->ensure(ctx->d[B_PREV], thr_a * stripe * sizeof(FmPrev))) return 1;
+    if (ctx->ensure(ctx->pipe_d[B_PREV], thr_a * stripe * sizeof(FmPrev))) return 1;
     // capacities grow from the counters when a batch overflows them (then the stage is re-run)
     const double rl = (double) total / n;                                  // mean read length
     unsigned long long cap = (unsigned long long) n * 16 + 4096;
@@ -1024,8 +1025,8 @@ int run_pipeline(bm2_ctx *ctx, const bm2_read_batch *rb, UpTo upto, BatchState &
     // a stage leaves the other lanes' host threads waiting at the token instead of queueing work.
     StageToken tok_smem((use_tokens & 1) ? &ctx->parent->tok_smem : nullptr);
     for (int attempt = 0; attempt < 3; ++attempt) {
-        if (ctx->ensure(ctx->d[B_SMEM_RAW], cap * sizeof(bm2_smem)) || ctx->ensure(ctx->d[B_POOL], pool_cap * sizeof(FmPrev)) ||
-            ctx->ensure(ctx->d[B_TASKS], task_cap * sizeof(SearchTask)) || ctx->ensure(ctx->d[B_RTASKS], rtask_cap * sizeof(ReseedTask))) return 1;
+        if (ctx->ensure(ctx->pipe_d[B_SMEM_RAW], cap * sizeof(bm2_smem)) || ctx->ensure(ctx->pipe_d[B_POOL], pool_cap * sizeof(FmPrev)) ||
+            ctx->ensure(ctx->pipe_d[B_TASKS], task_cap * sizeof(SearchTask)) || ctx->ensure(ctx->pipe_d[B_RTASKS], rtask_cap * sizeof(ReseedTask))) return 1;
         BM2_CUDA_OK(cudaMemsetAsync(d_cnt, 0, sizeof(Counters), st));
         bm2_smem *d_raw = P<bm2_smem>(ctx, B_SMEM_RAW); FmPrev *d_pool = P<FmPrev>(ctx, B_POOL);
         SearchTask *d_tasks = P<SearchTask>(ctx, B_TASKS); ReseedTask *d_rt = P<ReseedTask>(ctx, B_RTASKS);
@@ -1066,18 +1067,18 @@ int run_pipeline(bm2_ctx *ctx, const bm2_read_batch *rb, UpTo upto, BatchState &
     // ---- B. order SMEMs -----------------------------------------------------------------------------------
     if (sg.mark("sort")) return 1;
     const int64_t ns1 = n_smem > 0 ? n_smem : 1;
-    if (ctx->ensure(ctx->d[B_KEYS_IN], ns1 * 8) || ctx->ensure(ctx->d[B_KEYS_OUT], ns1 * 8) || ctx->ensure(ctx->d[B_VALS_IN], ns1 * 4) ||
-        ctx->ensure(ctx->d[B_VALS_OUT], ns1 * 4) || ctx->ensure(ctx->d[B_SMEM], (ns1 + 1) * sizeof(bm2_smem)) ||
-        ctx->ensure(ctx->d[B_SLOT_CNT], (ns1 + 1) * 8) || ctx->ensure(ctx->d[B_SLOT_OFF], (ns1 + 2) * 8) ||
-        ctx->ensure(ctx->d[B_READ_SMEM_OFF], (size_t) (n + 2) * 8)) return 1;
+    if (ctx->ensure(ctx->pipe_d[B_KEYS_IN], ns1 * 8) || ctx->ensure(ctx->pipe_d[B_KEYS_OUT], ns1 * 8) || ctx->ensure(ctx->pipe_d[B_VALS_IN], ns1 * 4) ||
+        ctx->ensure(ctx->pipe_d[B_VALS_OUT], ns1 * 4) || ctx->ensure(ctx->pipe_d[B_SMEM], (ns1 + 1) * sizeof(bm2_smem)) ||
+        ctx->ensure(ctx->pipe_d[B_SLOT_CNT], (ns1 + 1) * 8) || ctx->ensure(ctx->pipe_d[B_SLOT_OFF], (ns1 + 2) * 8) ||
+        ctx->ensure(ctx->pipe_d[B_READ_SMEM_OFF], (size_t) (n + 2) * 8)) return 1;
     if (n_smem > 0) {
         const int gb = (int) ((n_smem + 255) / 256);
         smem_keys_kernel<<<gb, 256, 0, st>>>(P<bm2_smem>(ctx, B_SMEM_RAW), n_smem, P<uint64_t>(ctx, B_KEYS_IN), P<uint32_t>(ctx, B_VALS_IN));
         size_t cub_bytes = 0;
         cub::DeviceRadixSort::SortPairs(nullptr, cub_bytes, P<uint64_t>(ctx, B_KEYS_IN), P<uint64_t>(ctx, B_KEYS_OUT), P<uint32_t>(ctx, B_VALS_IN),
                                         P<uint32_t>(ctx, B_VALS_OUT), (int) n_smem);
-        if (ctx->ensure(ctx->d[B_CUB], cub_bytes)) return 1;
-        BM2_CUDA_OK(cub::DeviceRadixSort::SortPairs(ctx->d[B_CUB].p, cub_bytes, P<uint64_t>(ctx, B_KEYS_IN), P<uint64_t>(ctx, B_KEYS_OUT),
+        if (ctx->ensure(ctx->pipe_d[B_CUB], cub_bytes)) return 1;
+        BM2_CUDA_OK(cub::DeviceRadixSort::SortPairs(ctx->pipe_d[B_CUB].p, cub_bytes, P<uint64_t>(ctx, B_KEYS_IN), P<uint64_t>(ctx, B_KEYS_OUT),
                                                     P<uint32_t>(ctx, B_VALS_IN), P<uint32_t>(ctx, B_VALS_OUT), (int) n_smem, 0, 64, st));
         BM2_CUDA_OK(cudaMemsetAsync(P<int64_t>(ctx, B_SLOT_CNT) + n_smem, 0, 8, st));
         smem_gather_kernel<<<gb, 256, 0, st>>>(P<bm2_smem>(ctx, B_SMEM_RAW), P<uint32_t>(ctx, B_VALS_OUT), n_smem, ctx->opt.max_occ,
@@ -1097,37 +1098,37 @@ int run_pipeline(bm2_ctx *ctx, const bm2_read_batch *rb, UpTo upto, BatchState &
     // ---- C. SA lookup -------------------------------------------------------------------------------------
     if (sg.mark("sal")) return 1;
     const size_t sl1 = (size_t) (n_slots > 0 ? n_slots : 1) + 1;
-    if (ctx->ensure(ctx->d[B_SA], sl1 * 8)) return 1;
+    if (ctx->ensure(ctx->pipe_d[B_SA], sl1 * 8)) return 1;
     if (n_slots > 0) {
-        if (ctx->ensure(ctx->d[B_OWNER], sl1 * 4 * 2)) return 1;
+        if (ctx->ensure(ctx->pipe_d[B_OWNER], sl1 * 4 * 2)) return 1;
         int32_t *own_in = P<int32_t>(ctx, B_OWNER), *own = own_in + sl1;
         BM2_CUDA_OK(cudaMemsetAsync(own_in, 0, sl1 * 4, st));
         slot_head_kernel<<<(unsigned) ((n_smem + 255) / 256), 256, 0, st>>>(P<int64_t>(ctx, B_SLOT_OFF), n_smem, own_in);
         size_t sbytes = 0;
         cub::DeviceScan::InclusiveScan(nullptr, sbytes, own_in, own, cub::Max(), (int) n_slots);
-        if (ctx->ensure(ctx->d[B_CUB], sbytes)) return 1;
-        BM2_CUDA_OK(cub::DeviceScan::InclusiveScan(ctx->d[B_CUB].p, sbytes, own_in, own, cub::Max(), (int) n_slots, st));
+        if (ctx->ensure(ctx->pipe_d[B_CUB], sbytes)) return 1;
+        BM2_CUDA_OK(cub::DeviceScan::InclusiveScan(ctx->pipe_d[B_CUB].p, sbytes, own_in, own, cub::Max(), (int) n_slots, st));
         sa_kernel<<<(unsigned) ((n_slots + 255) / 256), 256, 0, st>>>(pv.fm, P<bm2_smem>(ctx, B_SMEM), P<int64_t>(ctx, B_SLOT_OFF), own, n_slots,
                                                                         ctx->opt.max_occ, P<int64_t>(ctx, B_SA), d_cnt);
     }
 
     // ---- D. chaining --------------------------------------------------------------------------------------
     if (sg.mark("chain")) return 1;
-    if (ctx->ensure(ctx->d[B_WSEED], sl1 * sizeof(WSeed)) || ctx->ensure(ctx->d[B_WCHAIN], sl1 * sizeof(WChain)) ||
-        ctx->ensure(ctx->d[B_ORD], sl1 * 4) || ctx->ensure(ctx->d[B_SRT], sl1 * 4) || ctx->ensure(ctx->d[B_KV], sl1 * 4) ||
-        ctx->ensure(ctx->d[B_ORDPOS], sl1 * 8) || ctx->ensure(ctx->d[B_FLT], sl1 * sizeof(FltRec)) ||
-        ctx->ensure(ctx->d[B_FIN_CHAIN], sl1 * sizeof(bm2_chain)) || ctx->ensure(ctx->d[B_FIN_SEED], sl1 * sizeof(bm2_seed)) ||
-        ctx->ensure(ctx->d[B_PER_READ], al((size_t) (n + 1) * 4) * 5) || ctx->ensure(ctx->d[B_SCAN], al((size_t) (n + 2) * 8) * 10)) return 1;
+    if (ctx->ensure(ctx->pipe_d[B_WSEED], sl1 * sizeof(WSeed)) || ctx->ensure(ctx->pipe_d[B_WCHAIN], sl1 * sizeof(WChain)) ||
+        ctx->ensure(ctx->pipe_d[B_ORD], sl1 * 4) || ctx->ensure(ctx->pipe_d[B_SRT], sl1 * 4) || ctx->ensure(ctx->pipe_d[B_KV], sl1 * 4) ||
+        ctx->ensure(ctx->pipe_d[B_ORDPOS], sl1 * 8) || ctx->ensure(ctx->pipe_d[B_FLT], sl1 * sizeof(FltRec)) ||
+        ctx->ensure(ctx->pipe_d[B_FIN_CHAIN], sl1 * sizeof(bm2_chain)) || ctx->ensure(ctx->pipe_d[B_FIN_SEED], sl1 * sizeof(bm2_seed)) ||
+        ctx->ensure(ctx->pipe_d[B_PER_READ], al((size_t) (n + 1) * 4) * 5) || ctx->ensure(ctx->pipe_d[B_SCAN], al((size_t) (n + 2) * 8) * 10)) return 1;
     const size_t pr = al((size_t) (n + 1) * 4);
-    char *prb = (char *) ctx->d[B_PER_READ].p;
+    char *prb = (char *) ctx->pipe_d[B_PER_READ].p;
     int32_t *d_nchain = (int32_t *) prb, *d_nseed = (int32_t *) (prb + pr), *d_nleft = (int32_t *) (prb + 2 * pr),
             *d_nright = (int32_t *) (prb + 3 * pr), *d_nfinal = (int32_t *) (prb + 4 * pr);
     ChainBufs cb = { P<WSeed>(ctx, B_WSEED), P<WChain>(ctx, B_WCHAIN), P<int32_t>(ctx, B_ORD), P<int32_t>(ctx, B_SRT), P<int32_t>(ctx, B_KV),
                      P<int64_t>(ctx, B_ORDPOS), P<FltRec>(ctx, B_FLT),
                      P<bm2_chain>(ctx, B_FIN_CHAIN), P<bm2_seed>(ctx, B_FIN_SEED), d_nchain, d_nseed, d_nleft, d_nright };
-    if (ctx->ensure(ctx->d[B_PERM], al((size_t) n * 4) * 4)) return 1;
-    uint32_t *wk_in = (uint32_t *) ctx->d[B_PERM].p, *wk_out = (uint32_t *) ((char *) ctx->d[B_PERM].p + al((size_t) n * 4));
-    int32_t *wv_in = (int32_t *) ((char *) ctx->d[B_PERM].p + 2 * al((size_t) n * 4)), *d_perm = (int32_t *) ((char *) ctx->d[B_PERM].p + 3 * al((size_t) n * 4));
+    if (ctx->ensure(ctx->pipe_d[B_PERM], al((size_t) n * 4) * 4)) return 1;
+    uint32_t *wk_in = (uint32_t *) ctx->pipe_d[B_PERM].p, *wk_out = (uint32_t *) ((char *) ctx->pipe_d[B_PERM].p + al((size_t) n * 4));
+    int32_t *wv_in = (int32_t *) ((char *) ctx->pipe_d[B_PERM].p + 2 * al((size_t) n * 4)), *d_perm = (int32_t *) ((char *) ctx->pipe_d[B_PERM].p + 3 * al((size_t) n * 4));
     work_keys_slots_kernel<<<(n + 255) / 256, 256, 0, st>>>(P<int64_t>(ctx, B_READ_SMEM_OFF), P<int64_t>(ctx, B_SLOT_OFF), n, wk_in, wv_in);
     if (sort_work(ctx, wk_in, wk_out, wv_in, d_perm, n, true)) return 1;             // decreasing number of seed slots
     // light reads of the chain and tail kernels in work order instead of input order: no better in an A/B (neighbouring reads share
@@ -1148,7 +1149,7 @@ int run_pipeline(bm2_ctx *ctx, const bm2_read_batch *rb, UpTo upto, BatchState &
     // ---- E. scans + compaction ------------------------------------------------------------------------------
     if (sg.mark("compact")) return 1;
     const size_t sc = al((size_t) (n + 2) * 8);
-    char *scb = (char *) ctx->d[B_SCAN].p;
+    char *scb = (char *) ctx->pipe_d[B_SCAN].p;
     int64_t *w_tmp = (int64_t *) scb, *d_chain_off = (int64_t *) (scb + sc), *d_reg_off = (int64_t *) (scb + 2 * sc),
             *d_left_off = (int64_t *) (scb + 3 * sc), *d_right_off = (int64_t *) (scb + 4 * sc), *d_out_off = (int64_t *) (scb + 5 * sc);
     const int gw = (n + 1 + 255) / 256;
@@ -1167,7 +1168,7 @@ int run_pipeline(bm2_ctx *ctx, const bm2_read_batch *rb, UpTo upto, BatchState &
     const int64_t n_chains = tot[0], n_regs = tot[1], n_left = tot[2], n_right = tot[3];
     bs.n_chains = n_chains; bs.n_regs = n_regs; bs.n_left = n_left; bs.n_right = n_right;
     if (n_regs > 2000000000LL) { bm2_set_error(ctx, "too many seeds in one batch"); return 1; }
-    if (ctx->ensure(ctx->d[B_CHAINS], (size_t) (n_chains + 1) * sizeof(bm2_chain)) || ctx->ensure(ctx->d[B_SEEDS], (size_t) (n_regs + 1) * sizeof(bm2_seed))) return 1;
+    if (ctx->ensure(ctx->pipe_d[B_CHAINS], (size_t) (n_chains + 1) * sizeof(bm2_chain)) || ctx->ensure(ctx->pipe_d[B_SEEDS], (size_t) (n_regs + 1) * sizeof(bm2_seed))) return 1;
     chain_compact_kernel<<<(n + 127) / 128, 128, 0, st>>>(P<int64_t>(ctx, B_READ_SMEM_OFF), P<int64_t>(ctx, B_SLOT_OFF), n, P<bm2_chain>(ctx, B_FIN_CHAIN),
                                                           P<bm2_seed>(ctx, B_FIN_SEED), d_chain_off, d_reg_off, P<bm2_chain>(ctx, B_CHAINS), P<bm2_seed>(ctx, B_SEEDS));
     if (upto == UPTO_CHAIN) { if (sg.mark("end")) return 1; BM2_CUDA_OK(cudaStreamSynchronize(st)); return 0; }
@@ -1184,11 +1185,11 @@ int run_pipeline(bm2_ctx *ctx, const bm2_read_batch *rb, UpTo upto, BatchState &
     const size_t aux_bytes = al(nr1 * 4) * 3 + al(nr1 * 8) + al(nl1 * 4) * 2 + al(nrt1 * 4) * 2 + al(nr1 * sizeof(PfBox)) +
                              (lazy ? al(nr1) + al((size_t) n * sizeof(PfCursor)) + al(nl1 * 4) + al(nrt1 * 4) : 0);
     const size_t njmax = nl1 > nrt1 ? nl1 : nrt1;
-    if (ctx->ensure(ctx->d[B_REGS], nr1 * sizeof(bm2_alnreg_t)) || ctx->ensure(ctx->d[B_REG_AUX], aux_bytes) ||
-        ctx->ensure(ctx->d[B_JOBS], al(nl1 * sizeof(ExtJobRec)) + al(nrt1 * sizeof(ExtJobRec)) + al(njmax * sizeof(ExtJobRec)) + al(njmax * sizeof(BswOut)) +
+    if (ctx->ensure(ctx->pipe_d[B_REGS], nr1 * sizeof(bm2_alnreg_t)) || ctx->ensure(ctx->pipe_d[B_REG_AUX], aux_bytes) ||
+        ctx->ensure(ctx->pipe_d[B_JOBS], al(nl1 * sizeof(ExtJobRec)) + al(nrt1 * sizeof(ExtJobRec)) + al(njmax * sizeof(ExtJobRec)) + al(njmax * sizeof(BswOut)) +
                                     (lazy ? al(nl1 * sizeof(ExtJobRec)) + al(nrt1 * sizeof(ExtJobRec)) : 0)) ||
         ctx->ensure(ctx->bsw_scratch, bsw_scratch_bytes((int) njmax))) return 1;
-    char *ab = (char *) ctx->d[B_REG_AUX].p;
+    char *ab = (char *) ctx->pipe_d[B_REG_AUX].p;
     int32_t *d_reg_chain = (int32_t *) ab; ab += al(nr1 * 4);
     int32_t *d_reg_seed = (int32_t *) ab; ab += al(nr1 * 4);
     int32_t *d_srt2 = (int32_t *) ab; ab += al(nr1 * 4);
@@ -1205,7 +1206,7 @@ int run_pipeline(bm2_ctx *ctx, const bm2_read_batch *rb, UpTo upto, BatchState &
         d_wleft_reg = (int32_t *) ab; ab += al(nl1 * 4);
         d_wright_reg = (int32_t *) ab; ab += al(nrt1 * 4);
     }
-    char *jb = (char *) ctx->d[B_JOBS].p;
+    char *jb = (char *) ctx->pipe_d[B_JOBS].p;
     ExtJobRec *d_left = (ExtJobRec *) jb; jb += al(nl1 * sizeof(ExtJobRec));
     ExtJobRec *d_right = (ExtJobRec *) jb; jb += al(nrt1 * sizeof(ExtJobRec));
     ExtJobRec *d_retry_jobs = (ExtJobRec *) jb; jb += al(njmax * sizeof(ExtJobRec));
@@ -1290,7 +1291,7 @@ int run_pipeline(bm2_ctx *ctx, const bm2_read_batch *rb, UpTo upto, BatchState &
     // ---- I. post-filter + tail ----------------------------------------------------------------------------
     if (sg.mark("tail")) return 1;
     const int he_stride = 2 * (max_len + 2);
-    if (ctx->ensure(ctx->d[B_NW], (size_t) blocks_i * 128 * he_stride * 4)) return 1;
+    if (ctx->ensure(ctx->pipe_d[B_NW], (size_t) blocks_i * 128 * he_stride * 4)) return 1;
     if (getenv("BM2_DEBUG_NREG")) {     // the heaviest reads of the batch (their tail is the critical path of the warp-per-read kernel): stderr
         std::vector<int64_t> ho((size_t) n + 1);
         BM2_CUDA_OK(cudaMemcpyAsync(ho.data(), d_reg_off, (size_t) (n + 1) * 8, cudaMemcpyDeviceToHost, st));
@@ -1312,18 +1313,18 @@ int run_pipeline(bm2_ctx *ctx, const bm2_read_batch *rb, UpTo upto, BatchState &
     // ---- J. output ---------------------------------------------------------------------------------------
     if (sg.mark("output")) return 1;
     widen_kernel<<<gw, 256, 0, st>>>(d_nfinal, n, w_tmp); if (scan64(ctx, w_tmp, d_out_off, n)) return 1;
-    if (ctx->ensure(ctx->d[B_OUT], nr1 * sizeof(bm2_alnreg_t))) return 1;
+    if (ctx->ensure(ctx->pipe_d[B_OUT], nr1 * sizeof(bm2_alnreg_t))) return 1;
     regs_gather_kernel<<<(n + 127) / 128, 128, 0, st>>>(d_regs, d_reg_off, d_out_off, n, P<bm2_alnreg_t>(ctx, B_OUT));
-    if (ctx->ensure_host(ctx->h[H_OUT_OFF], (size_t) (n + 1) * 8)) return 1;
-    BM2_CUDA_OK(cudaMemcpyAsync(ctx->h[H_OUT_OFF].p, d_out_off, (size_t) (n + 1) * 8, cudaMemcpyDeviceToHost, st));
+    if (ctx->ensure_host(ctx->pipe_h[H_OUT_OFF], (size_t) (n + 1) * 8)) return 1;
+    BM2_CUDA_OK(cudaMemcpyAsync(ctx->pipe_h[H_OUT_OFF].p, d_out_off, (size_t) (n + 1) * 8, cudaMemcpyDeviceToHost, st));
     BM2_CUDA_OK(cudaMemcpyAsync(&h_cnt, d_cnt, sizeof(Counters), cudaMemcpyDeviceToHost, st));
     BM2_CUDA_OK(cudaStreamSynchronize(st));
     ctx->last_cells = h_cnt.cells;
     ctx->last_walk_done = h_cnt.n_walk_done;
-    const int64_t n_out = ((const int64_t *) ctx->h[H_OUT_OFF].p)[n];
+    const int64_t n_out = ((const int64_t *) ctx->pipe_h[H_OUT_OFF].p)[n];
     bs.n_out = n_out;
-    if (copy_out && ctx->ensure_host(ctx->h[H_OUT_REGS], (size_t) (n_out + 1) * sizeof(bm2_alnreg_t))) return 1;
-    if (n_out && copy_out) BM2_CUDA_OK(cudaMemcpyAsync(ctx->h[H_OUT_REGS].p, ctx->d[B_OUT].p, (size_t) n_out * sizeof(bm2_alnreg_t), cudaMemcpyDeviceToHost, st));
+    if (copy_out && ctx->ensure_host(ctx->pipe_h[H_OUT_REGS], (size_t) (n_out + 1) * sizeof(bm2_alnreg_t))) return 1;
+    if (n_out && copy_out) BM2_CUDA_OK(cudaMemcpyAsync(ctx->pipe_h[H_OUT_REGS].p, ctx->pipe_d[B_OUT].p, (size_t) n_out * sizeof(bm2_alnreg_t), cudaMemcpyDeviceToHost, st));
     if (sg.mark("end")) return 1;
     BM2_CUDA_OK(cudaStreamSynchronize(st));
     BM2_CUDA_OK(cudaGetLastError());
@@ -1360,11 +1361,11 @@ extern "C" int bm2_collect_smems(bm2_ctx *ctx, const bm2_read_batch *reads, bm2_
     BatchState bs;
     if (run_pipeline(ctx, reads, UPTO_SMEM, bs)) return 1;
     finish_stage_times(ctx);
-    if (ctx->ensure_host(ctx->h[H_SMEM], (size_t) (bs.n_smem + 1) * sizeof(bm2_smem)) || ctx->ensure_host(ctx->h[H_OUT_OFF], (size_t) (bs.n + 2) * 8)) return 1;
-    if (bs.n_smem) BM2_CUDA_OK(cudaMemcpy(ctx->h[H_SMEM].p, ctx->d[B_SMEM].p, (size_t) bs.n_smem * sizeof(bm2_smem), cudaMemcpyDeviceToHost));
-    if (bs.n > 0) BM2_CUDA_OK(cudaMemcpy(ctx->h[H_OUT_OFF].p, ctx->d[B_READ_SMEM_OFF].p, (size_t) (bs.n + 1) * 8, cudaMemcpyDeviceToHost));
-    else ((int64_t *) ctx->h[H_OUT_OFF].p)[0] = 0;
-    out->n = bs.n_smem; out->smems = (const bm2_smem *) ctx->h[H_SMEM].p; out->read_off = (const int64_t *) ctx->h[H_OUT_OFF].p;
+    if (ctx->ensure_host(ctx->pipe_h[H_SMEM], (size_t) (bs.n_smem + 1) * sizeof(bm2_smem)) || ctx->ensure_host(ctx->pipe_h[H_OUT_OFF], (size_t) (bs.n + 2) * 8)) return 1;
+    if (bs.n_smem) BM2_CUDA_OK(cudaMemcpy(ctx->pipe_h[H_SMEM].p, ctx->pipe_d[B_SMEM].p, (size_t) bs.n_smem * sizeof(bm2_smem), cudaMemcpyDeviceToHost));
+    if (bs.n > 0) BM2_CUDA_OK(cudaMemcpy(ctx->pipe_h[H_OUT_OFF].p, ctx->pipe_d[B_READ_SMEM_OFF].p, (size_t) (bs.n + 1) * 8, cudaMemcpyDeviceToHost));
+    else ((int64_t *) ctx->pipe_h[H_OUT_OFF].p)[0] = 0;
+    out->n = bs.n_smem; out->smems = (const bm2_smem *) ctx->pipe_h[H_SMEM].p; out->read_off = (const int64_t *) ctx->pipe_h[H_OUT_OFF].p;
     return 0;
 }
 
@@ -1374,16 +1375,16 @@ extern "C" int bm2_seed_chain(bm2_ctx *ctx, const bm2_read_batch *reads, bm2_cha
     BatchState bs;
     if (run_pipeline(ctx, reads, UPTO_CHAIN, bs)) return 1;
     finish_stage_times(ctx);
-    if (ctx->ensure_host(ctx->h[H_CHAINS], (size_t) (bs.n_chains + 1) * sizeof(bm2_chain)) ||
-        ctx->ensure_host(ctx->h[H_SEEDS], (size_t) (bs.n_regs + 1) * sizeof(bm2_seed)) || ctx->ensure_host(ctx->h[H_OUT_OFF], (size_t) (bs.n + 2) * 8)) return 1;
-    if (bs.n_chains) BM2_CUDA_OK(cudaMemcpy(ctx->h[H_CHAINS].p, ctx->d[B_CHAINS].p, (size_t) bs.n_chains * sizeof(bm2_chain), cudaMemcpyDeviceToHost));
-    if (bs.n_regs) BM2_CUDA_OK(cudaMemcpy(ctx->h[H_SEEDS].p, ctx->d[B_SEEDS].p, (size_t) bs.n_regs * sizeof(bm2_seed), cudaMemcpyDeviceToHost));
+    if (ctx->ensure_host(ctx->pipe_h[H_CHAINS], (size_t) (bs.n_chains + 1) * sizeof(bm2_chain)) ||
+        ctx->ensure_host(ctx->pipe_h[H_SEEDS], (size_t) (bs.n_regs + 1) * sizeof(bm2_seed)) || ctx->ensure_host(ctx->pipe_h[H_OUT_OFF], (size_t) (bs.n + 2) * 8)) return 1;
+    if (bs.n_chains) BM2_CUDA_OK(cudaMemcpy(ctx->pipe_h[H_CHAINS].p, ctx->pipe_d[B_CHAINS].p, (size_t) bs.n_chains * sizeof(bm2_chain), cudaMemcpyDeviceToHost));
+    if (bs.n_regs) BM2_CUDA_OK(cudaMemcpy(ctx->pipe_h[H_SEEDS].p, ctx->pipe_d[B_SEEDS].p, (size_t) bs.n_regs * sizeof(bm2_seed), cudaMemcpyDeviceToHost));
     if (bs.n > 0) {
         const size_t sc = al((size_t) (bs.n + 2) * 8);
-        BM2_CUDA_OK(cudaMemcpy(ctx->h[H_OUT_OFF].p, (char *) ctx->d[B_SCAN].p + sc, (size_t) (bs.n + 1) * 8, cudaMemcpyDeviceToHost));
-    } else ((int64_t *) ctx->h[H_OUT_OFF].p)[0] = 0;
-    out->n_chains = bs.n_chains; out->n_seeds = bs.n_regs; out->chains = (const bm2_chain *) ctx->h[H_CHAINS].p;
-    out->seeds = (const bm2_seed *) ctx->h[H_SEEDS].p; out->read_off = (const int64_t *) ctx->h[H_OUT_OFF].p;
+        BM2_CUDA_OK(cudaMemcpy(ctx->pipe_h[H_OUT_OFF].p, (char *) ctx->pipe_d[B_SCAN].p + sc, (size_t) (bs.n + 1) * 8, cudaMemcpyDeviceToHost));
+    } else ((int64_t *) ctx->pipe_h[H_OUT_OFF].p)[0] = 0;
+    out->n_chains = bs.n_chains; out->n_seeds = bs.n_regs; out->chains = (const bm2_chain *) ctx->pipe_h[H_CHAINS].p;
+    out->seeds = (const bm2_seed *) ctx->pipe_h[H_SEEDS].p; out->read_off = (const int64_t *) ctx->pipe_h[H_OUT_OFF].p;
     return 0;
 }
 
@@ -1402,10 +1403,10 @@ static int run_regs(bm2_ctx *ctx, const bm2_read_batch *rb, const uint8_t *d_cod
         if (run_pipeline(ctx, rb, UPTO_REGS, bs, d_codes, d_offs, copy_out)) return 1;
         finish_stage_times(ctx);
         if (bs.n <= 0) {
-            if (ctx->ensure_host(ctx->h[H_OUT_OFF], 16) || ctx->ensure_host(ctx->h[H_OUT_REGS], sizeof(bm2_alnreg_t))) return 1;
-            ((int64_t *) ctx->h[H_OUT_OFF].p)[0] = 0;
+            if (ctx->ensure_host(ctx->pipe_h[H_OUT_OFF], 16) || ctx->ensure_host(ctx->pipe_h[H_OUT_REGS], sizeof(bm2_alnreg_t))) return 1;
+            ((int64_t *) ctx->pipe_h[H_OUT_OFF].p)[0] = 0;
         }
-        out->n = bs.n_out; out->regs = copy_out ? (const bm2_alnreg_t *) ctx->h[H_OUT_REGS].p : nullptr; out->read_off = (const int64_t *) ctx->h[H_OUT_OFF].p;
+        out->n = bs.n_out; out->regs = copy_out ? (const bm2_alnreg_t *) ctx->pipe_h[H_OUT_REGS].p : nullptr; out->read_off = (const int64_t *) ctx->pipe_h[H_OUT_OFF].p;
         return 0;
     }
     BM2_CUDA_OK(cudaSetDevice(ctx->device));
@@ -1466,16 +1467,16 @@ static int run_regs(bm2_ctx *ctx, const bm2_read_batch *rb, const uint8_t *d_cod
     // gather: per-read offsets on the host, regs device -> the context's pinned buffer, one copy per lane on its own stream
     int64_t n_out = 0;
     for (int k = 0; k < K; ++k) n_out += jobs[k].bs.n_out;
-    if (ctx->ensure_host(ctx->h[H_OUT_OFF], (size_t) (n + 1) * 8) || ctx->ensure_host(ctx->h[H_OUT_REGS], (size_t) (n_out + 1) * sizeof(bm2_alnreg_t))) return 1;
-    int64_t *off = (int64_t *) ctx->h[H_OUT_OFF].p;
-    bm2_alnreg_t *regs = (bm2_alnreg_t *) ctx->h[H_OUT_REGS].p;
+    if (ctx->ensure_host(ctx->pipe_h[H_OUT_OFF], (size_t) (n + 1) * 8) || ctx->ensure_host(ctx->pipe_h[H_OUT_REGS], (size_t) (n_out + 1) * sizeof(bm2_alnreg_t))) return 1;
+    int64_t *off = (int64_t *) ctx->pipe_h[H_OUT_OFF].p;
+    bm2_alnreg_t *regs = (bm2_alnreg_t *) ctx->pipe_h[H_OUT_REGS].p;
     int64_t pos = 0;
     for (int k = 0; k < K; ++k) {
         const Job &j = jobs[k];
         bm2_ctx *l = ctx->lanes[k];
-        const int64_t *lo = (const int64_t *) l->h[H_OUT_OFF].p;
+        const int64_t *lo = (const int64_t *) l->pipe_h[H_OUT_OFF].p;
         if (copy_out && j.bs.n_out)
-            BM2_CUDA_OK(cudaMemcpyAsync(regs + pos, l->d[B_OUT].p, (size_t) j.bs.n_out * sizeof(bm2_alnreg_t), cudaMemcpyDeviceToHost, l->stream));
+            BM2_CUDA_OK(cudaMemcpyAsync(regs + pos, l->pipe_d[B_OUT].p, (size_t) j.bs.n_out * sizeof(bm2_alnreg_t), cudaMemcpyDeviceToHost, l->stream));
         for (int i = 0; i < j.n; ++i) off[j.first + i] = lo[i] + pos;
         pos += j.bs.n_out;
     }

@@ -28,12 +28,14 @@
 #include <string>
 
 namespace {
-enum { SB_CODES = 64, SB_OFFS, SB_REGS, SB_REGOFF, SB_DESC, SB_ARENA, SB_RECS_W, SB_XA_W, SB_OPS_W, SB_MD_W, SB_CNT, SB_FINAL, SB_LOG, SB_TERM,
-       SB_RECS, SB_XA, SB_OPS, SB_MD };
-enum { SJ_PAIRJOBS = 90, SJ_JOBS, SJ_RES, SJ_LISTS, SJ_STATS, SB_ORDER };          // staged rescue (84-89 belong to ksw.cu); processing order
-static_assert(SJ_STATS < 96, "bm2_ctx::d[] too small");
-enum { SH_RECS = 16, SH_XA, SH_OPS, SH_MD, SH_CNT, SH_STAGE };
-static_assert(SB_MD < 96, "bm2_ctx::d[] too small");
+enum { SB_CODES, SB_OFFS, SB_REGS, SB_REGOFF, SB_DESC, SB_ARENA, SB_RECS_W, SB_XA_W, SB_OPS_W, SB_MD_W, SB_CNT, SB_FINAL, SB_LOG, SB_TERM,
+       SB_RECS, SB_XA, SB_OPS, SB_MD,
+       SJ_PAIRJOBS, SJ_JOBS, SJ_RES, SJ_LISTS, SJ_STATS,          // staged rescue
+       SB_ORDER,                                                  // processing order
+       SB_COUNT_ };
+enum { SH_RECS, SH_XA, SH_OPS, SH_MD, SH_CNT, SH_COUNT_ };
+static_assert(SB_COUNT_ == std::extent<decltype(bm2_ctx::sam_d)>::value, "bm2_ctx::sam_d: one buffer per slot");
+static_assert(SH_COUNT_ == std::extent<decltype(bm2_ctx::sam_h)>::value, "bm2_ctx::sam_h: one buffer per slot");
 
 struct PairDesc {                 // one pair of a wave
     SamPairCaps caps;
@@ -223,7 +225,7 @@ __global__ void sam_gather_kernel(const PairDesc *__restrict__ desc, const PairC
     for (int64_t k = 0; k < c.md; ++k) md[f.md + k] = md_w[d.md_off + k];
 }
 
-template <class T> T *P(bm2_ctx *ctx, int b) { return (T *) ctx->d[b].p; }
+template <class T> T *P(bm2_ctx *ctx, int b) { return (T *) ctx->sam_d[b].p; }
 
 // pinned host buffer that keeps its content when it grows
 int grow_host(bm2_ctx *ctx, HostBuf &b, size_t used, size_t need) {
@@ -254,9 +256,9 @@ int run_sam(bm2_ctx *ctx, const bm2_read_batch *reads, const bm2_alnreg_t *regs,
     BM2_CUDA_OK(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
     memset(out, 0, sizeof(*out));
-    if (grow_host(ctx, ctx->h[SH_RECS], 0, 64) || grow_host(ctx, ctx->h[SH_XA], 0, 64) || grow_host(ctx, ctx->h[SH_OPS], 0, 64) || grow_host(ctx, ctx->h[SH_MD], 0, 64)) return 1;
-    out->recs = (const bm2_sam_rec *) ctx->h[SH_RECS].p; out->xa = (const bm2_sam_xa *) ctx->h[SH_XA].p;
-    out->cigar = (const uint32_t *) ctx->h[SH_OPS].p; out->md = (const char *) ctx->h[SH_MD].p;
+    if (grow_host(ctx, ctx->sam_h[SH_RECS], 0, 64) || grow_host(ctx, ctx->sam_h[SH_XA], 0, 64) || grow_host(ctx, ctx->sam_h[SH_OPS], 0, 64) || grow_host(ctx, ctx->sam_h[SH_MD], 0, 64)) return 1;
+    out->recs = (const bm2_sam_rec *) ctx->sam_h[SH_RECS].p; out->xa = (const bm2_sam_xa *) ctx->sam_h[SH_XA].p;
+    out->cigar = (const uint32_t *) ctx->sam_h[SH_OPS].p; out->md = (const char *) ctx->sam_h[SH_MD].p;
     const int n_pairs_all = paired ? nr >> 1 : nr;              // units
     if (n_pairs_all == 0) return 0;
     const bm2_mem_opt_t &o = ctx->opt;
@@ -289,9 +291,9 @@ int run_sam(bm2_ctx *ctx, const bm2_read_batch *reads, const bm2_alnreg_t *regs,
             const double ns = (dist - pes4[d].avg) / pes4[d].std;                 // src/bwamem_pair.cpp:320-322
             term[term_at[d] + (size_t) (dist - tb.pair_lo[d])] = .721 * log(2. * erfc(fabs(ns) * M_SQRT1_2)) * o.a;
         }
-    if (ctx->ensure(ctx->d[SB_LOG], tab.size() * 8) || ctx->ensure(ctx->d[SB_TERM], term.size() * 8)) return 1;
-    BM2_CUDA_OK(cudaMemcpyAsync(ctx->d[SB_LOG].p, tab.data(), tab.size() * 8, cudaMemcpyHostToDevice, st));
-    BM2_CUDA_OK(cudaMemcpyAsync(ctx->d[SB_TERM].p, term.data(), term.size() * 8, cudaMemcpyHostToDevice, st));
+    if (ctx->ensure(ctx->sam_d[SB_LOG], tab.size() * 8) || ctx->ensure(ctx->sam_d[SB_TERM], term.size() * 8)) return 1;
+    BM2_CUDA_OK(cudaMemcpyAsync(ctx->sam_d[SB_LOG].p, tab.data(), tab.size() * 8, cudaMemcpyHostToDevice, st));
+    BM2_CUDA_OK(cudaMemcpyAsync(ctx->sam_d[SB_TERM].p, term.data(), term.size() * 8, cudaMemcpyHostToDevice, st));
     tb.log_tab = P<double>(ctx, SB_LOG);
     for (int d = 0; d < 4; ++d) tb.pair_term[d] = P<double>(ctx, SB_TERM) + term_at[d];
     ContigView cv; cv.l_pac = ctx->idx.l_pac; cv.n_seqs = ctx->idx.n_seqs; cv.ann_off = ctx->idx.ann_off; cv.ann_len = ctx->idx.ann_len; cv.ann_alt = ctx->idx.ann_alt;
@@ -308,12 +310,12 @@ int run_sam(bm2_ctx *ctx, const bm2_read_batch *reads, const bm2_alnreg_t *regs,
 
     // ---- inputs ------------------------------------------------------------------------------------------------------------
     const int64_t total = reads->offsets[nr], n_regs = read_off[nr];
-    if (ctx->ensure(ctx->d[SB_CODES], (size_t) total + 16) || ctx->ensure(ctx->d[SB_OFFS], (size_t) (nr + 1) * 8) ||
-        ctx->ensure(ctx->d[SB_REGS], (size_t) (n_regs + 1) * sizeof(bm2_alnreg_t)) || ctx->ensure(ctx->d[SB_REGOFF], (size_t) (nr + 1) * 8)) return 1;
-    BM2_CUDA_OK(cudaMemcpyAsync(ctx->d[SB_CODES].p, reads->codes, (size_t) total, cudaMemcpyHostToDevice, st));
-    BM2_CUDA_OK(cudaMemcpyAsync(ctx->d[SB_OFFS].p, reads->offsets, (size_t) (nr + 1) * 8, cudaMemcpyHostToDevice, st));
-    if (n_regs) BM2_CUDA_OK(cudaMemcpyAsync(ctx->d[SB_REGS].p, regs, (size_t) n_regs * sizeof(bm2_alnreg_t), cudaMemcpyHostToDevice, st));
-    BM2_CUDA_OK(cudaMemcpyAsync(ctx->d[SB_REGOFF].p, read_off, (size_t) (nr + 1) * 8, cudaMemcpyHostToDevice, st));
+    if (ctx->ensure(ctx->sam_d[SB_CODES], (size_t) total + 16) || ctx->ensure(ctx->sam_d[SB_OFFS], (size_t) (nr + 1) * 8) ||
+        ctx->ensure(ctx->sam_d[SB_REGS], (size_t) (n_regs + 1) * sizeof(bm2_alnreg_t)) || ctx->ensure(ctx->sam_d[SB_REGOFF], (size_t) (nr + 1) * 8)) return 1;
+    BM2_CUDA_OK(cudaMemcpyAsync(ctx->sam_d[SB_CODES].p, reads->codes, (size_t) total, cudaMemcpyHostToDevice, st));
+    BM2_CUDA_OK(cudaMemcpyAsync(ctx->sam_d[SB_OFFS].p, reads->offsets, (size_t) (nr + 1) * 8, cudaMemcpyHostToDevice, st));
+    if (n_regs) BM2_CUDA_OK(cudaMemcpyAsync(ctx->sam_d[SB_REGS].p, regs, (size_t) n_regs * sizeof(bm2_alnreg_t), cudaMemcpyHostToDevice, st));
+    BM2_CUDA_OK(cudaMemcpyAsync(ctx->sam_d[SB_REGOFF].p, read_off, (size_t) (nr + 1) * 8, cudaMemcpyHostToDevice, st));
 
     // ---- capacities of every pair; waves by budget ---------------------------------------------------------------------------
     std::vector<PairDesc> desc((size_t) n_pairs_all);
@@ -340,7 +342,7 @@ int run_sam(bm2_ctx *ctx, const bm2_read_batch *reads, const bm2_alnreg_t *regs,
     // adds a quarter on top, and the seed-and-extend buffers of the next chunk need room beside them.
     size_t dev_free = 0, dev_total = 0;
     BM2_CUDA_OK(cudaMemGetInfo(&dev_free, &dev_total));
-    for (int b : { SB_ARENA, SB_RECS_W, SB_XA_W, SB_OPS_W, SB_MD_W }) dev_free += ctx->d[b].cap;
+    for (int b : { SB_ARENA, SB_RECS_W, SB_XA_W, SB_OPS_W, SB_MD_W }) dev_free += ctx->sam_d[b].cap;
     const size_t budget = std::min((size_t) 32 << 30, std::max((size_t) 1 << 30, dev_free / 8));
     size_t used[4] = { 0, 0, 0, 0 };                        // recs, xa, ops, md of the batch so far
     for (int w0 = 0; w0 < n_pairs_all;) {
@@ -357,14 +359,14 @@ int run_sam(bm2_ctx *ctx, const bm2_read_batch *reads, const bm2_alnreg_t *regs,
             ++w1;
         }
         const int np = w1 - w0;
-        if (ctx->ensure(ctx->d[SB_DESC], (size_t) np * sizeof(PairDesc)) || ctx->ensure(ctx->d[SB_ARENA], arena + 64) ||
-            ctx->ensure(ctx->d[SB_RECS_W], (size_t) (nrec + 1) * sizeof(bm2_sam_rec)) || ctx->ensure(ctx->d[SB_XA_W], (size_t) (nxa + 1) * sizeof(bm2_sam_xa)) ||
-            ctx->ensure(ctx->d[SB_OPS_W], (size_t) (nops + 4) * 4) || ctx->ensure(ctx->d[SB_MD_W], (size_t) nmd + 16) ||
-            ctx->ensure(ctx->d[SB_CNT], (size_t) np * sizeof(PairCount)) || ctx->ensure(ctx->d[SB_FINAL], (size_t) np * sizeof(PairFinal)) ||
-            ctx->ensure_host(ctx->h[SH_CNT], (size_t) np * (sizeof(PairCount) + sizeof(PairFinal)))) return 1;
-        BM2_CUDA_OK(cudaMemcpyAsync(ctx->d[SB_DESC].p, desc.data() + w0, (size_t) np * sizeof(PairDesc), cudaMemcpyHostToDevice, st));
-        if (ctx->ensure(ctx->d[SJ_STATS], 64)) return 1;
-        BM2_CUDA_OK(cudaMemsetAsync(ctx->d[SJ_STATS].p, 0, sizeof(SamStats), st));
+        if (ctx->ensure(ctx->sam_d[SB_DESC], (size_t) np * sizeof(PairDesc)) || ctx->ensure(ctx->sam_d[SB_ARENA], arena + 64) ||
+            ctx->ensure(ctx->sam_d[SB_RECS_W], (size_t) (nrec + 1) * sizeof(bm2_sam_rec)) || ctx->ensure(ctx->sam_d[SB_XA_W], (size_t) (nxa + 1) * sizeof(bm2_sam_xa)) ||
+            ctx->ensure(ctx->sam_d[SB_OPS_W], (size_t) (nops + 4) * 4) || ctx->ensure(ctx->sam_d[SB_MD_W], (size_t) nmd + 16) ||
+            ctx->ensure(ctx->sam_d[SB_CNT], (size_t) np * sizeof(PairCount)) || ctx->ensure(ctx->sam_d[SB_FINAL], (size_t) np * sizeof(PairFinal)) ||
+            ctx->ensure_host(ctx->sam_h[SH_CNT], (size_t) np * (sizeof(PairCount) + sizeof(PairFinal)))) return 1;
+        BM2_CUDA_OK(cudaMemcpyAsync(ctx->sam_d[SB_DESC].p, desc.data() + w0, (size_t) np * sizeof(PairDesc), cudaMemcpyHostToDevice, st));
+        if (ctx->ensure(ctx->sam_d[SJ_STATS], 64)) return 1;
+        BM2_CUDA_OK(cudaMemsetAsync(ctx->sam_d[SJ_STATS].p, 0, sizeof(SamStats), st));
         BM2_CUDA_OK(cudaEventRecord(ctx->sam_ev[0], st));
         if (staged) {
             int64_t bound = 0;
@@ -377,9 +379,9 @@ int run_sam(bm2_ctx *ctx, const bm2_read_batch *reads, const bm2_alnreg_t *regs,
             const size_t list_budget = (size_t) 1 << 30;
             while (ksw_blocks > ctx->n_sm && (size_t) ksw_blocks * 4 * 2 * (size_t) lcap * 4 > list_budget) ksw_blocks >>= 1;
             if ((size_t) ksw_blocks * 4 * 2 * (size_t) lcap * 4 > list_budget) lcap = (int) (list_budget / ((size_t) ksw_blocks * 4 * 2 * 4));   // longer windows: in place
-            if (ctx->ensure(ctx->d[SJ_PAIRJOBS], (size_t) np * sizeof(PairJobs)) || ctx->ensure(ctx->d[SJ_JOBS], ((size_t) job_cap + 1) * sizeof(MateJob)) ||
-                ctx->ensure(ctx->d[SJ_RES], ((size_t) job_cap + 1) * sizeof(MateJobRes)) ||
-                ctx->ensure(ctx->d[SJ_LISTS], (size_t) ksw_blocks * 4 * 2 * (size_t) lcap * 4 + 16)) return 1;
+            if (ctx->ensure(ctx->sam_d[SJ_PAIRJOBS], (size_t) np * sizeof(PairJobs)) || ctx->ensure(ctx->sam_d[SJ_JOBS], ((size_t) job_cap + 1) * sizeof(MateJob)) ||
+                ctx->ensure(ctx->sam_d[SJ_RES], ((size_t) job_cap + 1) * sizeof(MateJobRes)) ||
+                ctx->ensure(ctx->sam_d[SJ_LISTS], (size_t) ksw_blocks * 4 * 2 * (size_t) lcap * 4 + 16)) return 1;
             sam_jobs_kernel<<<(unsigned) ((np + 127) / 128), 128, 0, st>>>(cv, pes, o.min_seed_len, o.pen_unpaired, o.max_matesw, P<int64_t>(ctx, SB_OFFS),
                                                                           P<bm2_alnreg_t>(ctx, SB_REGS), P<int64_t>(ctx, SB_REGOFF), P<PairDesc>(ctx, SB_DESC), np,
                                                                           P<MateJob>(ctx, SJ_JOBS), job_cap, P<PairJobs>(ctx, SJ_PAIRJOBS), P<SamStats>(ctx, SJ_STATS));
@@ -391,7 +393,7 @@ int run_sam(bm2_ctx *ctx, const bm2_read_batch *reads, const bm2_alnreg_t *regs,
                 const size_t per_thread = sam_align16_d((size_t) 3 * (max_l + 16) * 4 + (size_t) 2 * lcap * 4 + (size_t) tcap + (size_t) max_l + 1);
                 int tblocks = ctx->n_sm * 8;
                 while (tblocks > ctx->n_sm && (size_t) tblocks * 128 * per_thread > ((size_t) 4 << 30)) tblocks >>= 1;
-                if (ctx->ensure(ctx->d[SJ_LISTS], (size_t) tblocks * 128 * per_thread + 16)) return 1;
+                if (ctx->ensure(ctx->sam_d[SJ_LISTS], (size_t) tblocks * 128 * per_thread + 16)) return 1;
                 sam_ksw_jobs_thread_kernel<<<(unsigned) tblocks, 128, 0, st>>>(m25, o.a, o.min_seed_len, o.o_del, o.e_del, o.o_ins, o.e_ins, ctx->idx.ref, 2 * ctx->idx.l_pac,
                               P<uint8_t>(ctx, SB_CODES), P<int64_t>(ctx, SB_OFFS), nr, P<MateJob>(ctx, SJ_JOBS), P<SamStats>(ctx, SJ_STATS), job_cap,
                               P<uint8_t>(ctx, SJ_LISTS), per_thread, max_l, lcap, tcap, P<MateJobRes>(ctx, SJ_RES));
@@ -435,8 +437,8 @@ int run_sam(bm2_ctx *ctx, const bm2_read_batch *reads, const bm2_alnreg_t *regs,
             if (env && env[0] == '1') std::stable_sort(keyed.begin(), keyed.end(), [](const std::pair<int, int32_t> &x, const std::pair<int, int32_t> &y) { return x.first < y.first; });
             std::vector<int32_t> order((size_t) np);
             for (int k = 0; k < np; ++k) order[(size_t) k] = keyed[(size_t) k].second;
-            if (ctx->ensure(ctx->d[SB_ORDER], (size_t) np * 4 + 16)) return 1;
-            BM2_CUDA_OK(cudaMemcpyAsync(ctx->d[SB_ORDER].p, order.data(), (size_t) np * 4, cudaMemcpyHostToDevice, st));
+            if (ctx->ensure(ctx->sam_d[SB_ORDER], (size_t) np * 4 + 16)) return 1;
+            BM2_CUDA_OK(cudaMemcpyAsync(ctx->sam_d[SB_ORDER].p, order.data(), (size_t) np * 4, cudaMemcpyHostToDevice, st));
             BM2_CUDA_OK(cudaStreamSynchronize(st));              // (order is a local vector)
         }
         BM2_CUDA_OK(cudaEventRecord(ctx->sam_ev[2], st));
@@ -449,9 +451,9 @@ int run_sam(bm2_ctx *ctx, const bm2_read_batch *reads, const bm2_alnreg_t *regs,
         BM2_CUDA_OK(cudaGetLastError());
         BM2_CUDA_OK(cudaEventRecord(ctx->sam_ev[3], st));
         SamStats wave_stats;
-        BM2_CUDA_OK(cudaMemcpyAsync(&wave_stats, ctx->d[SJ_STATS].p, sizeof(SamStats), cudaMemcpyDeviceToHost, st));
-        PairCount *hc = (PairCount *) ctx->h[SH_CNT].p; PairFinal *hf = (PairFinal *) (hc + np);
-        BM2_CUDA_OK(cudaMemcpyAsync(hc, ctx->d[SB_CNT].p, (size_t) np * sizeof(PairCount), cudaMemcpyDeviceToHost, st));
+        BM2_CUDA_OK(cudaMemcpyAsync(&wave_stats, ctx->sam_d[SJ_STATS].p, sizeof(SamStats), cudaMemcpyDeviceToHost, st));
+        PairCount *hc = (PairCount *) ctx->sam_h[SH_CNT].p; PairFinal *hf = (PairFinal *) (hc + np);
+        BM2_CUDA_OK(cudaMemcpyAsync(hc, ctx->sam_d[SB_CNT].p, (size_t) np * sizeof(PairCount), cudaMemcpyDeviceToHost, st));
         BM2_CUDA_OK(cudaStreamSynchronize(st));
         PairFinal run = { 0, 0, 0, 0 };
         for (int k = 0; k < np; ++k) {
@@ -462,9 +464,9 @@ int run_sam(bm2_ctx *ctx, const bm2_read_batch *reads, const bm2_alnreg_t *regs,
             hf[k] = run;
             run.recs += hc[k].recs; run.xa += hc[k].xa; run.ops += hc[k].ops; run.md += hc[k].md;
         }
-        if (ctx->ensure(ctx->d[SB_RECS], (size_t) (run.recs + 1) * sizeof(bm2_sam_rec)) || ctx->ensure(ctx->d[SB_XA], (size_t) (run.xa + 1) * sizeof(bm2_sam_xa)) ||
-            ctx->ensure(ctx->d[SB_OPS], (size_t) (run.ops + 4) * 4) || ctx->ensure(ctx->d[SB_MD], (size_t) run.md + 16)) return 1;
-        BM2_CUDA_OK(cudaMemcpyAsync(ctx->d[SB_FINAL].p, hf, (size_t) np * sizeof(PairFinal), cudaMemcpyHostToDevice, st));
+        if (ctx->ensure(ctx->sam_d[SB_RECS], (size_t) (run.recs + 1) * sizeof(bm2_sam_rec)) || ctx->ensure(ctx->sam_d[SB_XA], (size_t) (run.xa + 1) * sizeof(bm2_sam_xa)) ||
+            ctx->ensure(ctx->sam_d[SB_OPS], (size_t) (run.ops + 4) * 4) || ctx->ensure(ctx->sam_d[SB_MD], (size_t) run.md + 16)) return 1;
+        BM2_CUDA_OK(cudaMemcpyAsync(ctx->sam_d[SB_FINAL].p, hf, (size_t) np * sizeof(PairFinal), cudaMemcpyHostToDevice, st));
         sam_gather_kernel<<<(unsigned) ((np + 127) / 128), 128, 0, st>>>(P<PairDesc>(ctx, SB_DESC), P<PairCount>(ctx, SB_CNT), P<PairFinal>(ctx, SB_FINAL), np,
                                                                         P<bm2_sam_rec>(ctx, SB_RECS_W), P<bm2_sam_xa>(ctx, SB_XA_W), P<uint32_t>(ctx, SB_OPS_W),
                                                                         P<char>(ctx, SB_MD_W), (int64_t) (used[2] / 4), (int64_t) used[3], P<bm2_sam_rec>(ctx, SB_RECS),
@@ -473,8 +475,8 @@ int run_sam(bm2_ctx *ctx, const bm2_read_batch *reads, const bm2_alnreg_t *regs,
         const size_t add[4] = { (size_t) run.recs * sizeof(bm2_sam_rec), (size_t) run.xa * sizeof(bm2_sam_xa), (size_t) run.ops * 4, (size_t) run.md };
         const int hb[4] = { SH_RECS, SH_XA, SH_OPS, SH_MD }, db[4] = { SB_RECS, SB_XA, SB_OPS, SB_MD };
         for (int k = 0; k < 4; ++k) {
-            if (grow_host(ctx, ctx->h[hb[k]], used[k], used[k] + add[k] + 64)) return 1;
-            if (add[k]) BM2_CUDA_OK(cudaMemcpyAsync((char *) ctx->h[hb[k]].p + used[k], ctx->d[db[k]].p, add[k], cudaMemcpyDeviceToHost, st));
+            if (grow_host(ctx, ctx->sam_h[hb[k]], used[k], used[k] + add[k] + 64)) return 1;
+            if (add[k]) BM2_CUDA_OK(cudaMemcpyAsync((char *) ctx->sam_h[hb[k]].p + used[k], ctx->sam_d[db[k]].p, add[k], cudaMemcpyDeviceToHost, st));
             used[k] += add[k];
         }
         BM2_CUDA_OK(cudaEventRecord(ctx->sam_ev[4], st));
@@ -484,10 +486,10 @@ int run_sam(bm2_ctx *ctx, const bm2_read_batch *reads, const bm2_alnreg_t *regs,
         ctx->sam_counts[4] += wave_stats.window_moved; ctx->sam_counts[5] += 1;
         w0 = w1;
     }
-    out->n_recs = (int64_t) (used[0] / sizeof(bm2_sam_rec)); out->recs = (const bm2_sam_rec *) ctx->h[SH_RECS].p;
-    out->n_xa = (int64_t) (used[1] / sizeof(bm2_sam_xa)); out->xa = (const bm2_sam_xa *) ctx->h[SH_XA].p;
-    out->n_ops = (int64_t) (used[2] / 4); out->cigar = (const uint32_t *) ctx->h[SH_OPS].p;
-    out->n_md = (int64_t) used[3]; out->md = (const char *) ctx->h[SH_MD].p;
+    out->n_recs = (int64_t) (used[0] / sizeof(bm2_sam_rec)); out->recs = (const bm2_sam_rec *) ctx->sam_h[SH_RECS].p;
+    out->n_xa = (int64_t) (used[1] / sizeof(bm2_sam_xa)); out->xa = (const bm2_sam_xa *) ctx->sam_h[SH_XA].p;
+    out->n_ops = (int64_t) (used[2] / 4); out->cigar = (const uint32_t *) ctx->sam_h[SH_OPS].p;
+    out->n_md = (int64_t) used[3]; out->md = (const char *) ctx->sam_h[SH_MD].p;
     return 0;
 }
 }  // namespace
