@@ -206,6 +206,9 @@ SORT_REC_DT = np.dtype([("rid", "<i4"), ("pos", "<i4"), ("end", "<i4"), ("bin", 
 
 # bm2_dup_signatures / bm2_dup_resolve: one entry of a duplicate space (include/bm2_b200.h); kind 0 pair, 1 fragment, 2 pair end
 DUP_ENTRY_DT = np.dtype([("k1", "<u8"), ("k2", "<u8"), ("tid", "<i8"), ("score", "<i4"), ("kind", "<i4")])
+# bm2_dup_signatures_ex / bm2_dup_resolve_ex: a located pair entry; loc bit 0 has a location, bit 1 the orientation class (reverse)
+DUP_LOC_ENTRY_DT = np.dtype([("k1", "<u8"), ("k2", "<u8"), ("tid", "<i8"), ("score", "<i4"), ("kind", "<i4"), ("tile", "<i4"), ("x", "<i4"),
+                             ("y", "<i4"), ("loc", "<i4")])
 
 
 class SortOut(C.Structure):
@@ -218,7 +221,7 @@ EXPORTS = ["bm2_create_sibling", "bm2_fastq_encode", "bm2_seq_encode", "bm2_fast
            "bm2_seed_chain_extend", "bm2_last_stage_ms", "bm2_gen_cigar", "bm2_pestat", "bm2_sam_pe", "bm2_sam_se", "bm2_ksw_align2",
            "bm2_fasta_pack", "bm2_index_build", "bm2_bam_format_ex", "bm2_bgzf_compress", "bm2_last_bgzf_stats",
            "bm2_bam_sort_compress", "bm2_last_sort_stats", "bm2_bam_sort_memory", "bm2_bam_sort_memory_ex", "bm2_bam_sort_compress_ex",
-           "bm2_dup_signatures", "bm2_dup_resolve", "bm2_last_dup_stats", "bm2_dup_set"]
+           "bm2_dup_signatures", "bm2_dup_resolve", "bm2_last_dup_stats", "bm2_dup_set", "bm2_dup_signatures_ex", "bm2_dup_resolve_ex"]
 
 _lib = None
 
@@ -610,6 +613,42 @@ class Context:
         if resolve:
             return (_host(d.value, nd.value, np.int64) if nd.value else np.zeros(0, np.int64)), ms.value
         return (_host(srt.value, len(e), DUP_ENTRY_DT) if len(e) else np.zeros(0, DUP_ENTRY_DT)), ms.value
+
+    def dup_signatures_ex(self, data: bytes, starts, tmpl_first, tmpl_id):
+        """bm2_dup_signatures_ex: dup_signatures with the pair entries located -> (pair entries DUP_LOC_ENTRY_DT, fragment-space entries
+        DUP_ENTRY_DT, (secondary or supplementary records, unmapped primaries), device ms)."""
+        starts = np.ascontiguousarray(starts, np.int64); tf = np.ascontiguousarray(tmpl_first, np.int64); ti = np.ascontiguousarray(tmpl_id, np.int64)
+        buf = np.frombuffer(data, np.uint8) if len(data) else np.zeros(1, np.uint8)
+        sb = starts if len(starts) else np.zeros(1, np.int64)
+        tib = ti if len(ti) else np.zeros(1, np.int64)
+        p, f_ = C.c_void_p(), C.c_void_p(); n_p, n_f = C.c_int64(), C.c_int64()
+        counts = np.zeros(2, np.int64)
+        f = lib().bm2_dup_signatures_ex
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64] + [C.c_void_p] * 5
+        self._check(f(self._ctx, buf.ctypes.data, len(data), sb.ctypes.data, len(starts), tf.ctypes.data, tib.ctypes.data, len(ti),
+                      C.byref(p), C.byref(n_p), C.byref(f_), C.byref(n_f), counts.ctypes.data), "bm2_dup_signatures_ex")
+        ms = C.c_double()
+        lib().bm2_last_dup_stats.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        lib().bm2_last_dup_stats(self._ctx, C.byref(ms), None)
+        return (_host(p.value, n_p.value, DUP_LOC_ENTRY_DT) if n_p.value else np.zeros(0, DUP_LOC_ENTRY_DT),
+                _host(f_.value, n_f.value, DUP_ENTRY_DT) if n_f.value else np.zeros(0, DUP_ENTRY_DT), (int(counts[0]), int(counts[1])), ms.value)
+
+    def dup_resolve_ex(self, entries, distance: int = 100, resolve: bool = True):
+        """bm2_dup_resolve_ex: located entries (DUP_LOC_ENTRY_DT) of one space -> (the sorted located entries, device ms) when not resolve,
+        else (the duplicates' template ids in sorted order, the optical count at pixel distance `distance`, device ms)."""
+        e = np.ascontiguousarray(entries, DUP_LOC_ENTRY_DT)
+        eb = e if len(e) else np.zeros(1, DUP_LOC_ENTRY_DT)
+        srt, d = C.c_void_p(), C.c_void_p(); nd, nopt = C.c_int64(), C.c_int64()
+        f = lib().bm2_dup_resolve_ex
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        self._check(f(self._ctx, eb.ctypes.data, len(e), int(resolve), int(distance), None if resolve else C.byref(srt), C.byref(d) if resolve else None,
+                      C.byref(nd) if resolve else None, C.byref(nopt) if resolve else None), "bm2_dup_resolve_ex")
+        ms = C.c_double()
+        lib().bm2_last_dup_stats.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        lib().bm2_last_dup_stats(self._ctx, None, C.byref(ms))
+        if resolve:
+            return (_host(d.value, nd.value, np.int64) if nd.value else np.zeros(0, np.int64)), nopt.value, ms.value
+        return (_host(srt.value, len(e), DUP_LOC_ENTRY_DT) if len(e) else np.zeros(0, DUP_LOC_ENTRY_DT)), ms.value
 
     def dup_set(self, dup_tids, n_bits: int):
         """bm2_dup_set: the bitset of n_bits bits with the templates dup_tids set, kept on this context for bam_sort_compress_ex."""

@@ -24,6 +24,10 @@
 //           then grows by one entry per member of the largest group).  The duplicate templates become a bitset of 1 bit per input read,
 //           uploaded to the sort context before the one-run sort or the first merge window, which set 0x400 on their records.
 //
+//   metrics (--markdup-metrics) the pair space holds located entries (bm2_dup_loc_entry, 48 bytes, counted as such against sig_bytes, and
+//           spilled as such), resolved by the located call, which also returns the optical count of the call's pair groups.  A group never
+//           straddles a window, so the sum over the windows is exact.
+//
 // The device calls are parameters, so that tests/host_emul/bam_sort_emul.cpp and markdup_emul.cpp run all of this with the GPU swapped for a
 // CPU restatement.
 #pragma once
@@ -51,6 +55,9 @@ using SortCallEx = std::function<int(const uint8_t *recs, int64_t n, const int64
 // the entries of one duplicate space sorted (resolve 0) or resolved into the duplicates' template ids (bm2_dup_resolve's arguments)
 using DupCall = std::function<int(const bm2_dup_entry *e, int64_t n, int resolve, const bm2_dup_entry **sorted, const int64_t **dups, int64_t *n_dups,
                                   double *device_s)>;
+// the same over located entries with the optical count at the sink's optical_distance (bm2_dup_resolve_ex's arguments)
+using DupCallEx = std::function<int(const bm2_dup_loc_entry *e, int64_t n, int resolve, const bm2_dup_loc_entry **sorted, const int64_t **dups,
+                                    int64_t *n_dups, int64_t *n_optical, double *device_s)>;
 // the duplicate bitset to the sort context (bm2_dup_set)
 using DupSetCall = std::function<int(const uint64_t *bits, int64_t n_bits)>;
 // reports an error and does not return
@@ -147,6 +154,7 @@ struct BamSortSink {
     SortCall sort; SortFail fail;
     SortCallEx sort_ex;                          // when set, used instead of sort
     DupCall dup; DupSetCall dup_set;             // --markdup when dup is set (sort_ex must be set then)
+    DupCallEx dup_ex;                            // --markdup-metrics: the pair space through this one, with add_sigs_ex
     int64_t run_bytes = (int64_t) 2 << 30;
     int64_t sig_bytes = (int64_t) 256 << 20;     // entries held on the host (--sort-mem / 8)
     int64_t n_reads = 0;                         // the duplicate bitset's bits: set before finish
@@ -159,10 +167,12 @@ struct BamSortSink {
     std::vector<Run> runs;
     std::vector<bm2_dup_entry> sig_cur[2], sig_pend[2];   // [0] pair space, [1] fragment space
     std::vector<SigRun> sig_runs[2];
+    std::vector<bm2_dup_loc_entry> lsig_cur, lsig_pend;   // the pair space with dup_ex
     // stats
     double sort_s = 0, merge_s = 0, markdup_s = 0;
     int64_t spill_bytes = 0, merge_windows = 0;
     int64_t dup_templates = 0, dup_pair_templates = 0, dup_frag_templates = 0, dup_records = 0, dup_sig_runs = 0, dup_sig_bytes = 0;
+    int64_t dup_pair_entries = 0, dup_frag_entries = 0, dup_optical_pairs = 0;   // with dup_ex: pair and fragment entries, optical duplicates
 
     ~BamSortSink() {
         if (sorter.joinable()) sorter.join();
@@ -201,34 +211,61 @@ struct BamSortSink {
         for (int64_t i = 0; i < n_frags; ++i) dup_templates += frags[i].kind == 1;
         sig_cur[0].insert(sig_cur[0].end(), pairs, pairs + n_pairs);
         sig_cur[1].insert(sig_cur[1].end(), frags, frags + n_frags);
-        if ((int64_t) ((sig_cur[0].size() + sig_cur[1].size()) * sizeof(bm2_dup_entry)) > sig_bytes / 2) {
+        maybe_spill_sigs();
+    }
+
+    // the same with located pair entries (bm2_dup_signatures_ex), for dup_ex
+    void add_sigs_ex(const bm2_dup_loc_entry *pairs, int64_t n_pairs, const bm2_dup_entry *frags, int64_t n_frags) {
+        dup_templates += n_pairs; dup_pair_entries += n_pairs;
+        for (int64_t i = 0; i < n_frags; ++i) { dup_templates += frags[i].kind == 1; dup_frag_entries += frags[i].kind == 1; }
+        lsig_cur.insert(lsig_cur.end(), pairs, pairs + n_pairs);
+        sig_cur[1].insert(sig_cur[1].end(), frags, frags + n_frags);
+        maybe_spill_sigs();
+    }
+
+    void move_sigs_to_pending() {
+        for (int s = 0; s < 2; ++s) { sig_pend[s].swap(sig_cur[s]); sig_cur[s].clear(); }
+        lsig_pend.swap(lsig_cur); lsig_cur.clear();
+    }
+
+    void maybe_spill_sigs() {
+        if ((int64_t) ((sig_cur[0].size() + sig_cur[1].size()) * sizeof(bm2_dup_entry) + lsig_cur.size() * sizeof(bm2_dup_loc_entry)) > sig_bytes / 2) {
             if (sorter.joinable()) sorter.join();
-            for (int s = 0; s < 2; ++s) { sig_pend[s].swap(sig_cur[s]); sig_cur[s].clear(); }
+            move_sigs_to_pending();
             sorter = std::thread([this] { spill_sigs(); });
         }
+    }
+
+    int sort_entries(const bm2_dup_entry *e, int64_t n, const bm2_dup_entry **sorted, double *ds) { return dup(e, n, 0, sorted, nullptr, nullptr, ds); }
+    int sort_entries(const bm2_dup_loc_entry *e, int64_t n, const bm2_dup_loc_entry **sorted, double *ds) {
+        return dup_ex(e, n, 0, sorted, nullptr, nullptr, nullptr, ds);
     }
 
     // the pending entries, sorted on the device, as one more signature run of each space
     void spill_sigs() {
         for (int s = 0; s < 2; ++s) {
-            std::vector<bm2_dup_entry> &v = sig_pend[s];
-            if (v.empty()) continue;
-            char name[32];
-            snprintf(name, sizeof name, "d%04d", (int) (sig_runs[0].size() + sig_runs[1].size()));
-            const std::string path = tmp_prefix + name;
-            SigRun r;
-            r.f = open_tmp(path, fail);
-            const bm2_dup_entry *sorted = nullptr; double ds = 0;
-            if (dup(v.data(), (int64_t) v.size(), 0, &sorted, nullptr, nullptr, &ds)) fail("bm2_dup_resolve");
-            markdup_s += ds;
-            if (fwrite(sorted, sizeof(bm2_dup_entry), v.size(), r.f) != v.size() || fflush(r.f) || fseek(r.f, 0, SEEK_SET))
-                fail("cannot write the temporary file " + path);
-            r.n = (int64_t) v.size();
-            dup_sig_bytes += r.n * (int64_t) sizeof(bm2_dup_entry);
-            sig_runs[s].push_back(r);
-            std::vector<bm2_dup_entry>().swap(v);
+            if (s == 0 && dup_ex) spill_space(lsig_pend, 0);
+            else spill_space(sig_pend[s], s);
         }
         ++dup_sig_runs;
+    }
+
+    template <class E> void spill_space(std::vector<E> &v, int s) {
+        if (v.empty()) return;
+        char name[32];
+        snprintf(name, sizeof name, "d%04d", (int) (sig_runs[0].size() + sig_runs[1].size()));
+        const std::string path = tmp_prefix + name;
+        SigRun r;
+        r.f = open_tmp(path, fail);
+        const E *sorted = nullptr; double ds = 0;
+        if (sort_entries(v.data(), (int64_t) v.size(), &sorted, &ds)) fail(sizeof(E) == sizeof(bm2_dup_entry) ? "bm2_dup_resolve" : "bm2_dup_resolve_ex");
+        markdup_s += ds;
+        if (fwrite(sorted, sizeof(E), v.size(), r.f) != v.size() || fflush(r.f) || fseek(r.f, 0, SEEK_SET))
+            fail("cannot write the temporary file " + path);
+        r.n = (int64_t) v.size();
+        dup_sig_bytes += r.n * (int64_t) sizeof(E);
+        sig_runs[s].push_back(r);
+        std::vector<E>().swap(v);
     }
 
     // the current run to the sorter thread, once the one before is on disk
@@ -294,69 +331,90 @@ struct BamSortSink {
         dup_records = w.marked;
     }
 
-    static bool key_less(const bm2_dup_entry &a, const bm2_dup_entry &b) { return a.k1 != b.k1 ? a.k1 < b.k1 : a.k2 < b.k2; }
+    static const bm2_dup_entry &base(const bm2_dup_entry &e) { return e; }
+    static const bm2_dup_entry &base(const bm2_dup_loc_entry &e) { return e.e; }
+    template <class E> static bool key_less(const E &x, const E &y) {
+        const bm2_dup_entry &a = base(x), &b = base(y);
+        return a.k1 != b.k1 ? a.k1 < b.k1 : a.k2 < b.k2;
+    }
 
     // every duplicate template of both spaces, as the bitset given to dup_set
     void resolve() {
         std::vector<uint64_t> bits((size_t) ((n_reads + 63) / 64), 0);
         const bool spilled = dup_sig_runs > 0;
-        if (spilled && (!sig_cur[0].empty() || !sig_cur[1].empty())) {
-            for (int s = 0; s < 2; ++s) { sig_pend[s].swap(sig_cur[s]); sig_cur[s].clear(); }
+        if (spilled && (!sig_cur[0].empty() || !sig_cur[1].empty() || !lsig_cur.empty())) {
+            move_sigs_to_pending();
             spill_sigs();
         }
+        auto mark = [&](const int64_t *d, int64_t nd, int64_t &count) {
+            for (int64_t i = 0; i < nd; ++i) {
+                if (d[i] < 0 || d[i] >= n_reads) fail("a duplicate template id beyond the reads");
+                bits[(size_t) (d[i] >> 6)] |= (uint64_t) 1 << (d[i] & 63);
+            }
+            count += nd;
+        };
         for (int s = 0; s < 2; ++s) {
             int64_t &count = s ? dup_frag_templates : dup_pair_templates;
-            auto take = [&](const std::vector<bm2_dup_entry> &v) {
+            if (s == 0 && dup_ex) {
+                resolve_space(lsig_cur, sig_runs[0], spilled, [&](const std::vector<bm2_dup_loc_entry> &v) {
+                    const int64_t *d = nullptr; int64_t nd = 0, nopt = 0; double ds = 0;
+                    if (dup_ex(v.data(), (int64_t) v.size(), 1, nullptr, &d, &nd, &nopt, &ds)) fail("bm2_dup_resolve_ex");
+                    markdup_s += ds;
+                    dup_optical_pairs += nopt;
+                    mark(d, nd, count);
+                });
+                continue;
+            }
+            resolve_space(sig_cur[s], sig_runs[s], spilled, [&](const std::vector<bm2_dup_entry> &v) {
                 const int64_t *d = nullptr; int64_t nd = 0; double ds = 0;
                 if (dup(v.data(), (int64_t) v.size(), 1, nullptr, &d, &nd, &ds)) fail("bm2_dup_resolve");
                 markdup_s += ds;
-                for (int64_t i = 0; i < nd; ++i) {
-                    if (d[i] < 0 || d[i] >= n_reads) fail("a duplicate template id beyond the reads");
-                    bits[(size_t) (d[i] >> 6)] |= (uint64_t) 1 << (d[i] & 63);
-                }
-                count += nd;
-            };
-            if (!spilled) { take(sig_cur[s]); std::vector<bm2_dup_entry>().swap(sig_cur[s]); continue; }
-            // the sorted runs window by window: keys strictly below T settle, so every group is resolved whole
-            std::vector<SigRun> &rs = sig_runs[s];
-            const size_t nr = rs.size();
-            if (!nr) continue;
-            const int64_t quota = std::max<int64_t>(sig_bytes / (int64_t) sizeof(bm2_dup_entry) / (int64_t) nr, 1);
-            std::vector<std::vector<bm2_dup_entry>> buf(nr);
-            std::vector<int64_t> left(nr);
-            for (size_t r = 0; r < nr; ++r) left[r] = rs[r].n;
-            auto load = [&](size_t r, int64_t k) {
-                k = std::min(k, left[r]);
-                if (k <= 0) return;
-                const size_t at = buf[r].size();
-                buf[r].resize(at + (size_t) k);
-                if (fread(buf[r].data() + at, sizeof(bm2_dup_entry), (size_t) k, rs[r].f) != (size_t) k) fail("cannot read a temporary file");
-                left[r] -= k;
-            };
-            std::vector<bm2_dup_entry> win;
-            for (bool grow = false;;) {
-                for (size_t r = 0; r < nr; ++r) if (!grow) load(r, quota - (int64_t) buf[r].size());
-                grow = false;
-                bool open = false; bm2_dup_entry T{};
-                for (size_t r = 0; r < nr; ++r)
-                    if (left[r] > 0 && (!open || key_less(buf[r].back(), T))) { T = buf[r].back(); open = true; }
-                win.clear();
-                for (size_t r = 0; r < nr; ++r) {
-                    size_t k = 0;
-                    while (k < buf[r].size() && (!open || key_less(buf[r][k], T))) ++k;
-                    win.insert(win.end(), buf[r].begin(), buf[r].begin() + (long) k);
-                    buf[r].erase(buf[r].begin(), buf[r].begin() + (long) k);
-                }
-                if (open && win.empty()) {               // one group fills the window: load more of the runs that end in it
-                    for (size_t r = 0; r < nr; ++r) if (left[r] > 0 && !key_less(T, buf[r].back())) load(r, quota);
-                    grow = true;
-                    continue;
-                }
-                if (!win.empty()) take(win);
-                if (!open) break;
-            }
+                mark(d, nd, count);
+            });
         }
         if (dup_set(bits.data(), n_reads)) fail("bm2_dup_set");
+    }
+
+    // one space: its entries in one call when nothing spilled, else its sorted runs window by window, keys strictly below T settling, so
+    // that every group is resolved whole
+    template <class E, class Take> void resolve_space(std::vector<E> &cur, std::vector<SigRun> &rs, bool spilled, Take take) {
+        if (!spilled) { take(cur); std::vector<E>().swap(cur); return; }
+        const size_t nr = rs.size();
+        if (!nr) return;
+        const int64_t quota = std::max<int64_t>(sig_bytes / (int64_t) sizeof(E) / (int64_t) nr, 1);
+        std::vector<std::vector<E>> buf(nr);
+        std::vector<int64_t> left(nr);
+        for (size_t r = 0; r < nr; ++r) left[r] = rs[r].n;
+        auto load = [&](size_t r, int64_t k) {
+            k = std::min(k, left[r]);
+            if (k <= 0) return;
+            const size_t at = buf[r].size();
+            buf[r].resize(at + (size_t) k);
+            if (fread(buf[r].data() + at, sizeof(E), (size_t) k, rs[r].f) != (size_t) k) fail("cannot read a temporary file");
+            left[r] -= k;
+        };
+        std::vector<E> win;
+        for (bool grow = false;;) {
+            for (size_t r = 0; r < nr; ++r) if (!grow) load(r, quota - (int64_t) buf[r].size());
+            grow = false;
+            bool open = false; E T{};
+            for (size_t r = 0; r < nr; ++r)
+                if (left[r] > 0 && (!open || key_less(buf[r].back(), T))) { T = buf[r].back(); open = true; }
+            win.clear();
+            for (size_t r = 0; r < nr; ++r) {
+                size_t k = 0;
+                while (k < buf[r].size() && (!open || key_less(buf[r][k], T))) ++k;
+                win.insert(win.end(), buf[r].begin(), buf[r].begin() + (long) k);
+                buf[r].erase(buf[r].begin(), buf[r].begin() + (long) k);
+            }
+            if (open && win.empty()) {               // one group fills the window: load more of the runs that end in it
+                for (size_t r = 0; r < nr; ++r) if (left[r] > 0 && !key_less(T, buf[r].back())) load(r, quota);
+                grow = true;
+                continue;
+            }
+            if (!win.empty()) take(win);
+            if (!open) break;
+        }
     }
 
     struct Cursor {                              // a run being merged

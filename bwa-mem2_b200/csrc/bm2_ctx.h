@@ -86,12 +86,13 @@ struct bm2_ctx {
     std::vector<bm2_sort_rec> sort_recs;
     std::vector<int64_t> sort_tids;        // bm2_bam_sort_compress_ex: the template ids in output order
     // bm2_dup_signatures / bm2_dup_resolve / bm2_dup_set (markdup.cu): buffers, events, the last calls' device times and outputs, the bitset
-    DevBuf dup_d[14];
+    DevBuf dup_d[26];
     DevBuf dup_bits;
     int64_t dup_n_bits = 0;
     cudaEvent_t dup_ev[4] = {nullptr, nullptr, nullptr, nullptr};
     double dup_sig_ms = 0, dup_resolve_ms = 0;
     std::vector<bm2_dup_entry> dup_pairs, dup_frags, dup_sorted;
+    std::vector<bm2_dup_loc_entry> dup_lpairs, dup_lsorted;   // the _ex calls' located pair entries and sorted entries
     std::vector<int64_t> dup_ids;
 
     int ensure(DevBuf &b, size_t bytes);

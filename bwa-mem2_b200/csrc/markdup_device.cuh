@@ -15,6 +15,21 @@
 //   groups      entries with the same key, sorted by (key, score descending, template id).  Pair space: the first entry is kept, every other is
 //               a duplicate.  Fragment space: a group that holds a pair-end entry makes every fragment entry in it a duplicate; otherwise the
 //               first fragment entry is kept and the others are duplicates.  Pair-end entries are never duplicates.
+//
+// Optical duplicates (--markdup-metrics) are counted, never marked apart: Picard's defaults give them 0x400 like any other duplicate.
+//   location    of a template: the QNAME of its first record split on ':'.  Exactly 5 or 7 fields: tile, x, y from the last three, each as
+//               Picard's rapidParseInt (dup_parse_int); a field without a digit means no location.  Any other count (more than 7 included):
+//               no location.  The lane is not part of it.
+//   class       of a pair template: the strand of its primary with 0x40 (its first primary's when neither has 0x40), Picard's
+//               orientationForOpticalDuplicates split: an FR / RF group can hold both classes, counted apart; an FF / RR group holds one
+//   optical     of a pair group of 2 .. DUP_OPTICAL_MAX_SET members: within one class, two members are linked when both have a location,
+//               the same tile, |x1-x2| <= d and |y1-y2| <= d (in 64 bits); the count is the sum over the connected components of size - 1,
+//               a member without a location being a component of its own.  This is the count of Picard's graph path and of its small-set
+//               path, wherever the keeper sits.  It is at most the group's duplicates (size - 1).  Larger groups and fragment groups: 0.
+//   cells       (the exact pass of groups larger than a warp, markdup.cu) members of one class and tile binned by (floor(x / (d+1)),
+//               floor(y / (d+1))): two members of a cell are always linked, so a cell is one component, and only the four neighbouring cells
+//               behind a cell need tests - side neighbours by the cells' extreme x or y alone, diagonal ones per member by a binary search
+//               in the x-sorted neighbour and its suffix extreme of y (dup_cell_diag_linked).
 #pragma once
 #include "hd.h"
 #include "bam_sort_device.cuh"
@@ -138,3 +153,71 @@ BM2_HD uint16_t dup_marked_flag(uint16_t flag, int64_t tid, const uint64_t *bits
 }
 // the score key of the radix sort: descending score as an ascending 15-bit key (scores are at most 2 x 16383)
 BM2_HD uint64_t dup_score_key(int32_t score) { return (uint64_t) (32767 - score); }
+
+// ---- optical duplicates ----
+enum { DUP_LOC_HAS = 1, DUP_LOC_REV = 2 };
+constexpr int64_t DUP_OPTICAL_MAX_SET = 300000;          // Picard's MAX_OPTICAL_DUPLICATE_SET_SIZE
+
+// Picard's rapidParseInt of p[0..len): an optional leading '-', then the decimal digits up to the first non-digit, accumulated as a Java int
+// (wrapping); false when there is no digit
+BM2_HD bool dup_parse_int(const uint8_t *p, int len, int32_t *v) {
+    int i = 0;
+    const bool neg = len > 0 && p[0] == '-';
+    if (neg) i = 1;
+    uint32_t a = 0;
+    bool any = false;
+    for (; i < len && p[i] >= '0' && p[i] <= '9'; ++i) { a = a * 10u + (uint32_t) (p[i] - '0'); any = true; }
+    *v = (int32_t) (neg ? 0u - a : a);
+    return any;
+}
+
+// the location from the name's length and its colons: nc of them, c1 < c2 < c3 the last three (-1 when fewer).  Returns the loc bits (0 or
+// DUP_LOC_HAS) and sets tile / x / y (0 without a location).
+BM2_HD int dup_location_from_colons(const uint8_t *name, int len, int nc, int c1, int c2, int c3, int32_t *tile, int32_t *x, int32_t *y) {
+    *tile = *x = *y = 0;
+    if (nc != 4 && nc != 6) return 0;
+    int32_t t, a, b;
+    if (!dup_parse_int(name + c1 + 1, c2 - c1 - 1, &t) || !dup_parse_int(name + c2 + 1, c3 - c2 - 1, &a) || !dup_parse_int(name + c3 + 1, len - c3 - 1, &b))
+        return 0;
+    *tile = t; *x = a; *y = b;
+    return DUP_LOC_HAS;
+}
+
+// the same from the name alone, one byte at a time (the kernel finds the colons with a ballot)
+BM2_HD int dup_name_location(const uint8_t *name, int len, int32_t *tile, int32_t *x, int32_t *y) {
+    int nc = 0, c1 = -1, c2 = -1, c3 = -1;
+    for (int i = 0; i < len; ++i) if (name[i] == ':') { c1 = c2; c2 = c3; c3 = i; ++nc; }
+    return dup_location_from_colons(name, len, nc, c1, c2, c3, tile, x, y);
+}
+
+// a pair template's class from its two primaries' flags
+BM2_HD int dup_pair_class(int32_t flag0, int32_t flag1) {
+    const int32_t f = (flag0 & 0x40) || !(flag1 & 0x40) ? flag0 : flag1;
+    return (f & 16) ? DUP_LOC_REV : 0;
+}
+
+BM2_HD bool dup_optical_linked(const bm2_dup_loc_entry &a, const bm2_dup_loc_entry &b, int64_t d) {
+    if (!(a.loc & DUP_LOC_HAS) || !(b.loc & DUP_LOC_HAS) || a.loc != b.loc || a.tile != b.tile) return false;
+    const int64_t dx = (int64_t) a.x - b.x, dy = (int64_t) a.y - b.y;
+    return dx <= d && -dx <= d && dy <= d && -dy <= d;
+}
+
+// a coordinate's cell: floor(v / (d + 1)), as an order-preserving unsigned 32-bit value (|v| <= 2^31, d + 1 >= 1)
+BM2_HD uint32_t dup_cell(int32_t v, int64_t d) {
+    const int64_t w = d + 1, c = v >= 0 ? (int64_t) v / w : -((-(int64_t) v + w - 1) / w);
+    return (uint32_t) ((int32_t) c) ^ 0x80000000u;
+}
+// the cell sort's keys: (group, class, tile) and (cx, cy)
+BM2_HD uint64_t dup_cell_hi(uint32_t group, const bm2_dup_loc_entry &e) {
+    return (uint64_t) group << 33 | (uint64_t) ((e.loc & DUP_LOC_REV) ? 1 : 0) << 32 | (uint64_t) ((uint32_t) e.tile ^ 0x80000000u);
+}
+BM2_HD uint64_t dup_cell_lo(const bm2_dup_loc_entry &e, int64_t d) { return (uint64_t) dup_cell(e.x, d) << 32 | dup_cell(e.y, d); }
+
+// b against the cell A behind it diagonally (cx - 1, cy - 1 when below, cy + 1 when above): A's members ax[0..n) sorted by x, with
+// suf[k] the max (below) or min (above) of their y over [k, n).  Linked when some a has ax >= bx - d and ay within d of by.
+BM2_HD bool dup_cell_diag_linked(const int32_t *ax, const int32_t *suf, int64_t n, int32_t bx, int32_t by, int64_t d, bool below) {
+    int64_t lo = 0, hi = n;                              // the first a with ax >= bx - d
+    while (lo < hi) { const int64_t m = (lo + hi) / 2; if ((int64_t) ax[m] < (int64_t) bx - d) lo = m + 1; else hi = m; }
+    if (lo == n) return false;
+    return below ? (int64_t) suf[lo] >= (int64_t) by - d : (int64_t) suf[lo] <= (int64_t) by + d;
+}

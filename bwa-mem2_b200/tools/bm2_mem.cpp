@@ -23,6 +23,8 @@
 //        then bm2_bam_sort_compress_ex  --sort: the records in sorted runs, merged, compressed on the GPU, and the BAI (bam_sort.h)
 //        with bm2_dup_signatures     --markdup: each chunk's templates' entries, resolved by bm2_dup_resolve at the end; the duplicates' records get
 //                                    0x400 in the same sort, which then carries each record's template id (bam_sort.h, markdup_device.cuh)
+//        or bm2_dup_signatures_ex    --markdup-metrics: the same with located pair entries and the chunk's record counts, resolved by
+//                                    bm2_dup_resolve_ex with the optical pass; Picard's metrics file at the end (markdup_metrics.h)
 // Chunks in flight: the reference's kt_pipeline runs its three steps (read, process, write) on two worker threads so that one chunk's I/O
 // overlaps another's computation (src/fastmap.cpp:952-1003, src/kthread.cpp:122-176).  Here -p workers (default 2) each own a context
 // (bm2_create_sibling: one index in HBM) and take whole chunks off a queue; the GPU interleaves the kernels of the two chunks, the host side of
@@ -37,6 +39,7 @@
 #include "../csrc/seq_grammar.cuh"
 #include "../csrc/read_input.h"
 #include "../csrc/bam_sort.h"
+#include "../csrc/markdup_metrics.h"
 #include <algorithm>
 #include <chrono>
 #include <condition_variable>
@@ -78,6 +81,7 @@ struct Shared {
     bool copy_comment = false, bam = false;
     BamSortSink *sink = nullptr;                                 // --sort: the records go to the sorted runs instead of the output
     bool markdup = false; double t_dup_sig = 0;                  // --markdup: device time of the signature kernels
+    bool metrics = false; long long n_sec_supp = 0, n_unmapped = 0;   // --markdup-metrics: the records' counts of the signature kernels
     double t_split = 0;
     long long seq_chunks = 0;                                    // chunks that went through bm2_seq_encode
     size_t in_flight = 0;                                        // bytes of the chunks queued or being aligned
@@ -226,11 +230,15 @@ void worker(Shared *sh, bm2_ctx *ctx) {
         }
         ChunkTemplates tpl;
         const bm2_dup_entry *dp = nullptr, *df = nullptr; int64_t ndp = 0, ndf = 0;
+        const bm2_dup_loc_entry *dlp = nullptr; int64_t counts[2] = { 0, 0 };
         double sig_ms = 0;
         if (sh->markdup) {                                               // the templates' entries, on this worker's context
             chunk_templates(text, len, read_end, mate, ck.first_read, tpl);
-            if (bm2_dup_signatures(ctx, (const uint8_t *) text, len, tpl.starts.data(), (int64_t) tpl.starts.size(), tpl.first.data(), tpl.id.data(),
-                                   (int64_t) tpl.id.size(), &dp, &ndp, &df, &ndf)) die("bm2_dup_signatures", ctx);
+            if (sh->metrics) {
+                if (bm2_dup_signatures_ex(ctx, (const uint8_t *) text, len, tpl.starts.data(), (int64_t) tpl.starts.size(), tpl.first.data(), tpl.id.data(),
+                                          (int64_t) tpl.id.size(), &dlp, &ndp, &df, &ndf, counts)) die("bm2_dup_signatures_ex", ctx);
+            } else if (bm2_dup_signatures(ctx, (const uint8_t *) text, len, tpl.starts.data(), (int64_t) tpl.starts.size(), tpl.first.data(), tpl.id.data(),
+                                          (int64_t) tpl.id.size(), &dp, &ndp, &df, &ndf)) die("bm2_dup_signatures", ctx);
             bm2_last_dup_stats(ctx, &sig_ms, nullptr);
         }
         const uint8_t *outp = (const uint8_t *) text; int64_t out_len = len;
@@ -250,7 +258,8 @@ void worker(Shared *sh, bm2_ctx *ctx) {
         const double t6 = now_s();
         if (sh->sink) {
             sh->sink->add(outp, out_len, sh->markdup ? tpl.rec_id.data() : nullptr);
-            if (sh->markdup) sh->sink->add_sigs(dp, ndp, df, ndf);
+            if (sh->metrics) sh->sink->add_sigs_ex(dlp, ndp, df, ndf);
+            else if (sh->markdup) sh->sink->add_sigs(dp, ndp, df, ndf);
         }
         else fwrite(outp, 1, (size_t) out_len, sh->out);
         bm2_free(text);
@@ -258,7 +267,7 @@ void worker(Shared *sh, bm2_ctx *ctx) {
         {
             std::lock_guard<std::mutex> lk(sh->mu);
             sh->t_enc += t1 - t0; sh->t_aln += t.aln; sh->t_pes += t.pes; sh->t_sam += t.sam; sh->t_fmt += t.fmt; sh->t_turn += t6 - t5; sh->t_write += t7 - t6;
-            sh->t_bam += t.bam; sh->t_bgzf += bgzf_ms / 1e3; sh->t_dup_sig += sig_ms / 1e3; sh->bam_bytes += sh->bam ? len : 0; sh->bgzf_bytes += sh->bam && !sh->sink ? out_len : 0;
+            sh->t_bam += t.bam; sh->t_bgzf += bgzf_ms / 1e3; sh->t_dup_sig += sig_ms / 1e3; sh->n_sec_supp += counts[0]; sh->n_unmapped += counts[1]; sh->bam_bytes += sh->bam ? len : 0; sh->bgzf_bytes += sh->bam && !sh->sink ? out_len : 0;
             sh->n_processed += fq.n_reads; sh->seq_chunks += !ck.simple; sh->in_flight -= ck.bytes.size();
             sh->chunk_s.push_back(t7 - t0); sh->chunk_done_s.push_back(t7 - sh->t_loop); sh->chunk_reads.push_back(fq.n_reads);
             ++sh->next_to_write;
@@ -332,7 +341,11 @@ void usage(const bm2_mem_opt_t &o) {
 "  --write-index  write the BAI index <out>.bai (needs --sort and -o)\n"
 "  --markdup   mark duplicates (flag 0x400) in the sorted BAM (implies --sort): templates with the same unclipped 5' ends and strands,\n"
 "              the one with the highest sum of base qualities >= 15 kept (ties: the first in the input); Picard MarkDuplicates's\n"
-"              defaults without optical duplicates, not claimed byte-equal to it.  Holds --sort-mem / 8 bytes of signatures on the host\n"
+"              defaults, not claimed byte-equal to it (optical duplicates are marked like the others).  Holds --sort-mem / 8 bytes of\n"
+"              signatures on the host\n"
+"  --markdup-metrics FILE  write Picard's duplication metrics for the one library (-R's LB, else Unknown Library) to FILE, with optical\n"
+"              duplicates counted on the GPU from Illumina read names (implies --markdup)\n"
+"  --optical-distance N  the largest pixel distance of two optical duplicates, 0 to 2147483647 (needs --markdup-metrics) [100]\n"
 "  --dump-opt  print the parsed options, the -I values, the read group and the header as JSON, and exit before any GPU work\n"
 "  --dump-chunks  print the chunks the input is cut into (first read, byte ranges, whether bm2_fastq_encode takes them) as JSON lines,\n"
 "              and exit without loading the index\n",
@@ -416,6 +429,22 @@ std::string coordinate_header(const std::string &h) {
     return (hd.empty() ? std::string("@HD\tVN:1.6\tSO:coordinate") : hd) + "\n" + rest;
 }
 
+// "N" of --optical-distance: a decimal integer in [0, 2^31 - 1]
+bool parse_distance(const char *s, long long *v) {
+    if (!*s || strlen(s) > 10) return false;
+    for (const char *p = s; *p; ++p) if (!isdigit((unsigned char) *p)) return false;
+    *v = atoll(s);
+    return *v <= INT32_MAX;
+}
+
+// the LB field of a read group line, or "" without one
+std::string rg_library(const std::string &rg) {
+    const size_t at = rg.find("\tLB:");
+    if (at == std::string::npos) return std::string();
+    const size_t b = at + 4, e = rg.find_first_of("\t\n", b);
+    return rg.substr(b, (e == std::string::npos ? rg.size() : e) - b);
+}
+
 bool is_count(const char *s) {
     if (!*s) return false;
     for (const char *p = s; *p; ++p) if (!isdigit((unsigned char) *p)) return false;
@@ -429,7 +458,8 @@ int main(int argc, char **argv) {
     // this program's own arguments first: `-p N` (worker count), --bam and --dump-opt are taken out of the list, walking it the way getopt will
     // (option arguments skipped, `--` ends the options), so that everything left is parsed as main_mem parses it
     int workers = 2; bool dump = false, dump_chunks = false, bam = false, sort = false, write_index = false, markdup = false;
-    long long sort_mem = 2LL << 30;
+    long long sort_mem = 2LL << 30, optical_distance = 100;
+    const char *metrics_path = nullptr; bool have_distance = false;
     std::vector<char *> av = { argv[0] };
     for (int i = 1; i < argc; ++i) {
         char *s = argv[i];
@@ -439,6 +469,16 @@ int main(int argc, char **argv) {
         if (!strcmp(s, "--sort")) { sort = bam = true; continue; }
         if (!strcmp(s, "--write-index")) { write_index = true; continue; }
         if (!strcmp(s, "--markdup")) { markdup = sort = bam = true; continue; }
+        if (!strcmp(s, "--markdup-metrics")) {
+            if (i + 1 >= argc || !*argv[i + 1]) { fprintf(stderr, "[E::bm2_mem] --markdup-metrics takes a file name\n"); return 1; }
+            metrics_path = argv[++i]; markdup = sort = bam = true; continue;
+        }
+        if (!strcmp(s, "--optical-distance")) {
+            if (i + 1 >= argc || !parse_distance(argv[i + 1], &optical_distance)) {
+                fprintf(stderr, "[E::bm2_mem] --optical-distance takes a decimal integer from 0 to 2147483647\n"); return 1;
+            }
+            have_distance = true; ++i; continue;
+        }
         if (!strcmp(s, "--sort-mem")) {
             if (i + 1 >= argc || !parse_size(argv[i + 1], &sort_mem)) {
                 fprintf(stderr, "[E::bm2_mem] --sort-mem takes a positive byte count with an optional K, M or G suffix\n"); return 1;
@@ -586,6 +626,7 @@ int main(int argc, char **argv) {
     }
     const int threads = opt.n_threads;
     if (workers > 4) workers = 4;
+    if (have_distance && !metrics_path) { fprintf(stderr, "[E::bm2_mem] --optical-distance needs --markdup-metrics FILE\n"); return 1; }
     if (write_index && (!sort || !out_path)) { fprintf(stderr, "[E::bm2_mem] --write-index needs --sort and -o FILE\n"); return 1; }
     const bool smart = (opt.flag & 0x400) != 0;
     const char *prefix = v[optind], *f1 = v[optind + 1], *f2 = optind + 2 < ac ? v[optind + 2] : nullptr;
@@ -658,6 +699,7 @@ int main(int argc, char **argv) {
                workers, f2 ? 2 : 1, bam ? "true" : "false");
         if (sort) printf("\"sort\": true, \"sort_mem\": %lld, \"write_index\": %s, ", sort_mem, write_index ? "true" : "false");
         if (markdup) printf("\"markdup\": true, ");
+        if (metrics_path) printf("\"markdup_metrics\": %s, \"optical_distance\": %lld, ", json_str(metrics_path).c_str(), optical_distance);
         printf("\"header\": %s}\n", json_str(header).c_str());
         bm2_index_free(idx);
         return 0;
@@ -729,6 +771,15 @@ int main(int argc, char **argv) {
             };
             sink.dup_set = [sort_ctx](const uint64_t *bits, int64_t n_bits) { return bm2_dup_set(sort_ctx, bits, n_bits); };
             sink.sig_bytes = sort_mem / 8;
+            if (metrics_path)
+                sink.dup_ex = [sort_ctx, optical_distance](const bm2_dup_loc_entry *e, int64_t n, int resolve, const bm2_dup_loc_entry **sorted,
+                                                           const int64_t **dups, int64_t *n_dups, int64_t *n_optical, double *device_s) {
+                    const int rc = bm2_dup_resolve_ex(sort_ctx, e, n, resolve, optical_distance, sorted, dups, n_dups, n_optical);
+                    double ms = 0;
+                    bm2_last_dup_stats(sort_ctx, nullptr, &ms);
+                    *device_s = ms / 1e3;
+                    return rc;
+                };
         }
         if (out_path) sink.tmp_prefix = std::string(out_path) + ".tmp.";
         else {
@@ -739,6 +790,7 @@ int main(int argc, char **argv) {
     Shared sh;
     sh.opt = &opt; sh.idx = idx; sh.cnames = cnames.data(); sh.paired = f2 != nullptr; sh.smart = smart; sh.threads = threads; sh.out = out;
     sh.pes0 = use_pes ? pes : nullptr; sh.copy_comment = copy_comment; sh.bam = bam; sh.sink = sort ? &sink : nullptr; sh.markdup = markdup;
+    sh.metrics = metrics_path != nullptr;
     sh.extra.rg_id = have_rg ? rg_id.c_str() : nullptr; sh.extra.contig_anno = canno.data(); sh.extra.ref_hdr = (opt.flag & 0x100) != 0;
     sh.t_loop = now_s();
     std::vector<std::thread> pool;
@@ -774,6 +826,23 @@ int main(int argc, char **argv) {
         fwrite(eof, 1, sizeof eof, out);
     }
     if (out != stdout) fclose(out);
+    if (metrics_path) {
+        fflush(stdout);                                               // after the BAM is complete; through a temporary name, so never partial
+        DupMetrics m;
+        const std::string lb = have_rg ? rg_library(rg_line) : std::string();
+        if (!lb.empty()) m.library = lb;
+        m.unpaired_reads = sink.dup_frag_entries; m.read_pairs = sink.dup_pair_entries;
+        m.secondary_or_supplementary = sh.n_sec_supp; m.unmapped = sh.n_unmapped;
+        m.unpaired_dups = sink.dup_frag_templates; m.pair_dups = sink.dup_pair_templates; m.optical_pairs = sink.dup_optical_pairs;
+        std::string args;
+        for (int i = 1; i < argc; ++i) args += std::string(i > 1 ? " " : "") + argv[i];
+        const std::string text = dup_metrics_text(m, args), path = metrics_path, tmp = path + ".tmp";
+        FILE *f = fopen(tmp.c_str(), "wb");
+        if (!f || fwrite(text.data(), 1, text.size(), f) != text.size() || fclose(f) || rename(tmp.c_str(), path.c_str())) {
+            unlink(tmp.c_str());
+            fprintf(stderr, "bm2_mem: cannot write %s\n", path.c_str()); return 2;
+        }
+    }
     fprintf(stderr, "{\"reads\": %lld, \"chunks\": %lld, \"workers\": %d, \"loop_s\": %.6f, \"index_and_context_s\": %.3f, \"fastq_encode_s\": %.6f, \"seed_chain_extend_s\": %.6f, "
                     "\"pestat_s\": %.6f, \"sam_stage_s\": %.6f, \"sam_format_s\": %.6f, \"wait_for_turn_s\": %.6f, \"write_s\": %.6f, \"chunk_s\": [",
             sh.n_processed, n_chunks, workers, loop_s, t_index, sh.t_enc, sh.t_aln, sh.t_pes, sh.t_sam, sh.t_fmt, sh.t_turn, sh.t_write);
@@ -793,6 +862,7 @@ int main(int argc, char **argv) {
                         "\"dup_sig_runs\": %lld, \"dup_sig_bytes\": %lld", sh.t_dup_sig + sink.markdup_s, (long long) sink.dup_templates,
                 (long long) sink.dup_pair_templates, (long long) sink.dup_frag_templates, (long long) sink.dup_records, (long long) sink.dup_sig_runs,
                 (long long) sink.dup_sig_bytes);
+    if (metrics_path) fprintf(stderr, ", \"dup_optical_pairs\": %lld", (long long) sink.dup_optical_pairs);
     fprintf(stderr, "}\n");
     if (sort_ctx) bm2_destroy(sort_ctx);
     for (int w = workers - 1; w >= 0; --w) bm2_destroy(ctxs[w]);

@@ -451,7 +451,8 @@ int  bm2_bam_sort_memory(const bm2_ctx *ctx, int64_t run_bytes, int64_t *needed,
 int  bm2_bam_sort_memory_ex(const bm2_ctx *ctx, int64_t run_bytes, int with_tids, int64_t *needed, int64_t *free_bytes);
 
 /* ---- Duplicate marking (bm2_mem --markdup) ------------------------------------------------------------------------------------------------
- * The rule (csrc/markdup_device.cuh) follows Picard MarkDuplicates's defaults, SUM_OF_BASE_QUALITIES and no optical duplicates; equality with
+ * The rule (csrc/markdup_device.cuh) follows Picard MarkDuplicates's defaults, SUM_OF_BASE_QUALITIES; optical duplicates are marked like any
+ * other duplicate, and counted only for the metrics (bm2_dup_resolve_ex, below); equality with
  * Picard or samtools is not claimed.  A template is a read, or both reads of a pair; its id (tid) is the 0-based input-order index of its
  * first read.  Its primaries (no 0x100 / 0x800) give its entries:
  *   end    (refID, unclipped 5' coordinate, reverse) packed as refID << 34 | (coord + 2^32) << 1 | reverse (refID < 2^30, |coord| < 2^32):
@@ -488,6 +489,27 @@ int  bm2_dup_set(bm2_ctx *ctx, const uint64_t *bits, int64_t n_bits);
  * no other byte changes.  Without tids, or with no bitset, the bytes are bm2_bam_sort_compress's. */
 int  bm2_bam_sort_compress_ex(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int64_t *starts, int64_t n_recs, const int64_t *tids,
                               const uint8_t *carry, int64_t carry_len, int last, bm2_sort_out *out, const int64_t **tids_out);
+
+/* ---- Duplication metrics and optical duplicates (bm2_mem --markdup-metrics) ------------------------------------------------------------
+ * The rule (csrc/markdup_device.cuh) follows Picard MarkDuplicates's defaults; byte equality with Picard is not claimed.
+ *   location  of a template: its first record's QNAME split on ':'.  Exactly 5 or 7 fields: tile, x, y are the last three, each parsed as
+ *             Picard's rapidParseInt (an optional '-', then the digits up to the first non-digit, as a wrapping 32-bit int; no digit: no
+ *             location).  Any other field count: no location.  The lane is not part of it.
+ *   class     of a pair template: the strand (0x10) of its primary with 0x40 (of its first primary when neither has 0x40)
+ *   optical   in a pair group of 2 .. 300000 members, two members are linked when both have a location, the same class and tile, and
+ *             |x1 - x2| <= d and |y1 - y2| <= d (in 64 bits); the group's optical count is the sum over the connected components of
+ *             size - 1, a member without a location being a component of its own.  Larger groups and fragment groups have none.
+ * loc: bit 0 set when the template has a location, bit 1 its class (1: reverse); tile, x, y are 0 without a location. */
+typedef struct { bm2_dup_entry e; int32_t tile, x, y, loc; } bm2_dup_loc_entry;
+/* bm2_dup_signatures, with the pair entries located.  counts[0] gets the chunk's records with 0x100 or 0x800, counts[1] its primary records
+ * with 0x4.  The entries are bm2_dup_signatures's (pairs[i].e), in the same order. */
+int  bm2_dup_signatures_ex(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int64_t *starts, int64_t n_recs, const int64_t *tmpl_first,
+                           const int64_t *tmpl_id, int64_t n_tmpl, const bm2_dup_loc_entry **pairs, int64_t *n_pairs, const bm2_dup_entry **frags,
+                           int64_t *n_frags, int64_t counts[2]);
+/* bm2_dup_resolve over located entries: the same order (*sorted: the located entries in it, when resolve == 0) and the same *dups.  With
+ * resolve != 0, *n_optical (may be NULL) gets the optical count summed over the pair groups at pixel distance `distance` (0 .. 2^31-1). */
+int  bm2_dup_resolve_ex(bm2_ctx *ctx, const bm2_dup_loc_entry *entries, int64_t n, int resolve, int64_t distance, const bm2_dup_loc_entry **sorted,
+                        const int64_t **dups, int64_t *n_dups, int64_t *n_optical);
 
 /* Staged mate rescue inside bm2_sam_pe (same records, other kernels): the windows mem_matesw (src/bwamem_pair.cpp:150-283) can ask for are
  * listed for all pairs of a wave from the regions before any rescue, aligned as one batch with one window per warp (the job shape of
