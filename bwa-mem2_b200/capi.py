@@ -211,6 +211,16 @@ DUP_LOC_ENTRY_DT = np.dtype([("k1", "<u8"), ("k2", "<u8"), ("tid", "<i8"), ("sco
                              ("y", "<i4"), ("loc", "<i4")])
 
 
+# bm2_bqsr_tables: the recalibration counts (include/bm2_b200.h)
+class BqsrTables(C.Structure):
+    _fields_ = [("qual_obs", C.c_void_p), ("qual_err", C.c_void_p), ("ctx_obs", C.c_void_p), ("ctx_err", C.c_void_p), ("cyc_obs", C.c_void_p),
+                ("cyc_err", C.c_void_p), ("reads", C.c_int64), ("bases", C.c_int64), ("ms", C.c_double), ("err_kind", C.c_int32),
+                ("err_index", C.c_int64), ("err_name", C.c_char_p), ("read_group", C.c_char_p)]
+
+
+BQSR_NQ, BQSR_NCTX, BQSR_NCYC = 94, 16, 1001
+
+
 class SortOut(C.Structure):
     _fields_ = [("z", C.c_void_p), ("z_len", C.c_int64), ("member_size", C.c_void_p), ("n_members", C.c_int64), ("carry", C.c_void_p),
                 ("carry_len", C.c_int64), ("recs", C.c_void_p), ("n_recs", C.c_int64)]
@@ -221,7 +231,8 @@ EXPORTS = ["bm2_create_sibling", "bm2_fastq_encode", "bm2_seq_encode", "bm2_fast
            "bm2_seed_chain_extend", "bm2_last_stage_ms", "bm2_gen_cigar", "bm2_pestat", "bm2_sam_pe", "bm2_sam_se", "bm2_ksw_align2",
            "bm2_fasta_pack", "bm2_index_build", "bm2_bam_format_ex", "bm2_bgzf_compress", "bm2_last_bgzf_stats",
            "bm2_bam_sort_compress", "bm2_last_sort_stats", "bm2_bam_sort_memory", "bm2_bam_sort_memory_ex", "bm2_bam_sort_compress_ex",
-           "bm2_dup_signatures", "bm2_dup_resolve", "bm2_last_dup_stats", "bm2_dup_set", "bm2_dup_signatures_ex", "bm2_dup_resolve_ex"]
+           "bm2_dup_signatures", "bm2_dup_resolve", "bm2_last_dup_stats", "bm2_dup_set", "bm2_dup_signatures_ex", "bm2_dup_resolve_ex",
+           "bm2_bqsr_sites", "bm2_bqsr_count", "bm2_bqsr_tables"]
 
 _lib = None
 
@@ -658,6 +669,39 @@ class Context:
         f = lib().bm2_dup_set
         f.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
         self._check(f(self._ctx, bits.ctypes.data, int(n_bits)), "bm2_dup_set")
+
+    def bqsr_sites(self, covered, junction, n_bits: int, holes, read_group: str):
+        """bm2_bqsr_sites: the known-site bitsets (uint64 words, n_bits = the index's l_pac), the .amb holes ([beg, end) pairs) and the read
+        group to this context (which must hold an index); zeroes the counts and arms counting."""
+        cov = np.ascontiguousarray(covered, np.uint64); jun = np.ascontiguousarray(junction, np.uint64)
+        h = np.ascontiguousarray(holes, np.int64).reshape(-1)
+        hb = h if len(h) else np.zeros(2, np.int64)
+        f = lib().bm2_bqsr_sites
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_char_p]
+        self._check(f(self._ctx, cov.ctypes.data, jun.ctypes.data, int(n_bits), hb.ctypes.data, len(h) // 2, read_group.encode()), "bm2_bqsr_sites")
+
+    def bqsr_count(self, data: bytes, starts):
+        """bm2_bqsr_count: counts the records of data (uncompressed BAM) starting at starts."""
+        starts = np.ascontiguousarray(starts, np.int64)
+        buf = np.frombuffer(data, np.uint8) if len(data) else np.zeros(1, np.uint8)
+        sb = starts if len(starts) else np.zeros(1, np.int64)
+        f = lib().bm2_bqsr_count
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64]
+        self._check(f(self._ctx, buf.ctypes.data, len(data), sb.ctypes.data, len(starts)), "bm2_bqsr_count")
+
+    def bqsr_tables(self):
+        """bm2_bqsr_tables -> dict(qual_obs/qual_err [94], ctx_obs/ctx_err [94, 16], cyc_obs/cyc_err [94, 1001] (cycle + 500), reads, bases,
+        ms, err_kind, err_index, err_name, read_group)."""
+        t = BqsrTables()
+        f = lib().bm2_bqsr_tables
+        f.argtypes = [C.c_void_p, C.c_void_p]
+        self._check(f(self._ctx, C.byref(t)), "bm2_bqsr_tables")
+        out = dict(reads=t.reads, bases=t.bases, ms=t.ms, err_kind=t.err_kind, err_index=t.err_index,
+                   err_name=(t.err_name or b"").decode(), read_group=(t.read_group or b"").decode())
+        for k, shape in (("qual", (BQSR_NQ,)), ("ctx", (BQSR_NQ, BQSR_NCTX)), ("cyc", (BQSR_NQ, BQSR_NCYC))):
+            for s in ("obs", "err"):
+                out[k + "_" + s] = _host(getattr(t, k + "_" + s), int(np.prod(shape)), np.int64).reshape(shape)
+        return out
 
     def set_sam_staged(self, on: int):
         """bm2_set_sam_staged: 1 / 2 = the rescue's local alignments as a batch (one window per warp / per thread) before the per-pair kernel, 0 = inside it."""

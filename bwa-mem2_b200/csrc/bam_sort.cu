@@ -11,7 +11,8 @@
 //               sorted device buffer; the unfinished last block goes back as the carry
 // bm2_bam_sort_compress_ex is the same code with one template id per record carried through the permutation; with a duplicate bitset on the
 // context (bm2_dup_set, markdup.cu) the key kernel sets 0x400 in the index data of the records of duplicate templates and the gather writes it
-// into the copied record.
+// into the copied record.  With counting armed (bm2_bqsr_sites, bqsr.cu), the sorted records are counted for the recalibration tables after
+// the gather, where they carry their duplicate flags, and before BGZF.
 #include "bm2_common.cuh"
 #include "bm2_ctx.h"
 #include "bam_sort_device.cuh"
@@ -187,6 +188,7 @@ static int sort_compress(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int
                                                                                mark ? (const bm2_sort_rec *) b[SD_SINFO].p : nullptr);
         BM2_CUDA_OK(cudaGetLastError());
         BM2_CUDA_OK(cudaEventRecord(ctx->sort_ev[3], st));
+        if (ctx->bqsr_armed && bqsr_count_device(ctx, (const uint8_t *) b[SD_OUT].p + carry_len, (const int64_t *) b[SD_OFFS].p, nr, st)) return 1;
         BM2_CUDA_OK(cudaMemcpyAsync(h_offs, b[SD_OFFS].p, (size_t) (nr + 1) * 8, cudaMemcpyDeviceToHost, st));
         BM2_CUDA_OK(cudaMemcpyAsync(h_info, b[SD_SINFO].p, (size_t) nr * sizeof(bm2_sort_rec), cudaMemcpyDeviceToHost, st));
         if (tids) BM2_CUDA_OK(cudaMemcpyAsync(ctx->sort_tids.data(), d_stids, (size_t) nr * 8, cudaMemcpyDeviceToHost, st));
@@ -194,6 +196,7 @@ static int sort_compress(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int
         float ms[3] = { 0, 0, 0 };
         for (int k = 0; k < 3; ++k) BM2_CUDA_OK(cudaEventElapsedTime(&ms[k], ctx->sort_ev[k], ctx->sort_ev[k + 1]));
         for (int k = 0; k < 3; ++k) ctx->sort_ms[k] = ms[k];
+        if (ctx->bqsr_armed && bqsr_count_done(ctx, (const uint8_t *) b[SD_OUT].p + carry_len, h_offs, nr)) return 1;
     } else h_offs[0] = 0;
     const int64_t total = h_offs[nr];
     std::vector<int64_t> cut;

@@ -28,6 +28,10 @@
 //           spilled as such), resolved by the located call, which also returns the optical count of the call's pair groups.  A group never
 //           straddles a window, so the sum over the windows is exact.
 //
+//   recal   (--recal-file) before_final arms the sort context's covariate counting (bm2_bqsr_sites) after the duplicates are resolved, so
+//           that only the final pass (the one-run sort, or the merge windows) counts, with the records' final flags; the runs spilled
+//           before are never counted.
+//
 // The device calls are parameters, so that tests/host_emul/bam_sort_emul.cpp and markdup_emul.cpp run all of this with the GPU swapped for a
 // CPU restatement.
 #pragma once
@@ -155,6 +159,7 @@ struct BamSortSink {
     SortCallEx sort_ex;                          // when set, used instead of sort
     DupCall dup; DupSetCall dup_set;             // --markdup when dup is set (sort_ex must be set then)
     DupCallEx dup_ex;                            // --markdup-metrics: the pair space through this one, with add_sigs_ex
+    std::function<void()> before_final;          // --recal-file: called once the duplicates are known, before the one-run sort or the merge
     int64_t run_bytes = (int64_t) 2 << 30;
     int64_t sig_bytes = (int64_t) 256 << 20;     // entries held on the host (--sort-mem / 8)
     int64_t n_reads = 0;                         // the duplicate bitset's bits: set before finish
@@ -324,6 +329,7 @@ struct BamSortSink {
         const bool one_run = runs.empty();
         if (!one_run && !cur_starts.empty()) { hand_off(); sorter.join(); }
         if (dup) resolve();
+        if (before_final) before_final();
         if (one_run) {
             w.write(cur.data(), (int64_t) cur.size(), cur_starts.data(), (int64_t) cur_starts.size(), dup ? cur_tids.data() : nullptr, true);
             sort_s += w.device_s;

@@ -94,13 +94,24 @@ struct bm2_ctx {
     std::vector<bm2_dup_entry> dup_pairs, dup_frags, dup_sorted;
     std::vector<bm2_dup_loc_entry> dup_lpairs, dup_lsorted;   // the _ex calls' located pair entries and sorted entries
     std::vector<int64_t> dup_ids;
+    // bm2_bqsr_sites / bm2_bqsr_count / bm2_bqsr_tables (bqsr.cu): buffers, whether bm2_bam_sort_compress_ex counts, events, the device time,
+    // the records seen since the sites came, the first read error (kind 0: none), the read group, the last tables
+    DevBuf bqsr_d[7];
+    bool bqsr_armed = false;
+    cudaEvent_t bqsr_ev[2] = {nullptr, nullptr};
+    double bqsr_ms = 0;
+    int64_t bqsr_n_holes = 0, bqsr_seen = 0, bqsr_err_index = -1;
+    uint64_t bqsr_err_word = ~(uint64_t) 0;
+    int bqsr_err_kind = 0;
+    std::string bqsr_rg, bqsr_err_name;
+    std::vector<int64_t> bqsr_tables;
 
     int ensure(DevBuf &b, size_t bytes);
     int ensure_host(HostBuf &b, size_t bytes);
     std::vector<DevBuf *> all_dev() {
         std::vector<DevBuf *> v = {&io_pairs, &io_ref, &io_qer, &bsw_jobs, &bsw_outs, &bsw_scratch, &dup_bits};
         append(v, pipe_d); append(v, cigar_d); append(v, sam_d); append(v, ksw_d); append(v, fq_d);
-        append(v, bgzf_d); append(v, sort_d); append(v, dup_d);
+        append(v, bgzf_d); append(v, sort_d); append(v, dup_d); append(v, bqsr_d);
         return v;
     }
     std::vector<HostBuf *> all_host() {
@@ -114,3 +125,7 @@ struct bm2_ctx {
 // bgzf.cu: the members of the nb blocks [starts[b], starts[b+1]) of the device bytes d_in, on ctx's stream (the body of bm2_bgzf_compress),
 // gathered into *gather (nullptr: the context's own buffer) before they are copied to the host
 int bgzf_compress_device(bm2_ctx *ctx, const uint8_t *d_in, const int64_t *starts, int64_t nb, const uint8_t **out, int64_t *out_len, DevBuf *gather);
+// bqsr.cu: the covariate counts of the n records at d_base + d_starts[i] (device), enqueued on st; then, once st has finished,
+// bqsr_count_done adds the device time and returns 1 (the context's error set, naming the read) when one of these records is a read error
+int bqsr_count_device(bm2_ctx *ctx, const uint8_t *d_base, const int64_t *d_starts, int64_t n, cudaStream_t st);
+int bqsr_count_done(bm2_ctx *ctx, const uint8_t *d_base, const int64_t *h_starts, int64_t n);

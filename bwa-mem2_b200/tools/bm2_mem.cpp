@@ -25,6 +25,9 @@
 //                                    0x400 in the same sort, which then carries each record's template id (bam_sort.h, markdup_device.cuh)
 //        or bm2_dup_signatures_ex    --markdup-metrics: the same with located pair entries and the chunk's record counts, resolved by
 //                                    bm2_dup_resolve_ex with the optical pass; Picard's metrics file at the end (markdup_metrics.h)
+//        and bm2_bqsr_sites             --recal-file: the --known-sites VCFs, read on a thread of their own while the reads align (known_sites.h),
+//                                    go to the sort context before the final sort pass, which then counts the covariates of the sorted
+//                                    records on the GPU (bqsr_device.cuh); GATK's recalibration report at the end (bqsr_report.h)
 // Chunks in flight: the reference's kt_pipeline runs its three steps (read, process, write) on two worker threads so that one chunk's I/O
 // overlaps another's computation (src/fastmap.cpp:952-1003, src/kthread.cpp:122-176).  Here -p workers (default 2) each own a context
 // (bm2_create_sibling: one index in HBM) and take whole chunks off a queue; the GPU interleaves the kernels of the two chunks, the host side of
@@ -40,6 +43,8 @@
 #include "../csrc/read_input.h"
 #include "../csrc/bam_sort.h"
 #include "../csrc/markdup_metrics.h"
+#include "../csrc/bqsr_report.h"
+#include "../csrc/known_sites.h"
 #include <algorithm>
 #include <chrono>
 #include <condition_variable>
@@ -346,6 +351,9 @@ void usage(const bm2_mem_opt_t &o) {
 "  --markdup-metrics FILE  write Picard's duplication metrics for the one library (-R's LB, else Unknown Library) to FILE, with optical\n"
 "              duplicates counted on the GPU from Illumina read names (implies --markdup)\n"
 "  --optical-distance N  the largest pixel distance of two optical duplicates, 0 to 2147483647 (needs --markdup-metrics) [100]\n"
+"  --recal-file FILE  write GATK BaseRecalibrator's recalibration table (GATKReport, substitution covariates at GATK 4's defaults) of the\n"
+"              marked BAM to FILE, with the covariates counted on the GPU (implies --markdup; needs -R and --known-sites)\n"
+"  --known-sites VCF  known variant sites skipped by --recal-file, plain, gzip or BGZF; may be given more than once\n"
 "  --dump-opt  print the parsed options, the -I values, the read group and the header as JSON, and exit before any GPU work\n"
 "  --dump-chunks  print the chunks the input is cut into (first read, byte ranges, whether bm2_fastq_encode takes them) as JSON lines,\n"
 "              and exit without loading the index\n",
@@ -460,6 +468,7 @@ int main(int argc, char **argv) {
     int workers = 2; bool dump = false, dump_chunks = false, bam = false, sort = false, write_index = false, markdup = false;
     long long sort_mem = 2LL << 30, optical_distance = 100;
     const char *metrics_path = nullptr; bool have_distance = false;
+    const char *recal_path = nullptr; std::vector<std::string> known_paths;
     std::vector<char *> av = { argv[0] };
     for (int i = 1; i < argc; ++i) {
         char *s = argv[i];
@@ -472,6 +481,14 @@ int main(int argc, char **argv) {
         if (!strcmp(s, "--markdup-metrics")) {
             if (i + 1 >= argc || !*argv[i + 1]) { fprintf(stderr, "[E::bm2_mem] --markdup-metrics takes a file name\n"); return 1; }
             metrics_path = argv[++i]; markdup = sort = bam = true; continue;
+        }
+        if (!strcmp(s, "--recal-file")) {
+            if (i + 1 >= argc || !*argv[i + 1]) { fprintf(stderr, "[E::bm2_mem] --recal-file takes a file name\n"); return 1; }
+            recal_path = argv[++i]; markdup = sort = bam = true; continue;
+        }
+        if (!strcmp(s, "--known-sites")) {
+            if (i + 1 >= argc || !*argv[i + 1]) { fprintf(stderr, "[E::bm2_mem] --known-sites takes a VCF file name\n"); return 1; }
+            known_paths.push_back(argv[++i]); continue;
         }
         if (!strcmp(s, "--optical-distance")) {
             if (i + 1 >= argc || !parse_distance(argv[i + 1], &optical_distance)) {
@@ -627,6 +644,9 @@ int main(int argc, char **argv) {
     const int threads = opt.n_threads;
     if (workers > 4) workers = 4;
     if (have_distance && !metrics_path) { fprintf(stderr, "[E::bm2_mem] --optical-distance needs --markdup-metrics FILE\n"); return 1; }
+    if (!known_paths.empty() && !recal_path) { fprintf(stderr, "[E::bm2_mem] --known-sites needs --recal-file FILE\n"); return 1; }
+    if (recal_path && known_paths.empty()) { fprintf(stderr, "[E::bm2_mem] --recal-file needs at least one --known-sites VCF\n"); return 1; }
+    if (recal_path && !have_rg) { fprintf(stderr, "[E::bm2_mem] --recal-file needs a read group (-R)\n"); return 1; }
     if (write_index && (!sort || !out_path)) { fprintf(stderr, "[E::bm2_mem] --write-index needs --sort and -o FILE\n"); return 1; }
     const bool smart = (opt.flag & 0x400) != 0;
     const char *prefix = v[optind], *f1 = v[optind + 1], *f2 = optind + 2 < ac ? v[optind + 2] : nullptr;
@@ -650,7 +670,7 @@ int main(int argc, char **argv) {
     if (ignore_alt) memset((void *) idx->ann_is_alt, 0, (size_t) idx->n_seqs * sizeof(int32_t));
     // contig names and annotations: <prefix>.ann (src/bntseq.cpp:106-177): "l_pac n_seqs seed", then per contig "gi name[ anno]" and
     // "offset len n_ambs"; the annotation is the rest of the name line without its first character, "(null)" meaning none
-    std::vector<std::string> names, annos; std::vector<long long> lens;
+    std::vector<std::string> names, annos; std::vector<long long> lens; std::vector<int64_t> offs;
     {
         FILE *f = fopen((std::string(prefix) + ".ann").c_str(), "r");
         if (!f) { fprintf(stderr, "bm2_mem: cannot open %s.ann\n", prefix); return 2; }
@@ -663,7 +683,7 @@ int main(int argc, char **argv) {
             if (!rest.empty() && rest.back() == '\n') rest.pop_back();
             annos.push_back(rest.size() > 1 && rest != " (null)" ? rest.substr(1) : std::string());
             if (!fgets(line.data(), (int) line.size(), f) || sscanf(line.data(), "%lld %lld %d", &off, &len, &amb) != 3) return 2;
-            names.push_back(nm); lens.push_back(len);
+            names.push_back(nm); lens.push_back(len); offs.push_back(off);
         }
         fclose(f);
     }
@@ -700,6 +720,11 @@ int main(int argc, char **argv) {
         if (sort) printf("\"sort\": true, \"sort_mem\": %lld, \"write_index\": %s, ", sort_mem, write_index ? "true" : "false");
         if (markdup) printf("\"markdup\": true, ");
         if (metrics_path) printf("\"markdup_metrics\": %s, \"optical_distance\": %lld, ", json_str(metrics_path).c_str(), optical_distance);
+        if (recal_path) {
+            printf("\"recal_file\": %s, \"known_sites\": [", json_str(recal_path).c_str());
+            for (size_t k = 0; k < known_paths.size(); ++k) printf("%s%s", k ? ", " : "", json_str(known_paths[k]).c_str());
+            printf("], ");
+        }
         printf("\"header\": %s}\n", json_str(header).c_str());
         bm2_index_free(idx);
         return 0;
@@ -710,6 +735,10 @@ int main(int argc, char **argv) {
     if (write_index)                                                  // BAI's bins reach 2^29 (SAMv1 §5.3); longer contigs need CSI
         for (size_t i = 0; i < names.size(); ++i)
             if (lens[i] > (1LL << 29) - 1) { fprintf(stderr, "[E::bm2_mem] contig %s is %lld bp long: BAI cannot index a contig longer than 2^29-1\n", names[i].c_str(), lens[i]); return 1; }
+    // --known-sites: the VCFs are read on a thread of their own while the reads align; an error in them ends the program as soon as it is found
+    KnownSites known;
+    double known_s = 0;
+    std::thread known_thread;                                         // started with the workers, joined before the final sort pass
     std::vector<const char *> cnames, canno;
     for (size_t i = 0; i < names.size(); ++i) { cnames.push_back(names[i].c_str()); canno.push_back(annos[i].c_str()); }
     std::vector<bm2_ctx *> ctxs((size_t) workers, nullptr);
@@ -723,6 +752,13 @@ int main(int argc, char **argv) {
         if (bm2_bam_sort_memory_ex(sort_ctx, sort_mem, markdup ? 1 : 0, &need, &avail)) die("bm2_bam_sort_memory", sort_ctx);
         if (need > avail) {
             fprintf(stderr, "[E::bm2_mem] --sort-mem %lld: one run sort needs %lld bytes of device memory, %lld bytes free\n", sort_mem, (long long) need, (long long) avail);
+            return 3;
+        }
+        // --recal-file: the two known-site bitsets (2 bits per reference base) and the counters (1.5 MB) on the sort context too
+        const int64_t sites = recal_path ? 2 * ((idx->l_pac + 63) / 64) * 8 + (2 << 20) : 0;
+        if (sites && need + sites > avail) {
+            fprintf(stderr, "[E::bm2_mem] --recal-file: the run sort and the known-site bitsets need %lld bytes of device memory, %lld bytes free\n",
+                    (long long) (need + sites), (long long) avail);
             return 3;
         }
     }
@@ -750,9 +786,13 @@ int main(int argc, char **argv) {
     BamSortSink sink;
     if (sort) {
         // without --markdup no template ids are passed, and bm2_bam_sort_compress_ex is bm2_bam_sort_compress
-        sink.sort_ex = [sort_ctx](const uint8_t *r, int64_t n, const int64_t *st, int64_t nr, const int64_t *tids, const uint8_t *c, int64_t cl, int last,
+        sink.sort_ex = [sort_ctx, recal_path](const uint8_t *r, int64_t n, const int64_t *st, int64_t nr, const int64_t *tids, const uint8_t *c, int64_t cl, int last,
                                   bm2_sort_out *o, const int64_t **tids_out, double *device_s) {
             const int rc = bm2_bam_sort_compress_ex(sort_ctx, r, n, st, nr, tids, c, cl, last, o, tids_out);
+            bm2_bqsr_tables_t bt;
+            if (rc && recal_path && !bm2_bqsr_tables(sort_ctx, &bt) && bt.err_kind) {       // a read --recal-file cannot count
+                fprintf(stderr, "[E::bm2_mem] --recal-file: %s\n", bm2_last_error(sort_ctx)); fflush(stderr); _Exit(1);
+            }
             double ms[4] = { 0, 0, 0, 0 };
             bm2_last_sort_stats(sort_ctx, ms);
             *device_s = (ms[0] + ms[1] + ms[2] + ms[3]) / 1e3;
@@ -781,6 +821,22 @@ int main(int argc, char **argv) {
                     return rc;
                 };
         }
+        if (recal_path)
+            sink.before_final = [&] {
+                known_thread.join();
+                std::vector<int64_t> holes;                               // <prefix>.amb: "l_pac n_seqs n_holes", then "offset len char" per hole
+                FILE *f = fopen((std::string(prefix) + ".amb").c_str(), "r");
+                long long a, b, nh = 0; char ch;
+                if (!f || fscanf(f, "%lld %lld %lld", &a, &b, &nh) != 3) die("--recal-file: cannot read the index's .amb file", nullptr);
+                for (long long k = 0; k < nh; ++k) {
+                    if (fscanf(f, "%lld %lld %c", &a, &b, &ch) != 3) die("--recal-file: cannot read the index's .amb file", nullptr);
+                    holes.push_back(a); holes.push_back(a + b);
+                }
+                fclose(f);
+                const std::string rg = bqsr_read_group(rg_line);
+                if (bm2_bqsr_sites(sort_ctx, known.covered.data(), known.junction.data(), idx->l_pac, holes.data(), (int64_t) holes.size() / 2, rg.c_str()))
+                    die("bm2_bqsr_sites", sort_ctx);
+            };
         if (out_path) sink.tmp_prefix = std::string(out_path) + ".tmp.";
         else {
             const char *td = getenv("TMPDIR");
@@ -792,6 +848,15 @@ int main(int argc, char **argv) {
     sh.pes0 = use_pes ? pes : nullptr; sh.copy_comment = copy_comment; sh.bam = bam; sh.sink = sort ? &sink : nullptr; sh.markdup = markdup;
     sh.metrics = metrics_path != nullptr;
     sh.extra.rg_id = have_rg ? rg_id.c_str() : nullptr; sh.extra.contig_anno = canno.data(); sh.extra.ref_hdr = (opt.flag & 0x100) != 0;
+    if (recal_path) {
+        std::vector<int64_t> lens64(lens.begin(), lens.end());
+        known_thread = std::thread([&known, &known_s, &known_paths, &names, &offs, lens64, l_pac = idx->l_pac] {
+            const double t0 = now_s();
+            const std::string err = read_known_sites(known_paths, names, offs, lens64, l_pac, known);
+            if (!err.empty()) { fprintf(stderr, "[E::bm2_mem] --known-sites: %s\n", err.c_str()); fflush(stderr); _Exit(1); }
+            known_s = now_s() - t0;
+        });
+    }
     sh.t_loop = now_s();
     std::vector<std::thread> pool;
     for (int w = 0; w < workers; ++w) pool.emplace_back(worker, &sh, ctxs[w]);
@@ -843,6 +908,18 @@ int main(int argc, char **argv) {
             fprintf(stderr, "bm2_mem: cannot write %s\n", path.c_str()); return 2;
         }
     }
+    bm2_bqsr_tables_t bt; memset(&bt, 0, sizeof bt);
+    if (recal_path) {
+        fflush(stdout);                                               // after the BAM is complete; through a temporary name, so never partial
+        if (bm2_bqsr_tables(sort_ctx, &bt)) die("bm2_bqsr_tables", sort_ctx);
+        const std::string text = bqsr_report_text(bt.read_group, bt.qual_obs, bt.qual_err, bt.ctx_obs, bt.ctx_err, bt.cyc_obs, bt.cyc_err),
+                          path = recal_path, tmp = path + ".tmp";
+        FILE *f = fopen(tmp.c_str(), "wb");
+        if (!f || fwrite(text.data(), 1, text.size(), f) != text.size() || fclose(f) || rename(tmp.c_str(), path.c_str())) {
+            unlink(tmp.c_str());
+            fprintf(stderr, "bm2_mem: cannot write %s\n", path.c_str()); return 2;
+        }
+    }
     fprintf(stderr, "{\"reads\": %lld, \"chunks\": %lld, \"workers\": %d, \"loop_s\": %.6f, \"index_and_context_s\": %.3f, \"fastq_encode_s\": %.6f, \"seed_chain_extend_s\": %.6f, "
                     "\"pestat_s\": %.6f, \"sam_stage_s\": %.6f, \"sam_format_s\": %.6f, \"wait_for_turn_s\": %.6f, \"write_s\": %.6f, \"chunk_s\": [",
             sh.n_processed, n_chunks, workers, loop_s, t_index, sh.t_enc, sh.t_aln, sh.t_pes, sh.t_sam, sh.t_fmt, sh.t_turn, sh.t_write);
@@ -863,6 +940,9 @@ int main(int argc, char **argv) {
                 (long long) sink.dup_pair_templates, (long long) sink.dup_frag_templates, (long long) sink.dup_records, (long long) sink.dup_sig_runs,
                 (long long) sink.dup_sig_bytes);
     if (metrics_path) fprintf(stderr, ", \"dup_optical_pairs\": %lld", (long long) sink.dup_optical_pairs);
+    if (recal_path)
+        fprintf(stderr, ", \"bqsr_s\": %.6f, \"bqsr_reads\": %lld, \"bqsr_bases\": %lld, \"known_sites\": %lld, \"known_sites_s\": %.6f", bt.ms / 1e3,
+                (long long) bt.reads, (long long) bt.bases, (long long) known.records, known_s);
     fprintf(stderr, "}\n");
     if (sort_ctx) bm2_destroy(sort_ctx);
     for (int w = workers - 1; w >= 0; --w) bm2_destroy(ctxs[w]);

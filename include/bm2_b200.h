@@ -511,6 +511,37 @@ int  bm2_dup_signatures_ex(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const i
 int  bm2_dup_resolve_ex(bm2_ctx *ctx, const bm2_dup_loc_entry *entries, int64_t n, int resolve, int64_t distance, const bm2_dup_loc_entry **sorted,
                         const int64_t **dups, int64_t *n_dups, int64_t *n_optical);
 
+/* ---- Base quality recalibration tables (bm2_mem --recal-file) ---------------------------------------------------------------------------
+ * The rule (csrc/bqsr_device.cuh) restates GATK 4 BaseRecalibrator at its defaults, substitution table only; byte equality with GATK is not
+ * claimed.  Counted: records without 0x4 / 0x100 / 0x800 / 0x400 / 0x200, MAPQ not 0 or 255, after adaptor clipping and soft clips are
+ * removed, with at least one base left.  A base is skipped when it is N, its quality is below 6, or it is a known-site base; an aligned base
+ * is an error when it differs from the reference (N inside an .amb hole).  Keys: quality, context (two letters in sequencing order, the
+ * low-quality tails written as N) and cycle (+-1..500, negative for the second of a pair). */
+typedef struct bm2_bqsr_tables_t {
+    const int64_t *qual_obs, *qual_err;   /* [94]: quality (the sum of the cycle table over the cycles)                        */
+    const int64_t *ctx_obs, *ctx_err;     /* [94 * 16]: quality * 16 + context, context 4 * first + second letter, ACGT = 0..3   */
+    const int64_t *cyc_obs, *cyc_err;     /* [94 * 1001]: quality * 1001 + cycle + 500                                          */
+    int64_t reads, bases;                 /* records and bases counted                                                          */
+    double ms;                            /* device time of the counting kernels (CUDA events)                                  */
+    int32_t err_kind;                     /* the first read error: 0 none, 1 no qualities, 2 over 500 cycles after clipping,   */
+    int64_t err_index;                    /*   3 a quality above 93; its record's index over all records seen since the sites   */
+    const char *err_name;                 /*   and its read name                                                                */
+    const char *read_group;               /* the read group covariate given to bm2_bqsr_sites                                   */
+} bm2_bqsr_tables_t;
+/* The known sites over the context's index: covered and junction (n_bits == l_pac bits each over the forward strand's concatenated
+ * contigs; word w holds bits 64w..64w+63) - covered bit p: a VCF record covers p; junction bit p: one record covers both p and p + 1 -, the
+ * .amb holes as n_holes sorted [beg, end) pairs, and the read group covariate.  Zeroes the counts and arms counting: from then on
+ * bm2_bam_sort_compress_ex also counts the records it sorts, after the gather (with their duplicate flags) and before BGZF; a record that is
+ * a read error then makes that call fail with an error naming the read.  Bitsets larger than the free device memory are an error that gives
+ * both numbers. */
+int  bm2_bqsr_sites(bm2_ctx *ctx, const uint64_t *covered, const uint64_t *junction, int64_t n_bits, const int64_t *holes, int64_t n_holes,
+                    const char *rg);
+/* Counts the records of recs (uncompressed BAM records at starts) into the context's tables (after bm2_bqsr_sites).  A read error is not
+ * counted and is reported by bm2_bqsr_tables. */
+int  bm2_bqsr_count(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int64_t *starts, int64_t n_recs);
+/* The counts since bm2_bqsr_sites (HOST arrays owned by the context, valid until its next call). */
+int  bm2_bqsr_tables(bm2_ctx *ctx, bm2_bqsr_tables_t *out);
+
 /* Staged mate rescue inside bm2_sam_pe (same records, other kernels): the windows mem_matesw (src/bwamem_pair.cpp:150-283) can ask for are
  * listed for all pairs of a wave from the regions before any rescue, aligned as one batch with one window per warp (the job shape of
  * bm2_ksw_align2; the reference batches the same alignments across pairs in its kswv path, src/bwamem_pair.cpp:930-1248, src/kswv.cpp),
