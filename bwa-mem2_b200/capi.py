@@ -221,6 +221,17 @@ class BqsrTables(C.Structure):
 BQSR_NQ, BQSR_NCTX, BQSR_NCYC = 94, 16, 1001
 
 
+# bm2_bqsr_apply_set / bm2_last_bqsr_apply_stats (include/bm2_b200.h)
+class BqsrApplyTables(C.Structure):
+    _fields_ = [("n_rg", C.c_int32), ("P", C.c_void_p), ("ctx", C.c_void_p), ("cyc", C.c_void_p), ("n_ids", C.c_int32), ("ids", C.c_void_p),
+                ("id_table", C.c_void_p)]
+
+
+class BqsrApplyStats(C.Structure):
+    _fields_ = [("apply_ms", C.c_double), ("bgzf_ms", C.c_double), ("bases_changed", C.c_int64), ("recal_records", C.c_int64),
+                ("kept_records", C.c_int64), ("err_kind", C.c_int32), ("err_index", C.c_int64), ("err_name", C.c_char_p)]
+
+
 class SortOut(C.Structure):
     _fields_ = [("z", C.c_void_p), ("z_len", C.c_int64), ("member_size", C.c_void_p), ("n_members", C.c_int64), ("carry", C.c_void_p),
                 ("carry_len", C.c_int64), ("recs", C.c_void_p), ("n_recs", C.c_int64)]
@@ -232,7 +243,8 @@ EXPORTS = ["bm2_create_sibling", "bm2_fastq_encode", "bm2_seq_encode", "bm2_fast
            "bm2_fasta_pack", "bm2_index_build", "bm2_bam_format_ex", "bm2_bgzf_compress", "bm2_last_bgzf_stats",
            "bm2_bam_sort_compress", "bm2_last_sort_stats", "bm2_bam_sort_memory", "bm2_bam_sort_memory_ex", "bm2_bam_sort_compress_ex",
            "bm2_dup_signatures", "bm2_dup_resolve", "bm2_last_dup_stats", "bm2_dup_set", "bm2_dup_signatures_ex", "bm2_dup_resolve_ex",
-           "bm2_bqsr_sites", "bm2_bqsr_count", "bm2_bqsr_tables"]
+           "bm2_bqsr_sites", "bm2_bqsr_count", "bm2_bqsr_tables", "bm2_bqsr_apply_set", "bm2_bqsr_apply", "bm2_last_bqsr_apply_stats",
+           "bm2_bqsr_apply_memory"]
 
 _lib = None
 
@@ -701,6 +713,47 @@ class Context:
         for k, shape in (("qual", (BQSR_NQ,)), ("ctx", (BQSR_NQ, BQSR_NCTX)), ("cyc", (BQSR_NQ, BQSR_NCYC))):
             for s in ("obs", "err"):
                 out[k + "_" + s] = _host(getattr(t, k + "_" + s), int(np.prod(shape)), np.int64).reshape(shape)
+        return out
+
+    def bqsr_apply_set(self, P, ctx, cyc, ids, id_table):
+        """bm2_bqsr_apply_set: the dense tables (float64 [n_rg, 94], [n_rg, 94, 16], [n_rg, 94, 1001]) and the header's @RG IDs with each
+        one's table index (-1: none)."""
+        self._apply_keep = [np.ascontiguousarray(P, np.float64).reshape(-1), np.ascontiguousarray(ctx, np.float64).reshape(-1),
+                            np.ascontiguousarray(cyc, np.float64).reshape(-1), np.ascontiguousarray(id_table, np.int32)]
+        p, c, y, tb = self._apply_keep
+        names = (C.c_char_p * max(len(ids), 1))(*[i.encode() for i in ids])
+        t = BqsrApplyTables(len(p) // BQSR_NQ, p.ctypes.data if len(p) else None, c.ctypes.data if len(c) else None, y.ctypes.data if len(y) else None,
+                            len(ids), C.cast(names, C.c_void_p) if ids else None, tb.ctypes.data if len(tb) else None)
+        f = lib().bm2_bqsr_apply_set
+        f.argtypes = [C.c_void_p, C.c_void_p]
+        self._check(f(self._ctx, C.byref(t)), "bm2_bqsr_apply_set")
+
+    def bqsr_apply(self, data: bytes, starts, carry: bytes = b"", last: bool = True):
+        """bm2_bqsr_apply: the contiguous records of data recalibrated and compressed after carry -> bam_sort_compress's dict (z, member_size,
+        carry, recs in input order)."""
+        starts = np.ascontiguousarray(starts, np.int64)
+        buf = np.frombuffer(data, np.uint8) if len(data) else np.zeros(1, np.uint8)
+        sb = starts if len(starts) else np.zeros(1, np.int64)
+        cb = np.frombuffer(carry, np.uint8) if len(carry) else np.zeros(1, np.uint8)
+        o = SortOut()
+        f = lib().bm2_bqsr_apply
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int, C.c_void_p]
+        self._check(f(self._ctx, buf.ctypes.data, len(data), sb.ctypes.data, len(starts), cb.ctypes.data, len(carry), int(last), C.byref(o)),
+                    "bm2_bqsr_apply")
+        recs = np.ctypeslib.as_array(C.cast(o.recs, C.POINTER(C.c_uint8)), shape=(o.n_recs * SORT_REC_DT.itemsize,)).view(SORT_REC_DT).copy() \
+            if o.n_recs else np.zeros(0, SORT_REC_DT)
+        sizes = _host(o.member_size, o.n_members, np.int32) if o.n_members else np.zeros(0, np.int32)
+        return dict(z=C.string_at(o.z, o.z_len) if o.z_len else b"", member_size=sizes, carry=C.string_at(o.carry, o.carry_len) if o.carry_len else b"",
+                    recs=recs)
+
+    def bqsr_apply_stats(self):
+        """bm2_last_bqsr_apply_stats -> dict(apply_ms, bgzf_ms, bases_changed, recal_records, kept_records, err_kind, err_index, err_name)."""
+        s = BqsrApplyStats()
+        f = lib().bm2_last_bqsr_apply_stats
+        f.argtypes = [C.c_void_p, C.c_void_p]
+        self._check(f(self._ctx, C.byref(s)), "bm2_last_bqsr_apply_stats")
+        out = {k: getattr(s, k) for k, _ in s._fields_}
+        out["err_name"] = (s.err_name or b"").decode()
         return out
 
     def set_sam_staged(self, on: int):

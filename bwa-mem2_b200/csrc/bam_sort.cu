@@ -8,7 +8,7 @@
 //   scan        the lengths in sorted order, an exclusive scan: each record's place after the carry
 //   gather      one warp per record, 16-byte copies when source and destination agree modulo 16
 //   BGZF        the blocks are cut on the host (bam_sort_layout) from the scan, and bm2_bgzf_compress's kernels compress them straight from the
-//               sorted device buffer; the unfinished last block goes back as the carry
+//               sorted device buffer; the unfinished last block goes back as the carry (bam_compress_stream, which bm2_bqsr_apply shares)
 // bm2_bam_sort_compress_ex is the same code with one template id per record carried through the permutation; with a duplicate bitset on the
 // context (bm2_dup_set, markdup.cu) the key kernel sets 0x400 in the index data of the records of duplicate templates and the gather writes it
 // into the copied record.  With counting armed (bm2_bqsr_sites, bqsr.cu), the sorted records are counted for the recalibration tables after
@@ -198,22 +198,29 @@ static int sort_compress(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int
         for (int k = 0; k < 3; ++k) ctx->sort_ms[k] = ms[k];
         if (ctx->bqsr_armed && bqsr_count_done(ctx, (const uint8_t *) b[SD_OUT].p + carry_len, h_offs, nr)) return 1;
     } else h_offs[0] = 0;
-    const int64_t total = h_offs[nr];
+    // the members: the sorted buffer is free after the gather, so the compressed bytes are gathered into the records' input buffer
+    if (bam_compress_stream(ctx, (const uint8_t *) b[SD_OUT].p, carry_len, h_offs, nr, h_offs[nr], last, h_info, &b[SD_IN], ctx->sort_carry,
+                            ctx->sort_recs, out)) return 1;
+    ctx->sort_ms[3] = ctx->bgzf_ms;
+    return 0;
+}
+
+int bam_compress_stream(bm2_ctx *ctx, const uint8_t *d_stream, int64_t carry_len, const int64_t *offs, int64_t n_recs, int64_t total, int last,
+                        bm2_sort_rec *recs, DevBuf *gather, std::vector<uint8_t> &carry_v, std::vector<bm2_sort_rec> &recs_v, bm2_sort_out *out) {
+    bm2_ctx *ctx_for_error = ctx;
     std::vector<int64_t> cut;
     SortLayout L;
-    bam_sort_layout(carry_len, h_offs, nr, total, last != 0, cut, L, h_info);
-    // the members: the sorted buffer is free after the gather, so the compressed bytes are gathered into the records' input buffer
+    bam_sort_layout(carry_len, offs, n_recs, total, last != 0, cut, L, recs);
     const uint8_t *z = nullptr; int64_t zl = 0;
-    if (bgzf_compress_device(ctx, (const uint8_t *) b[SD_OUT].p, L.starts.data(), L.n_full, &z, &zl, &b[SD_IN])) return 1;
-    ctx->sort_ms[3] = ctx->bgzf_ms;
+    if (bgzf_compress_device(ctx, d_stream, L.starts.data(), L.n_full, &z, &zl, gather)) return 1;
     const int64_t c0 = L.starts[(size_t) L.n_full], c1 = carry_len + total;
-    ctx->sort_carry.resize((size_t) (c1 - c0));
-    if (c1 > c0) BM2_CUDA_OK(cudaMemcpy(ctx->sort_carry.data(), (const uint8_t *) b[SD_OUT].p + c0, (size_t) (c1 - c0), cudaMemcpyDeviceToHost));
-    ctx->sort_recs.assign(h_info, h_info + nr);
+    carry_v.resize((size_t) (c1 - c0));
+    if (c1 > c0) BM2_CUDA_OK(cudaMemcpy(carry_v.data(), d_stream + c0, (size_t) (c1 - c0), cudaMemcpyDeviceToHost));
+    recs_v.assign(recs, recs + n_recs);
     out->z = z; out->z_len = zl;
     out->member_size = ctx->bgzf_sizes.data(); out->n_members = L.n_full;
-    out->carry = ctx->sort_carry.data(); out->carry_len = c1 - c0;
-    out->recs = ctx->sort_recs.data(); out->n_recs = nr;
+    out->carry = carry_v.data(); out->carry_len = c1 - c0;
+    out->recs = recs_v.data(); out->n_recs = n_recs;
     return 0;
 }
 

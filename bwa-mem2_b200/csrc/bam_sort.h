@@ -4,9 +4,9 @@
 //           A full run goes to a sorter thread, which sorts and compresses it with the device call and writes it to a temporary file
 //           (opened, then unlinked at once, so that nothing is left behind whatever happens), while the next run fills: host memory is two
 //           runs.  When the whole output fits in one run, that run, sorted, is the output and no file is written.
-//   merge   window by window: every unfinished run loads its next members (inflated by zlib on a pool of threads) until it holds about
-//           run_bytes / runs of whole records.  T is the smallest last-loaded key over the runs not yet fully loaded, r* the first such run
-//           whose last key is T; every loaded record with key < T, and those with key == T of runs up to r*, are settled.  They are
+//   merge   window by window: every unfinished run loads its next members (inflated by zlib on a pool of threads: bgzf_inflate, which
+//           bm2_applybqsr's window reader shares) until it holds about run_bytes / runs of whole records.  T is the smallest last-loaded key
+//           over the runs not yet fully loaded, r* the first such run whose last key is T; every loaded record with key < T, and those with key == T of runs up to r*, are settled.  They are
 //           concatenated in run order and sorted with the same device call (stable, so ties keep run order and then the order within the
 //           run, which is input order), passing the carry: the BGZF blocks are cut over the whole sorted stream.  r*'s last record is
 //           always settled, so every window makes progress.
@@ -66,6 +66,36 @@ using DupCallEx = std::function<int(const bm2_dup_loc_entry *e, int64_t n, int r
 using DupSetCall = std::function<int(const uint64_t *bits, int64_t n_bits)>;
 // reports an error and does not return
 using SortFail = std::function<void(const std::string &)>;
+
+// one BGZF member's raw DEFLATE data to inflate into out: isize bytes whose CRC32 must be crc
+struct InflateJob { const uint8_t *deflate; size_t len; uint8_t *out; uint32_t isize, crc; };
+
+// the jobs inflated by zlib on up to `threads` threads; false when one does not inflate to exactly isize bytes with its CRC32.
+// busy_s (may be null) gets the threads' inflate time added, summed over the threads.
+inline bool bgzf_inflate(const std::vector<InflateJob> &jobs, int threads, double *busy_s = nullptr) {
+    std::atomic<size_t> next{0}; std::atomic<bool> bad{false};
+    std::vector<double> busy((size_t) std::max(threads, 1), 0.0);
+    auto inflate_some = [&](int t) {
+        const auto t0 = std::chrono::steady_clock::now();
+        for (size_t k; (k = next++) < jobs.size();) {
+            const InflateJob &j = jobs[k];
+            z_stream zs; memset(&zs, 0, sizeof zs);
+            if (inflateInit2(&zs, -15) != Z_OK) { bad = true; continue; }
+            zs.next_in = (Bytef *) j.deflate; zs.avail_in = (uInt) j.len;
+            zs.next_out = j.out; zs.avail_out = j.isize;
+            if (inflate(&zs, Z_FINISH) != Z_STREAM_END || zs.avail_out || zs.avail_in) bad = true;
+            else if ((uint32_t) crc32(crc32(0L, Z_NULL, 0), j.out, j.isize) != j.crc) bad = true;
+            inflateEnd(&zs);
+        }
+        busy[(size_t) t] = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+    };
+    std::vector<std::thread> pool;
+    for (int t = 1; t < std::min<int>(threads, (int) jobs.size()); ++t) pool.emplace_back(inflate_some, t);
+    inflate_some(0);
+    for (auto &t : pool) t.join();
+    if (busy_s) for (double b : busy) *busy_s += b;
+    return !bad;
+}
 
 struct BaiBuilder {
     static constexpr uint64_t kUnset = ~(uint64_t) 0;
@@ -462,23 +492,12 @@ struct BamSortSink {
                 std::vector<size_t> grow(nr, 0);
                 for (const Job &j : jobs) grow[j.run] += j.isize;
                 for (size_t r = 0; r < nr; ++r) c[r].buf.resize(c[r].buf.size() + grow[r]);
-                std::atomic<size_t> next{0}; std::atomic<bool> bad{false};
-                auto inflate_some = [&] {
-                    for (size_t k; (k = next++) < jobs.size();) {
-                        const Job &j = jobs[k];
-                        z_stream zs; memset(&zs, 0, sizeof zs);
-                        if (inflateInit2(&zs, -15) != Z_OK) { bad = true; continue; }
-                        zs.next_in = (Bytef *) j.z.data() + 18; zs.avail_in = (uInt) (j.z.size() - 26);
-                        zs.next_out = c[j.run].buf.data() + j.at; zs.avail_out = j.isize;
-                        if (inflate(&zs, Z_FINISH) != Z_STREAM_END || zs.avail_out) bad = true;
-                        inflateEnd(&zs);
-                    }
-                };
-                std::vector<std::thread> pool;
-                for (int t = 1; t < std::min<int>(threads, (int) jobs.size()); ++t) pool.emplace_back(inflate_some);
-                inflate_some();
-                for (auto &t : pool) t.join();
-                if (bad) fail("a temporary file does not inflate");
+                std::vector<InflateJob> ij;
+                for (const Job &j : jobs) {
+                    uint32_t crc; memcpy(&crc, j.z.data() + j.z.size() - 8, 4);
+                    ij.push_back({j.z.data() + 18, j.z.size() - 26, c[j.run].buf.data() + j.at, j.isize, crc});
+                }
+                if (!bgzf_inflate(ij, threads)) fail("a temporary file does not inflate");
                 for (size_t r = 0; r < nr; ++r) {                                    // the whole records now loaded
                     Cursor &x = c[r];
                     size_t q = x.recs.empty() ? x.pos : x.recs.back() + 4 + (size_t) bam_le32(x.buf.data() + x.recs.back());

@@ -105,18 +105,31 @@ struct bm2_ctx {
     int bqsr_err_kind = 0;
     std::string bqsr_rg, bqsr_err_name;
     std::vector<int64_t> bqsr_tables;
+    // bm2_bqsr_apply_set / bm2_bqsr_apply / bm2_last_bqsr_apply_stats (bqsr_apply.cu): buffers, whether tables are set, the read-group map's
+    // size, events, the device times and records seen since the tables came, the first read error (kind 0: none), the last call's outputs
+    DevBuf bqa_d[8];
+    HostBuf bqa_h[1];
+    bool bqa_set = false;
+    int bqa_n_ids = 0;
+    int64_t bqa_map_bytes = 0, bqa_seen = 0, bqa_err_index = -1;
+    cudaEvent_t bqa_ev[2] = {nullptr, nullptr};
+    double bqa_ms = 0, bqa_bgzf_ms = 0;
+    int bqa_err_kind = 0;
+    std::string bqa_err_name;
+    std::vector<uint8_t> bqa_carry;
+    std::vector<bm2_sort_rec> bqa_recs;
 
     int ensure(DevBuf &b, size_t bytes);
     int ensure_host(HostBuf &b, size_t bytes);
     std::vector<DevBuf *> all_dev() {
         std::vector<DevBuf *> v = {&io_pairs, &io_ref, &io_qer, &bsw_jobs, &bsw_outs, &bsw_scratch, &dup_bits};
         append(v, pipe_d); append(v, cigar_d); append(v, sam_d); append(v, ksw_d); append(v, fq_d);
-        append(v, bgzf_d); append(v, sort_d); append(v, dup_d); append(v, bqsr_d);
+        append(v, bgzf_d); append(v, sort_d); append(v, dup_d); append(v, bqsr_d); append(v, bqa_d);
         return v;
     }
     std::vector<HostBuf *> all_host() {
         std::vector<HostBuf *> v;
-        append(v, pipe_h); append(v, cigar_h); append(v, sam_h); append(v, fq_h); append(v, bgzf_h); append(v, sort_h);
+        append(v, pipe_h); append(v, cigar_h); append(v, sam_h); append(v, fq_h); append(v, bgzf_h); append(v, sort_h); append(v, bqa_h);
         return v;
     }
     template <class B, size_t N> static void append(std::vector<B *> &v, B (&t)[N]) { for (B &x : t) v.push_back(&x); }
@@ -129,3 +142,9 @@ int bgzf_compress_device(bm2_ctx *ctx, const uint8_t *d_in, const int64_t *start
 // bqsr_count_done adds the device time and returns 1 (the context's error set, naming the read) when one of these records is a read error
 int bqsr_count_device(bm2_ctx *ctx, const uint8_t *d_base, const int64_t *d_starts, int64_t n, cudaStream_t st);
 int bqsr_count_done(bm2_ctx *ctx, const uint8_t *d_base, const int64_t *h_starts, int64_t n);
+// bam_sort.cu: the tail of bm2_bam_sort_compress and bm2_bqsr_apply.  d_stream (device) holds carry_len bytes of the previous call's
+// unfinished block, then the records at carry_len + offs[i], total bytes of them; the stream is cut by bam_sort_layout (which sets each
+// record's block and offset in recs, HOST), the full blocks are compressed into *gather, the unfinished one (when !last) is copied to carry_v;
+// out gets the members, carry_v and recs_v (the records' bm2_sort_rec, copied from recs)
+int bam_compress_stream(bm2_ctx *ctx, const uint8_t *d_stream, int64_t carry_len, const int64_t *offs, int64_t n_recs, int64_t total, int last,
+                        bm2_sort_rec *recs, DevBuf *gather, std::vector<uint8_t> &carry_v, std::vector<bm2_sort_rec> &recs_v, bm2_sort_out *out);

@@ -139,6 +139,23 @@ BM2_HD int bqsr_ref_base(const BqsrRec &r, const BqsrView &v, int64_t g) {
     return v.ref[g];
 }
 
+// the context (-1: none) and cycle of read base k of [lo, hi), the tails set: what both the counting and the apply side key a base by
+BM2_HD void bqsr_covariates(const BqsrRec &r, int32_t k, int &cx, int &cyc) {
+    const int32_t i = k - r.lo, L = r.hi - r.lo;
+    cyc = (r.rev ? L - i : i + 1) * r.f;
+    cx = -1;
+    int c0, c1;
+    if (!r.rev) {
+        if (k == r.lo) return;
+        c0 = bqsr_ctx_letter(r, k - 1); c1 = bqsr_ctx_letter(r, k);
+    } else {
+        if (k == r.hi - 1) return;
+        c0 = bqsr_ctx_letter(r, k + 1); c1 = bqsr_ctx_letter(r, k);
+        c0 = c0 == 4 ? 4 : 3 - c0; c1 = c1 == 4 ? 4 : 3 - c1;
+    }
+    if (c0 != 4 && c1 != 4) cx = c0 * 4 + c1;
+}
+
 // read base k of a counted record, aligned at g (ins false) or inserted between g and g + 1 (ins true): false when skipped, else its
 // quality, context (-1: none), cycle and whether it is an error
 BM2_HD bool bqsr_base(const BqsrRec &r, const BqsrView &v, int32_t k, bool ins, int64_t g, int &q, int &cx, int &cyc, int &err) {
@@ -147,18 +164,7 @@ BM2_HD bool bqsr_base(const BqsrRec &r, const BqsrView &v, int32_t k, bool ins, 
     if (b == 4 || q < BQSR_MIN_Q) return false;
     if (ins ? (g >= 0 && g + 1 < v.l_pac && bqsr_bit(v.junction, g)) : bqsr_bit(v.covered, g)) return false;
     err = !ins && bqsr_ref_base(r, v, g) != b;
-    const int32_t i = k - r.lo, L = r.hi - r.lo;
-    cyc = (r.rev ? L - i : i + 1) * r.f;
-    int c0, c1;
-    if (!r.rev) {
-        if (k == r.lo) { cx = -1; return true; }
-        c0 = bqsr_ctx_letter(r, k - 1); c1 = bqsr_ctx_letter(r, k);
-    } else {
-        if (k == r.hi - 1) { cx = -1; return true; }
-        c0 = bqsr_ctx_letter(r, k + 1); c1 = bqsr_ctx_letter(r, k);
-        c0 = c0 == 4 ? 4 : 3 - c0; c1 = c1 == 4 ? 4 : 3 - c1;
-    }
-    cx = c0 == 4 || c1 == 4 ? -1 : c0 * 4 + c1;
+    bqsr_covariates(r, k, cx, cyc);
     return true;
 }
 
@@ -176,4 +182,68 @@ template <class Fn> BM2_HD void bqsr_walk(const BqsrRec &r, Fn fn) {
         } else if (op == 4) k += (int32_t) n;
         else if (op == 2 || op == 3) g += n;
     }
+}
+
+// ---- the apply side (bm2_applybqsr): GATK 4 ApplyBQSR's BQSRReadTransformer at its defaults (no quantization, qualities below 6 kept,
+// no OQ tag, no global prior), one BAM record at a time.  bqsr_apply.cu's kernel runs it with one warp per record;
+// tests/host_emul/applybqsr_emul.cpp compiles it for the host, and tests/applybqsr_util.py restates it in Python.
+//   read group  the RG:Z tag's value, matched to the input header's @RG IDs (the first line with that ID), that line's covariate (PU, else
+//               ID) and its tables (bqsr_report.h).  A record without the tag, with an ID not in the header, or of a read group without a
+//               RecalTable0 row is written unchanged; so are l_seq 0 and QUAL '*' (0xff).  Every flag is recalibrated.
+//   errors      more than 500 bases, a quality above 93: the record is not rewritten and the call reports it
+//   a base      q < 6 stays; else clamp(fastRound(P[q] + ((0.0 + D_ctx[q][ctx]) + D_cyc[q][cyc])), 1, 93), fastRound(d) = (int) (d + 0.5) for
+//               d > 0, else (int) (d - 0.5).  ctx and cyc are bqsr_covariates over the whole stored read (lo = 0, hi = l_seq: no adaptor
+//               clipping, soft clips kept), the tails being the qualities <= 2 at either end; no context: D_ctx = 0
+enum { BQSR_APPLY = 0, BQSR_KEEP = 1 };   // and BQSR_ERR_CYCLES, BQSR_ERR_QUAL
+
+// one read group's dense tables: P [94], D_ctx [94 * 16], D_cyc [94 * 1001] (cycle + 500)
+struct BqsrApplyView { const double *P, *ctx, *cyc; };
+
+// where a record's RG:Z value starts (offset from rec, its block_size field) and its length without the NUL; -1 without one.  The walk
+// stops at the first tag it cannot step over.
+BM2_HD int32_t bqsr_aux_rg(const uint8_t *rec, int32_t *len) {
+    const int32_t end = 4 + bqsr_le32(rec), l_seq = bqsr_le32(rec + 20);
+    int32_t p = 36 + rec[12] + 4 * (rec[16] | rec[17] << 8) + ((l_seq + 1) >> 1) + l_seq;
+    while (p + 3 <= end) {
+        const uint8_t t0 = rec[p], t1 = rec[p + 1], ty = rec[p + 2];
+        p += 3;
+        if (ty == 'Z' || ty == 'H') {
+            int32_t q = p;
+            while (q < end && rec[q]) ++q;
+            if (q >= end) return -1;
+            if (t0 == 'R' && t1 == 'G' && ty == 'Z') { *len = q - p; return p; }
+            p = q + 1;
+        } else if (ty == 'B') {
+            if (p + 5 > end) return -1;
+            const uint8_t s = rec[p];
+            const int es = s == 'c' || s == 'C' ? 1 : s == 's' || s == 'S' ? 2 : s == 'i' || s == 'I' || s == 'f' ? 4 : 0;
+            const int64_t n = (int64_t) (uint32_t) bqsr_le32(rec + p + 1);
+            if (!es || p + 5 + n * es > end) return -1;
+            p += 5 + (int32_t) (n * es);
+        } else {
+            const int sz = ty == 'A' || ty == 'c' || ty == 'C' ? 1 : ty == 's' || ty == 'S' ? 2 : ty == 'i' || ty == 'I' || ty == 'f' ? 4 : 0;
+            if (!sz) return -1;
+            p += sz;
+        }
+    }
+    return -1;
+}
+
+// the fixed fields of a record to recalibrate: status BQSR_APPLY, BQSR_KEEP or BQSR_ERR_CYCLES; lo = 0, hi = l_seq
+BM2_HD void bqsr_apply_prep(const uint8_t *rec, BqsrRec &r) {
+    const int l_name = rec[12], n_cigar = rec[16] | rec[17] << 8, flag = rec[18] | rec[19] << 8;
+    const int32_t l_seq = bqsr_le32(rec + 20);
+    r.seq = rec + 36 + l_name + 4 * n_cigar; r.qual = r.seq + ((l_seq + 1) >> 1); r.l_seq = l_seq;
+    r.rev = (flag & 16) != 0; r.f = (flag & 1) && (flag & 0x80) ? -1 : 1;
+    r.lo = 0; r.hi = l_seq; r.tl = 0; r.tr = l_seq;
+    r.cig = nullptr; r.n_cigar = 0; r.g0 = 0; r.hole = -1;
+    r.status = l_seq <= 0 || r.qual[0] == 0xff ? (int) BQSR_KEEP : l_seq > BQSR_MAX_CYCLE ? (int) BQSR_ERR_CYCLES : (int) BQSR_APPLY;
+}
+
+// the recalibrated quality of a base of quality q with context cx (-1: none) and cycle cyc
+BM2_HD int bqsr_recal_q(const BqsrApplyView &t, int q, int cx, int cyc) {
+    if (q < BQSR_MIN_Q) return q;
+    const double d = t.P[q] + ((0.0 + (cx >= 0 ? t.ctx[q * BQSR_NCTX + cx] : 0.0)) + t.cyc[q * BQSR_NCYC + cyc + BQSR_MAX_CYCLE]);
+    const int v = d > 0 ? (int) (d + 0.5) : (int) (d - 0.5);
+    return v < 1 ? 1 : v > BQSR_NQ - 1 ? BQSR_NQ - 1 : v;
 }

@@ -542,6 +542,42 @@ int  bm2_bqsr_count(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int64_t 
 /* The counts since bm2_bqsr_sites (HOST arrays owned by the context, valid until its next call). */
 int  bm2_bqsr_tables(bm2_ctx *ctx, bm2_bqsr_tables_t *out);
 
+/* ---- Base quality recalibration applied (bm2_applybqsr) ------------------------------------------------------------------------------
+ * The rule (csrc/bqsr_device.cuh, csrc/bqsr_report.h) restates GATK 4 ApplyBQSR's BQSRReadTransformer at its defaults: no quantization,
+ * qualities below 6 kept, no OQ tag, no global prior; byte equality with GATK is not claimed.  A record's read group is its RG:Z value looked
+ * up among the header's @RG IDs; a record without one, of a read group without tables, with l_seq 0 or with QUAL '*' is left unchanged.
+ * Any other record's qualities q >= 6 become clamp(fastRound(P[q] + ((0.0 + D_ctx[q][ctx]) + D_cyc[q][cyc])), 1, 93), the context and
+ * cycle taken over the whole stored read; a read of more than 500 bases or with a quality above 93 is an error. */
+typedef struct {
+    int32_t n_rg;                          /* read groups with tables                                                            */
+    const double *P, *ctx, *cyc;           /* per read group: P [94], D_ctx [94 * 16], D_cyc [94 * 1001] (cycle + 500)           */
+    int32_t n_ids;                         /* the input header's @RG lines                                                       */
+    const char *const *ids;                /* their IDs (the first of equal IDs is the one matched)                              */
+    const int32_t *id_table;               /* each ID's read group (its PU, else its ID) as an index into the tables, or -1      */
+} bm2_bqsr_apply_tables_t;
+typedef struct {
+    double apply_ms, bgzf_ms;              /* device time of the apply kernel and of BGZF (CUDA events)                          */
+    int64_t bases_changed;                 /* bases whose quality changed                                                        */
+    int64_t recal_records, kept_records;   /* records recalibrated, records left unchanged                                       */
+    int32_t err_kind;                      /* the first read error: 0 none, 1 more than 500 bases, 2 a quality above 93;         */
+    int64_t err_index;                     /*   its record's index over all records since bm2_bqsr_apply_set                     */
+    const char *err_name;                  /*   and its read name                                                                */
+} bm2_bqsr_apply_stats_t;
+/* The dense tables and the read-group map to the context (no index needed), copied; resets the counts.  The IDs with their 16-byte entries
+ * may take at most 32768 bytes. */
+int  bm2_bqsr_apply_set(bm2_ctx *ctx, const bm2_bqsr_apply_tables_t *tables);
+/* One window: recs (HOST, n bytes) holds n_recs whole records, the first at 0, each starting where the one before ends, the last ending at n;
+ * starts: their offsets.  They are recalibrated on the device and compressed after carry exactly as bm2_bam_sort_compress compresses its
+ * sorted records (same members, carry and bm2_sort_rec per record, in input order).  A read error writes nothing and fails with an error
+ * naming the read. */
+int  bm2_bqsr_apply(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int64_t *starts, int64_t n_recs, const uint8_t *carry, int64_t carry_len,
+                    int last, bm2_sort_out *out);
+/* The totals since bm2_bqsr_apply_set (err_name: owned by the context, valid until its next call). */
+int  bm2_last_bqsr_apply_stats(bm2_ctx *ctx, bm2_bqsr_apply_stats_t *out);
+/* Device bytes bm2_bqsr_apply needs for windows of window_bytes of records of about 300 bytes with n_rg read groups' tables, and the bytes
+ * free on ctx's device now. */
+int  bm2_bqsr_apply_memory(const bm2_ctx *ctx, int64_t window_bytes, int32_t n_rg, int64_t *needed, int64_t *free_bytes);
+
 /* Staged mate rescue inside bm2_sam_pe (same records, other kernels): the windows mem_matesw (src/bwamem_pair.cpp:150-283) can ask for are
  * listed for all pairs of a wave from the regions before any rescue, aligned as one batch with one window per warp (the job shape of
  * bm2_ksw_align2; the reference batches the same alignments across pairs in its kswv path, src/bwamem_pair.cpp:930-1248, src/kswv.cpp),
