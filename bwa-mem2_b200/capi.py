@@ -232,6 +232,16 @@ class BqsrApplyStats(C.Structure):
                 ("kept_records", C.c_int64), ("err_kind", C.c_int32), ("err_index", C.c_int64), ("err_name", C.c_char_p)]
 
 
+# bm2_wgs_set / bm2_wgs_finish (include/bm2_b200.h)
+class WgsParams(C.Structure):
+    _fields_ = [("min_mapq", C.c_int32), ("min_baseq", C.c_int32), ("coverage_cap", C.c_int32), ("count_unpaired", C.c_int32)]
+
+
+class WgsResult(C.Structure):
+    _fields_ = [("hist", C.c_void_p), ("cap", C.c_int32), ("exc", C.c_int64 * 6), ("records", C.c_int64), ("counted_records", C.c_int64),
+                ("carried_max", C.c_int64), ("add_ms", C.c_double), ("finish_ms", C.c_double)]
+
+
 class SortOut(C.Structure):
     _fields_ = [("z", C.c_void_p), ("z_len", C.c_int64), ("member_size", C.c_void_p), ("n_members", C.c_int64), ("carry", C.c_void_p),
                 ("carry_len", C.c_int64), ("recs", C.c_void_p), ("n_recs", C.c_int64)]
@@ -244,7 +254,7 @@ EXPORTS = ["bm2_create_sibling", "bm2_fastq_encode", "bm2_seq_encode", "bm2_fast
            "bm2_bam_sort_compress", "bm2_last_sort_stats", "bm2_bam_sort_memory", "bm2_bam_sort_memory_ex", "bm2_bam_sort_compress_ex",
            "bm2_dup_signatures", "bm2_dup_resolve", "bm2_last_dup_stats", "bm2_dup_set", "bm2_dup_signatures_ex", "bm2_dup_resolve_ex",
            "bm2_bqsr_sites", "bm2_bqsr_count", "bm2_bqsr_tables", "bm2_bqsr_apply_set", "bm2_bqsr_apply", "bm2_last_bqsr_apply_stats",
-           "bm2_bqsr_apply_memory"]
+           "bm2_bqsr_apply_memory", "bm2_wgs_set", "bm2_wgs_memory", "bm2_wgs_add", "bm2_wgs_finish"]
 
 _lib = None
 
@@ -755,6 +765,44 @@ class Context:
         out = {k: getattr(s, k) for k, _ in s._fields_}
         out["err_name"] = (s.err_name or b"").decode()
         return out
+
+    def wgs_set(self, contig_off, contig_len, l_pac: int, nocall, min_mapq=20, min_baseq=20, coverage_cap=250, count_unpaired=False):
+        """bm2_wgs_set: one coverage counter per reference base, the no-call ranges ([beg, end) pairs) and Picard's parameters."""
+        off = np.ascontiguousarray(contig_off, np.int64); ln = np.ascontiguousarray(contig_len, np.int32)
+        h = np.ascontiguousarray(nocall, np.int64).reshape(-1)
+        hb = h if len(h) else np.zeros(2, np.int64)
+        p = WgsParams(int(min_mapq), int(min_baseq), int(coverage_cap), int(bool(count_unpaired)))
+        f = lib().bm2_wgs_set
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]
+        self._check(f(self._ctx, off.ctypes.data if len(off) else None, ln.ctypes.data if len(ln) else None, len(off), int(l_pac), hb.ctypes.data,
+                      len(h) // 2, C.byref(p)), "bm2_wgs_set")
+
+    def wgs_memory(self, l_pac: int, window_bytes: int):
+        """bm2_wgs_memory -> (bytes needed, bytes free)."""
+        need, free = C.c_int64(), C.c_int64()
+        f = lib().bm2_wgs_memory
+        f.argtypes = [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p]
+        self._check(f(self._ctx, int(l_pac), int(window_bytes), C.byref(need), C.byref(free)), "bm2_wgs_memory")
+        return need.value, free.value
+
+    def wgs_add(self, data: bytes, starts):
+        """bm2_wgs_add: one window of records (uncompressed BAM at starts, in file order).  A read error raises Bm2Error naming the read."""
+        starts = np.ascontiguousarray(starts, np.int64)
+        buf = np.frombuffer(data, np.uint8) if len(data) else np.zeros(1, np.uint8)
+        sb = starts if len(starts) else np.zeros(1, np.int64)
+        f = lib().bm2_wgs_add
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64]
+        self._check(f(self._ctx, buf.ctypes.data, len(data), sb.ctypes.data, len(starts)), "bm2_wgs_add")
+
+    def wgs_finish(self):
+        """bm2_wgs_finish -> dict(hist [cap + 1], exc [6]: MAPQ, DUPE, UNPAIRED, BASEQ, OVERLAP, CAPPED, records, counted_records, carried_max,
+        add_ms, finish_ms)."""
+        r = WgsResult()
+        f = lib().bm2_wgs_finish
+        f.argtypes = [C.c_void_p, C.c_void_p]
+        self._check(f(self._ctx, C.byref(r)), "bm2_wgs_finish")
+        return dict(hist=_host(r.hist, r.cap + 1, np.int64), exc=[int(x) for x in r.exc], records=r.records, counted_records=r.counted_records,
+                    carried_max=r.carried_max, add_ms=r.add_ms, finish_ms=r.finish_ms)
 
     def set_sam_staged(self, on: int):
         """bm2_set_sam_staged: 1 / 2 = the rescue's local alignments as a batch (one window per warp / per thread) before the per-pair kernel, 0 = inside it."""

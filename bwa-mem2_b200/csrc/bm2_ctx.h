@@ -118,13 +118,27 @@ struct bm2_ctx {
     std::string bqa_err_name;
     std::vector<uint8_t> bqa_carry;
     std::vector<bm2_sort_rec> bqa_recs;
+    // bm2_wgs_set / bm2_wgs_add / bm2_wgs_finish (wgs.cu): buffers, whether counters are set, the parameters and contigs, events, the
+    // records seen and counted since the counters came, the carried records (bytes and starts, on the host), the device times, the histogram
+    DevBuf wgs_d[16];
+    bool wgs_set = false;
+    bm2_wgs_params_t wgs_params{};
+    int64_t wgs_l_pac = 0;
+    int32_t wgs_n_contigs = 0;
+    std::vector<int64_t> wgs_contig_off;
+    cudaEvent_t wgs_ev[2] = {nullptr, nullptr};
+    int64_t wgs_seen = 0, wgs_counted = 0, wgs_carried_max = 0;
+    std::vector<uint8_t> wgs_carry;
+    std::vector<int64_t> wgs_carry_starts;
+    double wgs_add_ms = 0, wgs_finish_ms = 0;
+    std::vector<int64_t> wgs_hist;
 
     int ensure(DevBuf &b, size_t bytes);
     int ensure_host(HostBuf &b, size_t bytes);
     std::vector<DevBuf *> all_dev() {
         std::vector<DevBuf *> v = {&io_pairs, &io_ref, &io_qer, &bsw_jobs, &bsw_outs, &bsw_scratch, &dup_bits};
         append(v, pipe_d); append(v, cigar_d); append(v, sam_d); append(v, ksw_d); append(v, fq_d);
-        append(v, bgzf_d); append(v, sort_d); append(v, dup_d); append(v, bqsr_d); append(v, bqa_d);
+        append(v, bgzf_d); append(v, sort_d); append(v, dup_d); append(v, bqsr_d); append(v, bqa_d); append(v, wgs_d);
         return v;
     }
     std::vector<HostBuf *> all_host() {

@@ -578,6 +578,44 @@ int  bm2_last_bqsr_apply_stats(bm2_ctx *ctx, bm2_bqsr_apply_stats_t *out);
  * free on ctx's device now. */
 int  bm2_bqsr_apply_memory(const bm2_ctx *ctx, int64_t window_bytes, int32_t n_rg, int64_t *needed, int64_t *free_bytes);
 
+/* ---- Whole-genome coverage metrics (bm2_wgsmetrics) ----------------------------------------------------------------------------------
+ * The rule (csrc/wgs_device.cuh, csrc/wgs_metrics.h) restates Picard CollectWgsMetrics at its defaults (USE_FAST_ALGORITHM=false, no
+ * INTERVALS); byte equality with Picard is not claimed.  Records with 0x4, refID -1 or 0x200 count nowhere.  Then the first filter that
+ * matches takes a record and its aligned (M / = / X) bases: MAPQ < min_mapq -> EXC_MAPQ, 0x400 -> EXC_DUPE, unless count_unpaired no 0x1 or
+ * 0x8 -> EXC_UNPAIRED, 0x100 -> counted nowhere.  Each aligned base of a record that passes, at locus g (contig offset + pos + reference
+ * offset): nothing at a no-call locus; quality < min_baseq or base N -> EXC_BASEQ; else EXC_OVERLAP when an earlier record of the same QNAME
+ * has such a base at g, else pileup[g] += 1.  Every locus that is not no-call: H[min(pileup, cap)] += 1, EXC_CAPPED += max(0, pileup - cap). */
+#define BM2_WGS_MAX_CAP 10000
+typedef struct {
+    int32_t min_mapq, min_baseq;           /* Picard's MINIMUM_MAPPING_QUALITY and MINIMUM_BASE_QUALITY (20, 20)                 */
+    int32_t coverage_cap;                  /* COVERAGE_CAP, 1 .. BM2_WGS_MAX_CAP (250)                                            */
+    int32_t count_unpaired;                /* COUNT_UNPAIRED (0)                                                                  */
+} bm2_wgs_params_t;
+typedef struct {
+    const int64_t *hist;                   /* [cap + 1]: loci by min(pileup, cap), no-call loci left out (owned by the context)   */
+    int32_t cap;
+    int64_t exc[6];                        /* bases excluded: MAPQ, DUPE, UNPAIRED, BASEQ, OVERLAP, CAPPED                        */
+    int64_t records, counted_records;      /* records added, records that passed the filters                                     */
+    int64_t carried_max;                   /* the most records carried from one window into the next                             */
+    double add_ms, finish_ms;              /* device time of the add kernels and of the finish (CUDA events)                     */
+} bm2_wgs_result_t;
+/* One uint32 counter per reference base (l_pac of them, 4 bytes each) and a no-call bitset (1 bit per base) set over `nocall` (n_nocall
+ * sorted [beg, end) pairs: the .amb holes of N, n or .); the contigs' offsets and lengths in the concatenated reference.  Zeroes the counters
+ * and the exclusion counts.  Counters larger than the free device memory are an error that gives both numbers. */
+int  bm2_wgs_set(bm2_ctx *ctx, const int64_t *contig_off, const int32_t *contig_len, int32_t n_contigs, int64_t l_pac, const int64_t *nocall,
+                 int64_t n_nocall, const bm2_wgs_params_t *params);
+/* Device bytes bm2_wgs_set and bm2_wgs_add need for a reference of l_pac bases and windows of window_bytes of records of about 300 bytes,
+ * and the bytes free on ctx's device now (counting the counters this context already holds). */
+int  bm2_wgs_memory(const bm2_ctx *ctx, int64_t l_pac, int64_t window_bytes, int64_t *needed, int64_t *free_bytes);
+/* One window: recs (HOST, n bytes) holds n_recs records at starts, in file order, after those of earlier calls.  Every record is checked
+ * before anything is counted: a record that is not skipped whose refID is not a contig or whose alignment does not lie inside its contig, or
+ * whose CG:B,I CIGAR runs past the record, and a record that passes the filters with l_seq 0, QUAL '*' or a CIGAR whose query length is not
+ * l_seq is a read error: the first such record by index is named in the error and 2 is returned, with nothing of the window counted.  The
+ * overlap rule is exact across windows: the records a later window may still overlap are carried. */
+int  bm2_wgs_add(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int64_t *starts, int64_t n_recs);
+/* The pass over every locus: the histogram, the exclusion counts and the totals since bm2_wgs_set.  It may be called again. */
+int  bm2_wgs_finish(bm2_ctx *ctx, bm2_wgs_result_t *out);
+
 /* Staged mate rescue inside bm2_sam_pe (same records, other kernels): the windows mem_matesw (src/bwamem_pair.cpp:150-283) can ask for are
  * listed for all pairs of a wave from the regions before any rescue, aligned as one batch with one window per warp (the job shape of
  * bm2_ksw_align2; the reference batches the same alignments across pairs in its kswv path, src/bwamem_pair.cpp:930-1248, src/kswv.cpp),
