@@ -242,6 +242,13 @@ class WgsResult(C.Structure):
                 ("carried_max", C.c_int64), ("add_ms", C.c_double), ("finish_ms", C.c_double)]
 
 
+# bm2_mm_finish (include/bm2_b200.h)
+class MmResult(C.Structure):
+    _fields_ = [("counts", C.c_int64 * 63), ("max_len", C.c_int32), ("len_hist", C.c_void_p), ("mism_hist", C.c_void_p), ("nocall", C.c_void_p),
+                ("max_insert", C.c_int32), ("insert_hist", C.c_void_p), ("insert_big", C.c_void_p), ("n_big", C.c_int64), ("records", C.c_int64),
+                ("add_ms", C.c_double), ("finish_ms", C.c_double)]
+
+
 class SortOut(C.Structure):
     _fields_ = [("z", C.c_void_p), ("z_len", C.c_int64), ("member_size", C.c_void_p), ("n_members", C.c_int64), ("carry", C.c_void_p),
                 ("carry_len", C.c_int64), ("recs", C.c_void_p), ("n_recs", C.c_int64)]
@@ -254,7 +261,8 @@ EXPORTS = ["bm2_create_sibling", "bm2_fastq_encode", "bm2_seq_encode", "bm2_fast
            "bm2_bam_sort_compress", "bm2_last_sort_stats", "bm2_bam_sort_memory", "bm2_bam_sort_memory_ex", "bm2_bam_sort_compress_ex",
            "bm2_dup_signatures", "bm2_dup_resolve", "bm2_last_dup_stats", "bm2_dup_set", "bm2_dup_signatures_ex", "bm2_dup_resolve_ex",
            "bm2_bqsr_sites", "bm2_bqsr_count", "bm2_bqsr_tables", "bm2_bqsr_apply_set", "bm2_bqsr_apply", "bm2_last_bqsr_apply_stats",
-           "bm2_bqsr_apply_memory", "bm2_wgs_set", "bm2_wgs_memory", "bm2_wgs_add", "bm2_wgs_finish"]
+           "bm2_bqsr_apply_memory", "bm2_wgs_set", "bm2_wgs_memory", "bm2_wgs_add", "bm2_wgs_finish",
+           "bm2_mm_set", "bm2_mm_memory", "bm2_mm_add", "bm2_mm_finish"]
 
 _lib = None
 
@@ -803,6 +811,48 @@ class Context:
         self._check(f(self._ctx, C.byref(r)), "bm2_wgs_finish")
         return dict(hist=_host(r.hist, r.cap + 1, np.int64), exc=[int(x) for x in r.exc], records=r.records, counted_records=r.counted_records,
                     carried_max=r.carried_max, add_ms=r.add_ms, finish_ms=r.finish_ms)
+
+    def mm_set(self, contig_off, contig_len, l_pac: int, pac, holes, hole_char: bytes):
+        """bm2_mm_set: the contigs, the packed reference ((l_pac + 3) // 4 bytes) and the .amb holes ([beg, end) pairs, one letter each)."""
+        off = np.ascontiguousarray(contig_off, np.int64); ln = np.ascontiguousarray(contig_len, np.int32)
+        pb = np.ascontiguousarray(pac, np.uint8)
+        h = np.ascontiguousarray(holes, np.int64).reshape(-1)
+        hb = h if len(h) else np.zeros(2, np.int64)
+        f = lib().bm2_mm_set
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_char_p, C.c_int64]
+        self._check(f(self._ctx, off.ctypes.data if len(off) else None, ln.ctypes.data if len(ln) else None, len(off), int(l_pac), pb.ctypes.data,
+                      hb.ctypes.data, bytes(hole_char), len(h) // 2), "bm2_mm_set")
+
+    def mm_memory(self, l_pac: int, window_bytes: int):
+        """bm2_mm_memory -> (bytes needed, bytes free)."""
+        need, free = C.c_int64(), C.c_int64()
+        f = lib().bm2_mm_memory
+        f.argtypes = [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p]
+        self._check(f(self._ctx, int(l_pac), int(window_bytes), C.byref(need), C.byref(free)), "bm2_mm_memory")
+        return need.value, free.value
+
+    def mm_add(self, data: bytes, starts):
+        """bm2_mm_add: one window of records (uncompressed BAM at starts, any order).  A read error raises Bm2Error naming the read."""
+        starts = np.ascontiguousarray(starts, np.int64)
+        buf = np.frombuffer(data, np.uint8) if len(data) else np.zeros(1, np.uint8)
+        sb = starts if len(starts) else np.zeros(1, np.int64)
+        f = lib().bm2_mm_add
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64]
+        self._check(f(self._ctx, buf.ctypes.data, len(data), sb.ctypes.data, len(starts)), "bm2_mm_add")
+
+    def mm_finish(self):
+        """bm2_mm_finish -> dict(counts [3, 21], len_hist / mism_hist / nocall [3, max_len + 1], insert_hist [3, max_insert + 1], insert_big
+        (orientation << 32 | size, sorted), records, add_ms, finish_ms)."""
+        r = MmResult()
+        f = lib().bm2_mm_finish
+        f.argtypes = [C.c_void_p, C.c_void_p]
+        self._check(f(self._ctx, C.byref(r)), "bm2_mm_finish")
+        L, I = r.max_len + 1, r.max_insert + 1
+        return dict(counts=np.array(r.counts, np.int64).reshape(3, 21), len_hist=_host(r.len_hist, 3 * L, np.int64).reshape(3, L),
+                    mism_hist=_host(r.mism_hist, 3 * L, np.int64).reshape(3, L), nocall=_host(r.nocall, 3 * L, np.int64).reshape(3, L),
+                    insert_hist=_host(r.insert_hist, 3 * I, np.int64).reshape(3, I),
+                    insert_big=_host(r.insert_big, r.n_big, np.uint64) if r.n_big else np.zeros(0, np.uint64), records=r.records,
+                    add_ms=r.add_ms, finish_ms=r.finish_ms)
 
     def set_sam_staged(self, on: int):
         """bm2_set_sam_staged: 1 / 2 = the rescue's local alignments as a batch (one window per warp / per thread) before the per-pair kernel, 0 = inside it."""

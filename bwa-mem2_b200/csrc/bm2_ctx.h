@@ -132,6 +132,17 @@ struct bm2_ctx {
     std::vector<int64_t> wgs_carry_starts;
     double wgs_add_ms = 0, wgs_finish_ms = 0;
     std::vector<int64_t> wgs_hist;
+    // bm2_mm_set / bm2_mm_add / bm2_mm_finish (mm.cu): buffers, whether a reference is set, its contigs and holes, events, the records seen
+    // since, the insert sizes of 2^20 or more (copied back after each window), the device times, the histograms copied back by the finish
+    DevBuf mm_d[16];
+    bool mm_set = false;
+    int64_t mm_l_pac = 0, mm_n_holes = 0;
+    int32_t mm_n_contigs = 0;
+    cudaEvent_t mm_ev[2] = {nullptr, nullptr};
+    int64_t mm_seen = 0;
+    std::vector<uint64_t> mm_big;
+    double mm_add_ms = 0, mm_finish_ms = 0;
+    std::vector<int64_t> mm_hist;
 
     int ensure(DevBuf &b, size_t bytes);
     int ensure_host(HostBuf &b, size_t bytes);
@@ -139,6 +150,7 @@ struct bm2_ctx {
         std::vector<DevBuf *> v = {&io_pairs, &io_ref, &io_qer, &bsw_jobs, &bsw_outs, &bsw_scratch, &dup_bits};
         append(v, pipe_d); append(v, cigar_d); append(v, sam_d); append(v, ksw_d); append(v, fq_d);
         append(v, bgzf_d); append(v, sort_d); append(v, dup_d); append(v, bqsr_d); append(v, bqa_d); append(v, wgs_d);
+        append(v, mm_d);
         return v;
     }
     std::vector<HostBuf *> all_host() {

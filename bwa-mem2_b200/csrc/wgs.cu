@@ -31,17 +31,8 @@ constexpr unsigned kFull = 0xFFFFFFFFu;
 constexpr int kRecBytes = 300;              // a short read's record, for bm2_wgs_memory's estimate
 
 __global__ void wgs_nocall_kernel(uint32_t *bits, int64_t n_words, const int64_t *ranges, int64_t n) {
-    for (int64_t w = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; w < n_words; w += (int64_t) gridDim.x * blockDim.x) {
-        const int64_t b = w * 32, e = b + 32;
-        int64_t lo = 0, hi = n;                                          // the first range ending after b
-        while (lo < hi) { const int64_t m = (lo + hi) / 2; if (ranges[2 * m + 1] <= b) lo = m + 1; else hi = m; }
-        uint32_t v = 0;
-        for (int64_t h = lo; h < n && ranges[2 * h] < e; ++h) {
-            const int64_t x = bm2_max(ranges[2 * h], b) - b, y = bm2_min(ranges[2 * h + 1], e) - b;
-            for (int64_t k = x; k < y; ++k) v |= 1u << k;
-        }
-        bits[w] = v;
-    }
+    for (int64_t w = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; w < n_words; w += (int64_t) gridDim.x * blockDim.x)
+        bits[w] = wgs_range_word(ranges, n, w);
 }
 
 __global__ void __launch_bounds__(kWarps * 32) wgs_check_kernel(const uint8_t *__restrict__ base, const int64_t *__restrict__ starts, int64_t n,

@@ -99,6 +99,19 @@ BM2_HD bool wgs_hq(const WgsSeq &s, int64_t k, int min_baseq) {
 
 BM2_HD bool wgs_nocall(const uint32_t *bits, int64_t g) { return (bits[g >> 5] >> (g & 31)) & 1; }
 
+// word w of a bitset over n sorted, disjoint [beg, end) ranges (ranges[2h], ranges[2h + 1]): bit k set when locus 32w + k lies in one
+BM2_HD uint32_t wgs_range_word(const int64_t *ranges, int64_t n, int64_t w) {
+    const int64_t b = w * 32, e = b + 32;
+    int64_t lo = 0, hi = n;                                              // the first range ending after b
+    while (lo < hi) { const int64_t m = (lo + hi) / 2; if (ranges[2 * m + 1] <= b) lo = m + 1; else hi = m; }
+    uint32_t v = 0;
+    for (int64_t h = lo; h < n && ranges[2 * h] < e; ++h) {
+        const int64_t x = bm2_max(ranges[2 * h], b) - b, y = bm2_min(ranges[2 * h + 1], e) - b;
+        for (int64_t k = x; k < y; ++k) v |= 1u << k;
+    }
+    return v;
+}
+
 // whether a passing record has a high-quality base at locus g (a linear walk of its CIGAR; false outside its aligned blocks)
 BM2_HD bool wgs_hq_at(const uint8_t *r, const DupCigar &c, int64_t g0, int64_t g, int min_baseq) {
     if (g < g0) return false;

@@ -2,8 +2,9 @@
 // order, and Picard's WgsMetrics formulas and file text (the per-locus rule is wgs_device.cuh's; byte equality with Picard is not claimed).
 //
 //   reference  .ann: "l_pac n_seqs seed", then per contig "gi name[ anno]" and "offset len n_ambs"; .amb: "l_pac n_seqs n_holes", then
-//              "offset len char" per hole.  The holes of N, n and . are the no-call loci.
+//              "offset len char" per hole.  The holes of N, n and . are the no-call loci; every hole is kept with its letter as well.
 //   header     @HD must say SO:coordinate; the binary reference list must equal the .ann contigs in order, names and lengths
+//              (wgs_check_refs, which bm2_multiplemetrics calls alone)
 //   order      bam_coord_key never decreases from one record to the next
 //   metrics    T = sum H[d], C = sum d H[d]; MEAN = C / T; SD = sqrt(sum H[d] (d - MEAN)^2 / (T - 1)); MEDIAN of the multiset of depths (even T:
 //              the mean of the T/2-th and T/2+1-th smallest, odd T: the ceil(T/2)-th); MAD the same median over |d - MEDIAN|;
@@ -28,6 +29,8 @@ struct WgsReference {
     std::vector<int64_t> off;
     std::vector<int32_t> len;
     std::vector<int64_t> nocall;          // [beg, end) pairs, sorted
+    std::vector<int64_t> holes;           // every hole as [beg, end) pairs, in .amb order
+    std::vector<char> hole_char;          // each hole's letter
 };
 
 inline std::string wgs_read_reference(const std::string &prefix, WgsReference &r) {
@@ -53,11 +56,24 @@ inline std::string wgs_read_reference(const std::string &prefix, WgsReference &r
     for (long long h = 0; h < nh; ++h) {
         char c;
         if (fscanf(f, "%lld %lld %c", &a, &b, &c) != 3 || a < 0 || b < 0 || a + b > l_pac) { fclose(f); return prefix + ".amb: a bad hole line"; }
+        r.holes.push_back(a); r.holes.push_back(a + b); r.hole_char.push_back(c);
         if (c != 'N' && c != 'n' && c != '.') continue;
         if (!r.nocall.empty() && a < r.nocall.back()) { fclose(f); return prefix + ".amb: the holes are not sorted"; }
         r.nocall.push_back(a); r.nocall.push_back(a + b);
     }
     fclose(f);
+    return "";
+}
+
+// the header's reference list against the index: the first difference
+inline std::string wgs_check_refs(const std::vector<std::pair<std::string, int32_t>> &refs, const WgsReference &r) {
+    for (size_t k = 0; k < std::max(refs.size(), r.names.size()); ++k) {
+        if (k >= refs.size()) return "the header has " + std::to_string(refs.size()) + " references, the index " + std::to_string(r.names.size()) + " contigs";
+        if (k >= r.names.size()) return "the header has " + std::to_string(refs.size()) + " references, the index " + std::to_string(r.names.size()) + " contigs";
+        if (refs[k].first != r.names[k] || refs[k].second != r.len[k])
+            return "reference " + std::to_string(k) + " is " + refs[k].first + " of length " + std::to_string(refs[k].second) + " in the header, " +
+                   r.names[k] + " of length " + std::to_string(r.len[k]) + " in the index";
+    }
     return "";
 }
 
@@ -69,14 +85,7 @@ inline std::string wgs_check_header(const std::string &text, const std::vector<s
         if (at != std::string::npos && at < e) so = text.substr(at + 4, std::min(text.find('\t', at + 4), e) - at - 4);
     }
     if (so != "coordinate") return "the input is not coordinate-sorted (@HD SO:" + (so.empty() ? std::string("<none>") : so) + ")";
-    for (size_t k = 0; k < std::max(refs.size(), r.names.size()); ++k) {
-        if (k >= refs.size()) return "the header has " + std::to_string(refs.size()) + " references, the index " + std::to_string(r.names.size()) + " contigs";
-        if (k >= r.names.size()) return "the header has " + std::to_string(refs.size()) + " references, the index " + std::to_string(r.names.size()) + " contigs";
-        if (refs[k].first != r.names[k] || refs[k].second != r.len[k])
-            return "reference " + std::to_string(k) + " is " + refs[k].first + " of length " + std::to_string(refs[k].second) + " in the header, " +
-                   r.names[k] + " of length " + std::to_string(r.len[k]) + " in the index";
-    }
-    return "";
+    return wgs_check_refs(refs, r);
 }
 
 // the coordinate order, record by record; the error names the read

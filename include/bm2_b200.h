@@ -616,6 +616,44 @@ int  bm2_wgs_add(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int64_t *st
 /* The pass over every locus: the histogram, the exclusion counts and the totals since bm2_wgs_set.  It may be called again. */
 int  bm2_wgs_finish(bm2_ctx *ctx, bm2_wgs_result_t *out);
 
+/* ---- Alignment summary and insert size metrics (bm2_multiplemetrics) -------------------------------------------------------------------
+ * The rule (csrc/mm_device.cuh, csrc/mm_metrics.h) restates Picard CollectAlignmentSummaryMetrics and CollectInsertSizeMetrics at their
+ * defaults; byte equality with Picard is not claimed.  Records without 0x100 and 0x800 are counted, in three categories: FIRST_OF_PAIR (0x1
+ * and 0x40), SECOND_OF_PAIR (0x1 without 0x40) and UNPAIRED.  Per category: read and base counters (the mm_device.cuh enum order), the
+ * read-length histogram, the per-read histogram of high-quality mismatch counts and the no-calls by cycle.  Per pair orientation (FR, RF,
+ * TANDEM): the insert-size histogram of second reads with both ends mapped, not duplicates, TLEN != 0. */
+#define BM2_MM_NCAT 3
+#define BM2_MM_NCOUNT 21
+typedef struct {
+    int64_t counts[BM2_MM_NCAT][BM2_MM_NCOUNT]; /* per category: the counters of mm_device.cuh                                         */
+    int32_t max_len;                       /* the longest counted read; the three arrays below are [BM2_MM_NCAT][max_len + 1]        */
+    const int64_t *len_hist;               /* reads by l_seq                                                                         */
+    const int64_t *mism_hist;              /* high-quality aligned reads by their mismatch count                                     */
+    const int64_t *nocall;                 /* read bases N by cycle (0-based, in sequencing order)                                   */
+    int32_t max_insert;                    /* the largest insert size below 2^20; insert_hist is [3][max_insert + 1]                 */
+    const int64_t *insert_hist;            /* pairs by orientation (FR, RF, TANDEM) and insert size, sizes below 2^20                */
+    const uint64_t *insert_big;            /* n_big sizes of 2^20 or more, as orientation << 32 | size, sorted                       */
+    int64_t n_big;
+    int64_t records;                       /* records added                                                                          */
+    double add_ms, finish_ms;              /* device time of the add kernels and of the finish's copies (CUDA events)                */
+} bm2_mm_result_t;                         /* the pointers are owned by the context                                                  */
+/* The reference: the contigs' offsets and lengths in the concatenated reference, pac ((l_pac + 3) / 4 bytes, base i at
+ * pac[i >> 2] >> ((~i & 3) << 1) & 3) and the .amb holes (n_holes sorted, disjoint [beg, end) pairs and their letters, which stand for the
+ * reference base inside them).  Uploads the packed bases and a hole bitset (1 bit per base), and zeroes the counters.  A reference larger than
+ * the free device memory is an error that gives both numbers. */
+int  bm2_mm_set(bm2_ctx *ctx, const int64_t *contig_off, const int32_t *contig_len, int32_t n_contigs, int64_t l_pac, const uint8_t *pac,
+                const int64_t *holes, const char *hole_char, int64_t n_holes);
+/* Device bytes bm2_mm_set and bm2_mm_add need for a reference of l_pac bases and windows of window_bytes of records of about 300 bytes, and
+ * the bytes free on ctx's device now (counting the reference this context already holds). */
+int  bm2_mm_memory(const bm2_ctx *ctx, int64_t l_pac, int64_t window_bytes, int64_t *needed, int64_t *free_bytes);
+/* One window: recs (HOST, n bytes) holds n_recs records at starts, in any order.  Every record is checked before anything is counted: a
+ * counted record with l_seq 0 or above 2^20, and an aligned one (PF, without 0x4) whose CG:B,I CIGAR runs past the record, whose refID is
+ * not a contig or whose alignment runs past its contig, or whose CIGAR query length is not l_seq, is a read error: the first such record
+ * by index is named in the error and 2 is returned, with nothing of the window counted.  No record is carried between windows. */
+int  bm2_mm_add(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int64_t *starts, int64_t n_recs);
+/* The counters and histograms since bm2_mm_set, copied back up to their largest keys.  It may be called again. */
+int  bm2_mm_finish(bm2_ctx *ctx, bm2_mm_result_t *out);
+
 /* Staged mate rescue inside bm2_sam_pe (same records, other kernels): the windows mem_matesw (src/bwamem_pair.cpp:150-283) can ask for are
  * listed for all pairs of a wave from the regions before any rescue, aligned as one batch with one window per warp (the job shape of
  * bm2_ksw_align2; the reference batches the same alignments across pairs in its kswv path, src/bwamem_pair.cpp:930-1248, src/kswv.cpp),
