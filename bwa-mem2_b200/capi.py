@@ -262,7 +262,8 @@ EXPORTS = ["bm2_create_sibling", "bm2_fastq_encode", "bm2_seq_encode", "bm2_fast
            "bm2_dup_signatures", "bm2_dup_resolve", "bm2_last_dup_stats", "bm2_dup_set", "bm2_dup_signatures_ex", "bm2_dup_resolve_ex",
            "bm2_bqsr_sites", "bm2_bqsr_count", "bm2_bqsr_tables", "bm2_bqsr_apply_set", "bm2_bqsr_apply", "bm2_last_bqsr_apply_stats",
            "bm2_bqsr_apply_memory", "bm2_wgs_set", "bm2_wgs_memory", "bm2_wgs_add", "bm2_wgs_finish",
-           "bm2_mm_set", "bm2_mm_memory", "bm2_mm_add", "bm2_mm_finish"]
+           "bm2_mm_set", "bm2_mm_memory", "bm2_mm_add", "bm2_mm_finish", "bm2_markdup_set", "bm2_markdup_records", "bm2_markdup_pair", "bm2_markdup_counts",
+           "bm2_markdup_mark", "bm2_last_markdup_stats", "bm2_markdup_memory"]
 
 _lib = None
 
@@ -830,6 +831,58 @@ class Context:
         f.argtypes = [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p]
         self._check(f(self._ctx, int(l_pac), int(window_bytes), C.byref(need), C.byref(free)), "bm2_mm_memory")
         return need.value, free.value
+
+    def markdup_set(self, ids, libs, n_lib: int, unknown_lib: int):
+        """bm2_markdup_set: the merged header's @RG IDs, each one's library index, the library count and the unknown library's index."""
+        self._mdb_keep = np.ascontiguousarray(list(libs) + [0], np.int32)
+        names = (C.c_char_p * max(len(ids), 1))(*[i.encode() for i in ids])
+        f = lib().bm2_markdup_set
+        f.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32]
+        self._check(f(self._ctx, len(ids), C.cast(names, C.c_void_p), self._mdb_keep.ctypes.data, int(n_lib), int(unknown_lib)), "bm2_markdup_set")
+
+    def markdup_records(self, data: bytes, starts):
+        """bm2_markdup_records: one window of records (uncompressed BAM at starts, contiguous) -> structured array of bm2_markdup_rec
+        (end, hash, score, kind, rg, lib, tile, x, y, loc)."""
+        starts = np.ascontiguousarray(starts, np.int64)
+        buf = np.frombuffer(data, np.uint8) if len(data) else np.zeros(1, np.uint8)
+        sb = starts if len(starts) else np.zeros(1, np.int64)
+        out = C.c_void_p()
+        f = lib().bm2_markdup_records
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]
+        self._check(f(self._ctx, buf.ctypes.data, len(data), sb.ctypes.data, len(starts), C.byref(out)), "bm2_markdup_records")
+        dt = np.dtype([("end", "<u8"), ("hash", "<u8"), ("score", "<i4"), ("kind", "<i4"), ("rg", "<i4"), ("lib", "<i4"), ("tile", "<i4"), ("x", "<i4"), ("y", "<i4"),
+                       ("loc", "<i4")])
+        if not len(starts):
+            return np.zeros(0, dt)
+        return np.frombuffer((C.c_uint8 * (len(starts) * dt.itemsize)).from_address(out.value), dt).copy()
+
+    def markdup_pair(self, halves, names: bytes):
+        """bm2_markdup_pair: halves (structured: hash u8, rg i4, name_len i4, name_off i8) and their names -> each one's partner or -1."""
+        h = np.ascontiguousarray(halves)
+        buf = np.frombuffer(names + b"\0", np.uint8)
+        out = C.c_void_p()
+        f = lib().bm2_markdup_pair
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]
+        self._check(f(self._ctx, h.ctypes.data if len(h) else None, len(h), buf.ctypes.data, len(names), C.byref(out)), "bm2_markdup_pair")
+        if not len(h):
+            return []
+        return np.frombuffer((C.c_int32 * len(h)).from_address(out.value), np.int32).tolist()
+
+    def markdup_counts(self, n_lib: int):
+        """bm2_markdup_counts -> int64 [n_lib, 2]: secondary or supplementary records, unmapped primaries."""
+        c = np.zeros(2 * n_lib, np.int64)
+        f = lib().bm2_markdup_counts
+        f.argtypes = [C.c_void_p, C.c_void_p]
+        self._check(f(self._ctx, c.ctypes.data), "bm2_markdup_counts")
+        return c.reshape(-1, 2)
+
+    def markdup_stats(self):
+        """bm2_last_markdup_stats -> (records_ms, pair_ms, mark_ms, bgzf_ms)."""
+        v = (C.c_double * 4)()
+        f = lib().bm2_last_markdup_stats
+        f.argtypes = [C.c_void_p, C.c_void_p]
+        self._check(f(self._ctx, v), "bm2_last_markdup_stats")
+        return tuple(v)
 
     def mm_add(self, data: bytes, starts):
         """bm2_mm_add: one window of records (uncompressed BAM at starts, any order).  A read error raises Bm2Error naming the read."""

@@ -42,6 +42,7 @@
 #include <chrono>
 #include <cstdio>
 #include <cstring>
+#include <exception>
 #include <functional>
 #include <map>
 #include <string>
@@ -199,6 +200,7 @@ struct BamSortSink {
     std::vector<uint8_t> cur; std::vector<int64_t> cur_starts, cur_tids;
     std::vector<uint8_t> pend; std::vector<int64_t> pend_starts, pend_tids;
     std::thread sorter;
+    std::exception_ptr sorter_error;             // a throwing fail() in the sorter thread, rethrown by join_sorter
     std::vector<Run> runs;
     std::vector<bm2_dup_entry> sig_cur[2], sig_pend[2];   // [0] pair space, [1] fragment space
     std::vector<SigRun> sig_runs[2];
@@ -213,6 +215,15 @@ struct BamSortSink {
         if (sorter.joinable()) sorter.join();
         for (Run &r : runs) { if (r.f) fclose(r.f); if (r.tf) fclose(r.tf); }
         for (auto &v : sig_runs) for (SigRun &r : v) if (r.f) fclose(r.f);
+    }
+
+    // waits for the sorter thread; a fail() that threw there (the host emulation's) is thrown here, on the caller's thread
+    void join_sorter() {
+        if (sorter.joinable()) sorter.join();
+        if (sorter_error) { const std::exception_ptr e = sorter_error; sorter_error = nullptr; std::rethrow_exception(e); }
+    }
+    template <class F> void start_sorter(F f) {
+        sorter = std::thread([this, f] { try { f(); } catch (...) { sorter_error = std::current_exception(); } });
     }
 
     SortCallEx call() const {
@@ -265,9 +276,9 @@ struct BamSortSink {
 
     void maybe_spill_sigs() {
         if ((int64_t) ((sig_cur[0].size() + sig_cur[1].size()) * sizeof(bm2_dup_entry) + lsig_cur.size() * sizeof(bm2_dup_loc_entry)) > sig_bytes / 2) {
-            if (sorter.joinable()) sorter.join();
+            join_sorter();
             move_sigs_to_pending();
-            sorter = std::thread([this] { spill_sigs(); });
+            start_sorter([this] { spill_sigs(); });
         }
     }
 
@@ -305,10 +316,10 @@ struct BamSortSink {
 
     // the current run to the sorter thread, once the one before is on disk
     void hand_off() {
-        if (sorter.joinable()) sorter.join();
+        join_sorter();
         pend.swap(cur); pend_starts.swap(cur_starts); pend_tids.swap(cur_tids);
         cur.clear(); cur_starts.clear(); cur_tids.clear();
-        sorter = std::thread([this] { spill(); });
+        start_sorter([this] { spill(); });
     }
 
     static FILE *open_tmp(const std::string &path, const SortFail &fail) {
@@ -355,9 +366,9 @@ struct BamSortSink {
     // everything has been added: the sorted records to out (its compressed offset now: out_off), the index to bai when not null
     void finish(FILE *out, uint64_t out_off, BaiBuilder *bai) {
         SortedWriter w{call(), fail, out, bai, out_off};
-        if (sorter.joinable()) sorter.join();
+        join_sorter();
         const bool one_run = runs.empty();
-        if (!one_run && !cur_starts.empty()) { hand_off(); sorter.join(); }
+        if (!one_run && !cur_starts.empty()) { hand_off(); join_sorter(); }
         if (dup) resolve();
         if (before_final) before_final();
         if (one_run) {

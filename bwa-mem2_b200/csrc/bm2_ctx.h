@@ -86,7 +86,7 @@ struct bm2_ctx {
     std::vector<bm2_sort_rec> sort_recs;
     std::vector<int64_t> sort_tids;        // bm2_bam_sort_compress_ex: the template ids in output order
     // bm2_dup_signatures / bm2_dup_resolve / bm2_dup_set (markdup.cu): buffers, events, the last calls' device times and outputs, the bitset
-    DevBuf dup_d[26];
+    DevBuf dup_d[27];
     DevBuf dup_bits;
     int64_t dup_n_bits = 0;
     cudaEvent_t dup_ev[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -143,6 +143,19 @@ struct bm2_ctx {
     std::vector<uint64_t> mm_big;
     double mm_add_ms = 0, mm_finish_ms = 0;
     std::vector<int64_t> mm_hist;
+    // bm2_markdup_set / bm2_markdup_records / bm2_markdup_mark (markdup_bam.cu): buffers, whether read groups are set, the map's size, the
+    // libraries, events, the device times, the last call's outputs
+    DevBuf mdb_d[14];
+    HostBuf mdb_h[1];
+    bool mdb_set = false;
+    int mdb_n_ids = 0, mdb_n_lib = 0, mdb_unknown_lib = 0;
+    int64_t mdb_map_bytes = 0;
+    cudaEvent_t mdb_ev[2] = {nullptr, nullptr};
+    double mdb_records_ms = 0, mdb_pair_ms = 0, mdb_mark_ms = 0, mdb_bgzf_ms = 0;
+    std::vector<bm2_markdup_rec> mdb_recs;
+    std::vector<int32_t> mdb_partner;
+    std::vector<uint8_t> mdb_carry;
+    std::vector<bm2_sort_rec> mdb_srecs;
 
     int ensure(DevBuf &b, size_t bytes);
     int ensure_host(HostBuf &b, size_t bytes);
@@ -150,12 +163,12 @@ struct bm2_ctx {
         std::vector<DevBuf *> v = {&io_pairs, &io_ref, &io_qer, &bsw_jobs, &bsw_outs, &bsw_scratch, &dup_bits};
         append(v, pipe_d); append(v, cigar_d); append(v, sam_d); append(v, ksw_d); append(v, fq_d);
         append(v, bgzf_d); append(v, sort_d); append(v, dup_d); append(v, bqsr_d); append(v, bqa_d); append(v, wgs_d);
-        append(v, mm_d);
+        append(v, mm_d); append(v, mdb_d);
         return v;
     }
     std::vector<HostBuf *> all_host() {
         std::vector<HostBuf *> v;
-        append(v, pipe_h); append(v, cigar_h); append(v, sam_h); append(v, fq_h); append(v, bgzf_h); append(v, sort_h); append(v, bqa_h);
+        append(v, pipe_h); append(v, cigar_h); append(v, sam_h); append(v, fq_h); append(v, bgzf_h); append(v, sort_h); append(v, bqa_h); append(v, mdb_h);
         return v;
     }
     template <class B, size_t N> static void append(std::vector<B *> &v, B (&t)[N]) { for (B &x : t) v.push_back(&x); }

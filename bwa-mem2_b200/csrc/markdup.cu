@@ -11,7 +11,8 @@
 //                        and the chunk's secondary / supplementary records and unmapped primaries counted (a ballot, one atomic per warp)
 //   bm2_dup_resolve_ex   the same sort and duplicates, the located entries permuted with the order, then the optical pass over the pair
 //                        groups: 2 .. 32 members one warp each (adjacency rows from ballots, closed under OR); 33 .. 300000 the exact cell
-//                        pass (markdup_device.cuh): the located members sorted by (group, class, tile, cell, x), cells found by a scan,
+//                        pass (markdup_device.cuh): the located members sorted by (group, class, tile, read group, cell, x) - the read-group
+//                        pass only when some member has one (bm2_markdup) - cells found by a scan,
 //                        union-find over cells with atomicMin hooking and pointer jumping, side neighbours by extremes, diagonal ones by a
 //                        binary search per member
 //   bm2_dup_set          the duplicate bitset, kept on the context for bm2_bam_sort_compress_ex (bam_sort.cu)
@@ -204,14 +205,23 @@ __global__ void dup_optical_flag_kernel(const bm2_dup_loc_entry *__restrict__ s,
     flag[i] = (sz > 32 && sz <= DUP_OPTICAL_MAX_SET && s[i].e.kind == DUP_KIND_PAIR && (s[i].loc & DUP_LOC_HAS)) ? 1 : 0;
 }
 
-// the cell sort's key of each member at its place in the current order: 0 x, 1 (cx, cy), 2 (group, class, tile)
+// the cell sort's key of each member at its place in the current order: 0 x, 1 (cx, cy), 2 (group, class, tile), 3 read group
 __global__ void dup_cell_field_kernel(const bm2_dup_loc_entry *__restrict__ s, const int32_t *__restrict__ seg, const uint32_t *__restrict__ idx,
                                       int64_t m, int field, int64_t d, uint64_t *keys) {
     const int64_t p = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= m) return;
     const uint32_t i = idx[p];
     const bm2_dup_loc_entry &e = s[i];
-    keys[p] = field == 0 ? (uint64_t) ((uint32_t) e.x ^ 0x80000000u) : field == 1 ? dup_cell_lo(e, d) : dup_cell_hi((uint32_t) (seg[i] - 1), e);
+    keys[p] = field == 0 ? (uint64_t) ((uint32_t) e.x ^ 0x80000000u) : field == 1 ? dup_cell_lo(e, d) : field == 2 ? dup_cell_hi((uint32_t) (seg[i] - 1), e)
+                                                                                                                   : (uint64_t) dup_loc_rg(e.loc);
+}
+
+// the OR of the exact pass's members' read groups (0 for bm2_mem's entries, whose cell sort then skips the read-group pass)
+__global__ void dup_cell_rg_or_kernel(const bm2_dup_loc_entry *__restrict__ s, const uint8_t *__restrict__ flag, int64_t n, unsigned *rg_or) {
+    const int64_t p = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
+    unsigned v = p < n && flag[p] ? dup_loc_rg(s[p].loc) : 0u;
+    for (int o = 16; o; o >>= 1) v |= __shfl_xor_sync(kFull, v, o);
+    if ((threadIdx.x & 31) == 0 && v) atomicOr(rg_or, v);
 }
 
 // the members in cell order: their x and y, and a 1 where a cell starts
@@ -223,12 +233,14 @@ __global__ void dup_cell_head_kernel(const bm2_dup_loc_entry *__restrict__ s, co
     mx[p] = e.x; my[p] = e.y;
     if (p == 0) { head[p] = 1; return; }
     const bm2_dup_loc_entry &f = s[idx[p - 1]];
-    head[p] = (dup_cell_hi((uint32_t) (seg[idx[p]] - 1), e) != dup_cell_hi((uint32_t) (seg[idx[p - 1]] - 1), f) || dup_cell_lo(e, d) != dup_cell_lo(f, d)) ? 1 : 0;
+    head[p] = (dup_cell_hi((uint32_t) (seg[idx[p]] - 1), e) != dup_cell_hi((uint32_t) (seg[idx[p - 1]] - 1), f) || dup_loc_rg(e.loc) != dup_loc_rg(f.loc) ||
+               dup_cell_lo(e, d) != dup_cell_lo(f, d)) ? 1 : 0;
 }
 
-// per cell (cell = 1-based numbers from the scan of the heads): its first member, its keys, its own root, and its y range reset
+// per cell (cell = 1-based numbers from the scan of the heads): its first member, its keys and read group, its own root, and its y range reset
 __global__ void dup_cell_init_kernel(const bm2_dup_loc_entry *__restrict__ s, const int32_t *__restrict__ seg, const uint32_t *__restrict__ idx,
-                                     const int32_t *__restrict__ cell, int64_t m, int64_t d, int32_t *cstart, uint64_t *ckey, int32_t *parent, int32_t *cy) {
+                                     const int32_t *__restrict__ cell, int64_t m, int64_t d, int32_t *cstart, uint64_t *ckey, uint32_t *crg, int32_t *parent,
+                                     int32_t *cy) {
     const int64_t p = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= m) return;
     if (p == m - 1) cstart[cell[p]] = (int32_t) m;
@@ -236,7 +248,7 @@ __global__ void dup_cell_init_kernel(const bm2_dup_loc_entry *__restrict__ s, co
     const int32_t c = cell[p] - 1;
     const bm2_dup_loc_entry &e = s[idx[p]];
     cstart[c] = (int32_t) p; parent[c] = c;
-    ckey[2 * c] = dup_cell_hi((uint32_t) (seg[idx[p]] - 1), e); ckey[2 * c + 1] = dup_cell_lo(e, d);
+    ckey[2 * c] = dup_cell_hi((uint32_t) (seg[idx[p]] - 1), e); ckey[2 * c + 1] = dup_cell_lo(e, d); crg[c] = dup_loc_rg(e.loc);
     cy[2 * c] = INT32_MAX; cy[2 * c + 1] = INT32_MIN;
 }
 
@@ -255,13 +267,15 @@ __global__ void dup_cell_suffix_kernel(const int32_t *__restrict__ cstart, int64
     for (int64_t p = cstart[c + 1] - 1; p >= cstart[c]; --p) { hi = bm2_max(hi, my[p]); lo = bm2_min(lo, my[p]); suf[p] = hi; suf[m + p] = lo; }
 }
 
-__device__ __forceinline__ int64_t dup_find_cell(const uint64_t *__restrict__ ckey, int64_t nc, uint64_t hi, uint64_t lo) {
+// the cell with keys (hi, rg, lo), the cells' sort order, or -1
+__device__ __forceinline__ int64_t dup_find_cell(const uint64_t *__restrict__ ckey, const uint32_t *__restrict__ crg, int64_t nc, uint64_t hi, uint32_t rg,
+                                                 uint64_t lo) {
     int64_t a = 0, b = nc;
     while (a < b) {
         const int64_t k = (a + b) / 2;
-        if (ckey[2 * k] < hi || (ckey[2 * k] == hi && ckey[2 * k + 1] < lo)) a = k + 1; else b = k;
+        if (ckey[2 * k] < hi || (ckey[2 * k] == hi && (crg[k] < rg || (crg[k] == rg && ckey[2 * k + 1] < lo)))) a = k + 1; else b = k;
     }
-    return a < nc && ckey[2 * a] == hi && ckey[2 * a + 1] == lo ? a : -1;
+    return a < nc && ckey[2 * a] == hi && crg[a] == rg && ckey[2 * a + 1] == lo ? a : -1;
 }
 
 __device__ __forceinline__ int32_t dup_root(const int32_t *parent, int32_t c) { while (parent[c] != c) c = parent[c]; return c; }
@@ -276,24 +290,25 @@ __device__ __forceinline__ void dup_hook(int32_t *parent, int32_t a, int32_t b, 
 // one round of hooking: member p of cell B tests the cells behind B diagonally; B's first member also tests the side neighbours (cx - 1, cy)
 // and (cx, cy - 1) by the cells' extremes.  Roots only move to smaller cells, so every round with a change leaves fewer components.
 __global__ void dup_cell_link_kernel(const int32_t *__restrict__ cell, const int32_t *__restrict__ cstart, const uint64_t *__restrict__ ckey,
-                                     const int32_t *__restrict__ cy, const int32_t *__restrict__ mx, const int32_t *__restrict__ my,
+                                     const uint32_t *__restrict__ crg, const int32_t *__restrict__ cy, const int32_t *__restrict__ mx, const int32_t *__restrict__ my,
                                      const int32_t *__restrict__ suf, int64_t m, int64_t nc, int64_t d, int32_t *parent, int32_t *changed) {
     const int64_t p = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= m) return;
     const int32_t c = cell[p] - 1;
     const uint64_t hi = ckey[2 * c], lo = ckey[2 * c + 1];
+    const uint32_t rg = crg[c];
     const uint32_t x = (uint32_t) (lo >> 32), y = (uint32_t) lo;
     const uint64_t left = (uint64_t) (x - 1) << 32;        // unused when x == 0: no cell to the left
     if (p == cstart[c]) {
-        const int64_t a = x ? dup_find_cell(ckey, nc, hi, left | y) : -1;
+        const int64_t a = x ? dup_find_cell(ckey, crg, nc, hi, rg, left | y) : -1;
         if (a >= 0 && (int64_t) mx[cstart[a + 1] - 1] >= (int64_t) mx[p] - d) dup_hook(parent, (int32_t) a, c, changed);
-        const int64_t b = y ? dup_find_cell(ckey, nc, hi, (uint64_t) x << 32 | (y - 1)) : -1;
+        const int64_t b = y ? dup_find_cell(ckey, crg, nc, hi, rg, (uint64_t) x << 32 | (y - 1)) : -1;
         if (b >= 0 && (int64_t) cy[2 * b + 1] >= (int64_t) cy[2 * c] - d) dup_hook(parent, (int32_t) b, c, changed);
     }
     for (int k = 0; k < 2 && x; ++k) {
         const bool below = k == 0;
         if (below ? y == 0 : y == 0xFFFFFFFFu) continue;
-        const int64_t a = dup_find_cell(ckey, nc, hi, left | (below ? y - 1 : y + 1));
+        const int64_t a = dup_find_cell(ckey, crg, nc, hi, rg, left | (below ? y - 1 : y + 1));
         if (a < 0) continue;
         const int32_t s0 = cstart[a];
         if (dup_cell_diag_linked(mx + s0, suf + (below ? 0 : m) + s0, cstart[a + 1] - s0, mx[p], my[p], d, below)) dup_hook(parent, (int32_t) a, c, changed);
@@ -314,7 +329,9 @@ __global__ void dup_cell_roots_kernel(const int32_t *__restrict__ parent, int64_
 enum { DD_IN, DD_STARTS, DD_TFIRST, DD_TID, DD_PAIR, DD_FRAG, DD_OUT, DD_CNT, DD_TEMP, DD_KEYS0, DD_KEYS1, DD_ORD0, DD_ORD1, DD_SORTED,
        // bm2_dup_resolve_ex: the located entries as given and sorted, group starts; the exact pass's members (flags, compacted ids, x / y,
        // suffix extremes of y, cell numbers) and cells (first members, keys, y ranges, roots)
-       DD_LOC_IN, DD_LOC_SORTED, DD_GSTART, DD_OPT_FLAG, DD_OPT_IDX, DD_MXY, DD_SUF, DD_CELL, DD_CSTART, DD_CKEY, DD_CY, DD_PARENT, DD_END };
+       DD_LOC_IN, DD_LOC_SORTED, DD_GSTART, DD_OPT_FLAG, DD_OPT_IDX, DD_MXY, DD_SUF, DD_CELL, DD_CSTART, DD_CKEY, DD_CY, DD_PARENT,
+       DD_CRG,                          // the cells' read groups
+       DD_END };
 static_assert(DD_END == std::extent<decltype(bm2_ctx::dup_d)>::value, "bm2_ctx::dup_d: one buffer per slot");
 // bm2_dup_resolve reuses the signature slots: entries in DD_PAIR, group numbers / flags / ids in DD_IN / DD_STARTS / DD_TFIRST / DD_TID / DD_FRAG
 
@@ -421,7 +438,8 @@ int optical_pass(bm2_ctx *ctx, const bm2_dup_loc_entry *S, const int32_t *head, 
     const unsigned g = (unsigned) ((n + 255) / 256);
     int32_t *gstart = (int32_t *) b[DD_GSTART].p;
     unsigned long long *cnt = (unsigned long long *) ((uint8_t *) b[DD_CNT].p + 16);   // [0] small-group count, [1] roots of the exact pass
-    BM2_CUDA_OK(cudaMemsetAsync(cnt, 0, 16, st));
+    unsigned *rg_or = (unsigned *) ((uint8_t *) b[DD_CNT].p + 12);
+    BM2_CUDA_OK(cudaMemsetAsync(rg_or, 0, 20, st));
     dup_gstart_kernel<<<g, 256, 0, st>>>(head, seg, n, gstart);
     BM2_CUDA_OK(cudaGetLastError());
     dup_optical_small_kernel<<<(unsigned) ((groups * 32 + 255) / 256), 256, 0, st>>>(S, gstart, groups, d, cnt);
@@ -429,34 +447,40 @@ int optical_pass(bm2_ctx *ctx, const bm2_dup_loc_entry *S, const int32_t *head, 
     uint8_t *flag = (uint8_t *) b[DD_OPT_FLAG].p;
     dup_optical_flag_kernel<<<g, 256, 0, st>>>(S, seg, gstart, n, flag);
     BM2_CUDA_OK(cudaGetLastError());
+    dup_cell_rg_or_kernel<<<g, 256, 0, st>>>(S, flag, n, rg_or);
+    BM2_CUDA_OK(cudaGetLastError());
     uint32_t *ord0 = (uint32_t *) b[DD_ORD0].p;
     size_t tb = b[DD_TEMP].cap;
     BM2_CUDA_OK(cub::DeviceSelect::Flagged(b[DD_TEMP].p, tb, cub::CountingInputIterator<uint32_t>(0), flag, ord0, (int64_t *) b[DD_CNT].p, (int) n, st));
     int64_t m = 0;
+    unsigned rgs = 0;
     BM2_CUDA_OK(cudaMemcpyAsync(&m, b[DD_CNT].p, 8, cudaMemcpyDeviceToHost, st));
+    BM2_CUDA_OK(cudaMemcpyAsync(&rgs, rg_or, 4, cudaMemcpyDeviceToHost, st));
     BM2_CUDA_OK(cudaStreamSynchronize(st));
     unsigned long long small = 0, roots = 0;
     if (m) {
         const unsigned gm = (unsigned) ((m + 255) / 256);
         cub::DoubleBuffer<uint64_t> kb((uint64_t *) b[DD_KEYS0].p, (uint64_t *) b[DD_KEYS1].p);
         cub::DoubleBuffer<uint32_t> vb(ord0, (uint32_t *) b[DD_ORD1].p);
-        for (int f = 0; f < 3; ++f) {                    // x, then (cx, cy), then (group, class, tile): each pass stable
+        for (int f : { 0, 1, 3, 2 }) {                   // x, (cx, cy), read group, (group, class, tile): each pass stable
+            if (f == 3 && !rgs) continue;
             dup_cell_field_kernel<<<gm, 256, 0, st>>>(S, seg, vb.Current(), m, f, d, kb.Current());
             BM2_CUDA_OK(cudaGetLastError());
             tb = b[DD_TEMP].cap;
-            BM2_CUDA_OK(cub::DeviceRadixSort::SortPairs(b[DD_TEMP].p, tb, kb, vb, (int) m, 0, f ? 64 : 32, st));
+            BM2_CUDA_OK(cub::DeviceRadixSort::SortPairs(b[DD_TEMP].p, tb, kb, vb, (int) m, 0, f == 0 ? 32 : f == 3 ? bits_of(rgs) : 64, st));
         }
         const uint32_t *idx = vb.Current();
         int32_t *mx = (int32_t *) b[DD_MXY].p, *my = mx + m, *cell = (int32_t *) b[DD_CELL].p, *cstart = (int32_t *) b[DD_CSTART].p;
         int32_t *parent = (int32_t *) b[DD_PARENT].p, *cy = (int32_t *) b[DD_CY].p, *suf = (int32_t *) b[DD_SUF].p;
         uint64_t *ckey = (uint64_t *) b[DD_CKEY].p;
+        uint32_t *crg = (uint32_t *) b[DD_CRG].p;
         dup_cell_head_kernel<<<gm, 256, 0, st>>>(S, seg, idx, m, d, parent, mx, my);    // the heads in parent, for the scan
         BM2_CUDA_OK(cudaGetLastError());
         tb = b[DD_TEMP].cap;
         BM2_CUDA_OK(cub::DeviceScan::InclusiveSum(b[DD_TEMP].p, tb, (const int32_t *) parent, cell, (int) m, st));
         int32_t nc32 = 0;
         BM2_CUDA_OK(cudaMemcpyAsync(&nc32, cell + m - 1, 4, cudaMemcpyDeviceToHost, st));
-        dup_cell_init_kernel<<<gm, 256, 0, st>>>(S, seg, idx, cell, m, d, cstart, ckey, parent, cy);
+        dup_cell_init_kernel<<<gm, 256, 0, st>>>(S, seg, idx, cell, m, d, cstart, ckey, crg, parent, cy);
         BM2_CUDA_OK(cudaGetLastError());
         dup_cell_y_kernel<<<gm, 256, 0, st>>>(cell, my, m, cy);
         BM2_CUDA_OK(cudaGetLastError());
@@ -468,7 +492,7 @@ int optical_pass(bm2_ctx *ctx, const bm2_dup_loc_entry *S, const int32_t *head, 
         int32_t *changed = (int32_t *) ((uint8_t *) b[DD_CNT].p + 8);
         for (int32_t ch = 1; ch;) {
             BM2_CUDA_OK(cudaMemsetAsync(changed, 0, 4, st));
-            dup_cell_link_kernel<<<gm, 256, 0, st>>>(cell, cstart, ckey, cy, mx, my, suf, m, nc, d, parent, changed);
+            dup_cell_link_kernel<<<gm, 256, 0, st>>>(cell, cstart, ckey, crg, cy, mx, my, suf, m, nc, d, parent, changed);
             BM2_CUDA_OK(cudaGetLastError());
             dup_cell_jump_kernel<<<gc, 256, 0, st>>>(parent, nc);
             BM2_CUDA_OK(cudaGetLastError());
@@ -530,7 +554,7 @@ int dup_resolve(bm2_ctx *ctx, const bm2_dup_entry *entries, const bm2_dup_loc_en
                           ctx->ensure(b[DD_MXY], (size_t) n * 8 + 8) || ctx->ensure(b[DD_SUF], (size_t) n * 8 + 8) ||
                           ctx->ensure(b[DD_CELL], (size_t) n * 4 + 8) || ctx->ensure(b[DD_CSTART], (size_t) n * 4 + 8) ||
                           ctx->ensure(b[DD_CKEY], (size_t) n * 16 + 8) || ctx->ensure(b[DD_CY], (size_t) n * 8 + 8) ||
-                          ctx->ensure(b[DD_PARENT], (size_t) n * 4 + 8))) return 1;
+                          ctx->ensure(b[DD_PARENT], (size_t) n * 4 + 8) || ctx->ensure(b[DD_CRG], (size_t) n * 4 + 8))) return 1;
     ctx->dup_resolve_ms = 0;
     ctx->dup_sorted.clear(); ctx->dup_lsorted.clear(); ctx->dup_ids.clear();
     if (n_optical) *n_optical = 0;

@@ -26,7 +26,9 @@
 //               the same tile, |x1-x2| <= d and |y1-y2| <= d (in 64 bits); the count is the sum over the connected components of size - 1,
 //               a member without a location being a component of its own.  This is the count of Picard's graph path and of its small-set
 //               path, wherever the keeper sits.  It is at most the group's duplicates (size - 1).  Larger groups and fragment groups: 0.
-//   cells       (the exact pass of groups larger than a warp, markdup.cu) members of one class and tile binned by (floor(x / (d+1)),
+//   read group  (bm2_markdup) loc's bits 2 and up hold the pair's read-group index (DUP_LOC_RG_SHIFT); dup_optical_linked compares the whole
+//               loc, so members of different read groups are never linked.  bm2_mem's entries have 0 there.
+//   cells       (the exact pass of groups larger than a warp, markdup.cu) members of one class, tile and read group binned by (floor(x / (d+1)),
 //               floor(y / (d+1))): two members of a cell are always linked, so a cell is one component, and only the four neighbouring cells
 //               behind a cell need tests - side neighbours by the cells' extreme x or y alone, diagonal ones per member by a binary search
 //               in the x-sorted neighbour and its suffix extreme of y (dup_cell_diag_linked).
@@ -156,6 +158,8 @@ BM2_HD uint64_t dup_score_key(int32_t score) { return (uint64_t) (32767 - score)
 
 // ---- optical duplicates ----
 enum { DUP_LOC_HAS = 1, DUP_LOC_REV = 2 };
+constexpr int DUP_LOC_RG_SHIFT = 2;
+BM2_HD uint32_t dup_loc_rg(int32_t loc) { return (uint32_t) loc >> DUP_LOC_RG_SHIFT; }
 constexpr int64_t DUP_OPTICAL_MAX_SET = 300000;          // Picard's MAX_OPTICAL_DUPLICATE_SET_SIZE
 
 // Picard's rapidParseInt of p[0..len): an optional leading '-', then the decimal digits up to the first non-digit, accumulated as a Java int
@@ -220,4 +224,29 @@ BM2_HD bool dup_cell_diag_linked(const int32_t *ax, const int32_t *suf, int64_t 
     while (lo < hi) { const int64_t m = (lo + hi) / 2; if ((int64_t) ax[m] < (int64_t) bx - d) lo = m + 1; else hi = m; }
     if (lo == n) return false;
     return below ? (int64_t) suf[lo] >= (int64_t) by - d : (int64_t) suf[lo] <= (int64_t) by + d;
+}
+
+// ---- mate pairing (bm2_markdup) ----
+// a QNAME's hash: 64-bit FNV-1a over its bytes
+BM2_HD uint64_t dup_name_hash(const uint8_t *name, int len) {
+    uint64_t h = 14695981039346656037ull;
+    for (int i = 0; i < len; ++i) { h ^= name[i]; h *= 1099511628211ull; }
+    return h;
+}
+
+// one run [a, b) of the halves sorted by (hash, read group, index): ord[i] the index of the i-th.  Each half is joined to the first earlier
+// half of the run that is still unjoined and whose name equals its own byte for byte; partner[] gets both indices (-1: unjoined).  This is
+// a table keyed by the whole name, visited in index order, so equal hashes of different names never join.
+BM2_HD void dup_pair_run(const bm2_markdup_half *h, const uint32_t *ord, int64_t a, int64_t b, const uint8_t *names, int32_t *partner) {
+    for (int64_t i = a; i < b; ++i) partner[ord[i]] = -1;
+    for (int64_t i = a + 1; i < b; ++i) {
+        const bm2_markdup_half &u = h[ord[i]];
+        for (int64_t j = a; j < i; ++j) {
+            if (partner[ord[j]] != -1) continue;
+            const bm2_markdup_half &v = h[ord[j]];
+            bool same = u.name_len == v.name_len;
+            for (int32_t k = 0; same && k < u.name_len; ++k) same = names[u.name_off + k] == names[v.name_off + k];
+            if (same) { partner[ord[j]] = (int32_t) ord[i]; partner[ord[i]] = (int32_t) ord[j]; break; }
+        }
+    }
 }

@@ -499,7 +499,8 @@ int  bm2_bam_sort_compress_ex(bm2_ctx *ctx, const uint8_t *recs, int64_t n, cons
  *   optical   in a pair group of 2 .. 300000 members, two members are linked when both have a location, the same class and tile, and
  *             |x1 - x2| <= d and |y1 - y2| <= d (in 64 bits); the group's optical count is the sum over the connected components of
  *             size - 1, a member without a location being a component of its own.  Larger groups and fragment groups have none.
- * loc: bit 0 set when the template has a location, bit 1 its class (1: reverse); tile, x, y are 0 without a location. */
+ * loc: bit 0 set when the template has a location, bit 1 its class (1: reverse), bits 2 and up a read-group index (0 from bm2_mem; bm2_markdup
+ * sets it, and members of different read groups are never linked); tile, x, y are 0 without a location. */
 typedef struct { bm2_dup_entry e; int32_t tile, x, y, loc; } bm2_dup_loc_entry;
 /* bm2_dup_signatures, with the pair entries located.  counts[0] gets the chunk's records with 0x100 or 0x800, counts[1] its primary records
  * with 0x4.  The entries are bm2_dup_signatures's (pairs[i].e), in the same order. */
@@ -577,6 +578,47 @@ int  bm2_last_bqsr_apply_stats(bm2_ctx *ctx, bm2_bqsr_apply_stats_t *out);
 /* Device bytes bm2_bqsr_apply needs for windows of window_bytes of records of about 300 bytes with n_rg read groups' tables, and the bytes
  * free on ctx's device now. */
 int  bm2_bqsr_apply_memory(const bm2_ctx *ctx, int64_t window_bytes, int32_t n_rg, int64_t *needed, int64_t *free_bytes);
+
+/* ---- Duplicate marking of coordinate-sorted BAM files (bm2_markdup) ---------------------------------------------------------------------
+ * The rule (csrc/markdup_device.cuh, the host half csrc/markdup_bam.h) restates Picard MarkDuplicates on coordinate-sorted input at its
+ * defaults, over the merged records of one or more files; byte equality with Picard is not claimed.  The GPU computes each record's part of
+ * it; the mates are paired and the entries resolved (bm2_dup_resolve, bm2_dup_resolve_ex) on the host's side of this ABI. */
+enum { BM2_MDB_NONE = 0,           /* no entry: a secondary or supplementary record, or an unmapped primary of no pair */
+       BM2_MDB_FRAG = 1,           /* a mapped primary without 0x1, or with 0x8: a fragment */
+       BM2_MDB_HALF = 2,           /* a mapped primary with 0x1 and without 0x8: half of a pair */
+       BM2_MDB_UNMAPPED_HALF = 3   /* an unmapped primary with 0x1 and without 0x8 (its mate must not claim 0x8 is unset for it) */ };
+/* One record: kind; rg, the index of its RG:Z value among bm2_markdup_set's IDs (n_ids without the tag, -1 for a value that is no ID); lib,
+ * its library index (unknown_lib without the tag or with a value that is no ID).  A mapped primary: end (dup_end_key) and score (at most
+ * 16383); a half (mapped or not) also hash, the 64-bit FNV-1a hash of its QNAME, and a mapped half its location: loc DUP_LOC_HAS or 0,
+ * tile, x, y (0 without a location) from its QNAME. */
+typedef struct { uint64_t end, hash; int32_t score, kind, rg, lib, tile, x, y, loc; } bm2_markdup_rec;   /* 48 bytes */
+/* A half of a pair for bm2_markdup_pair: its QNAME's hash (a half's hash from bm2_markdup_records), read group, and its name's bytes at
+ * name_off of the names buffer. */
+typedef struct { uint64_t hash; int32_t rg, name_len; int64_t name_off; } bm2_markdup_half;
+typedef struct { double records_ms, pair_ms, mark_ms, bgzf_ms; } bm2_markdup_stats_t;
+/* The merged header's read groups: ids[i] (n_ids of them, at most 32 KiB with 16 bytes each) belongs to library libs[i] (< n_lib);
+ * unknown_lib is the library of records without a known read group.  Zeroes the per-library counts and the times. */
+int  bm2_markdup_set(bm2_ctx *ctx, int32_t n_ids, const char *const *ids, const int32_t *libs, int32_t n_lib, int32_t unknown_lib);
+/* One window of whole records (HOST, contiguous, each where the one before ends), one warp per record: *out (HOST, n_recs, owned by the
+ * context, valid until its next call) gets each record's bm2_markdup_rec.  The per-library counts grow by the window's records. */
+int  bm2_markdup_records(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int64_t *starts, int64_t n_recs, const bm2_markdup_rec **out);
+/* The halves of one window, in ordinal order (those carried from earlier windows first): stably sorted by (hash, rg) with cub, then in each
+ * run of equal (hash, rg) each half is joined to the first earlier half of the run that is still unjoined and has the same name byte for
+ * byte, so a hash collision never joins two reads.  *partner (HOST, n of them, owned by the context, valid until its next call): the index
+ * of each half's partner, or -1. */
+int  bm2_markdup_pair(bm2_ctx *ctx, const bm2_markdup_half *halves, int64_t n, const uint8_t *names, int64_t names_len, const int32_t **partner);
+/* The counts since bm2_markdup_set: counts[2 lib] records with 0x100 or 0x800, counts[2 lib + 1] unmapped primaries (2 n_lib values). */
+int  bm2_markdup_counts(bm2_ctx *ctx, int64_t *counts);
+/* One window of the second pass: record i is the merged stream's record first + i; its 0x400 is set when that bit of the bitset of bm2_dup_set
+ * is set and cleared otherwise.  The stream carry + records is then compressed as bm2_bqsr_apply compresses it (out, carry and index data
+ * alike). */
+int  bm2_markdup_mark(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int64_t *starts, int64_t n_recs, int64_t first, const uint8_t *carry,
+                      int64_t carry_len, int last, bm2_sort_out *out);
+/* Device ms (CUDA events) since bm2_markdup_set: the record kernel, the pairing (sort and runs), the flag kernel, BGZF of the second pass. */
+int  bm2_last_markdup_stats(const bm2_ctx *ctx, bm2_markdup_stats_t *out);
+/* Device bytes bm2_markdup_records and bm2_markdup_mark need for windows of window_bytes of records of about 300 bytes, and the bytes free on
+ * ctx's device now.  The duplicate bitset and the resolve's buffers come on top. */
+int  bm2_markdup_memory(const bm2_ctx *ctx, int64_t window_bytes, int64_t *needed, int64_t *free_bytes);
 
 /* ---- Whole-genome coverage metrics (bm2_wgsmetrics) ----------------------------------------------------------------------------------
  * The rule (csrc/wgs_device.cuh, csrc/wgs_metrics.h) restates Picard CollectWgsMetrics at its defaults (USE_FAST_ALGORITHM=false, no
