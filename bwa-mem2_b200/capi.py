@@ -232,6 +232,13 @@ class BqsrApplyStats(C.Structure):
                 ("kept_records", C.c_int64), ("err_kind", C.c_int32), ("err_index", C.c_int64), ("err_name", C.c_char_p)]
 
 
+# bm2_recal_set (include/bm2_b200.h)
+class RecalSet(C.Structure):
+    _fields_ = [("n_contigs", C.c_int32), ("contig_off", C.c_void_p), ("contig_len", C.c_void_p), ("l_pac", C.c_int64), ("pac", C.c_void_p),
+                ("holes", C.c_void_p), ("n_holes", C.c_int64), ("covered", C.c_void_p), ("junction", C.c_void_p), ("n_ids", C.c_int32),
+                ("ids", C.c_void_p), ("id_cov", C.c_void_p), ("n_cov", C.c_int32)]
+
+
 # bm2_wgs_set / bm2_wgs_finish (include/bm2_b200.h)
 class WgsParams(C.Structure):
     _fields_ = [("min_mapq", C.c_int32), ("min_baseq", C.c_int32), ("coverage_cap", C.c_int32), ("count_unpaired", C.c_int32)]
@@ -263,7 +270,7 @@ EXPORTS = ["bm2_create_sibling", "bm2_fastq_encode", "bm2_seq_encode", "bm2_fast
            "bm2_bqsr_sites", "bm2_bqsr_count", "bm2_bqsr_tables", "bm2_bqsr_apply_set", "bm2_bqsr_apply", "bm2_last_bqsr_apply_stats",
            "bm2_bqsr_apply_memory", "bm2_wgs_set", "bm2_wgs_memory", "bm2_wgs_add", "bm2_wgs_finish",
            "bm2_mm_set", "bm2_mm_memory", "bm2_mm_add", "bm2_mm_finish", "bm2_markdup_set", "bm2_markdup_records", "bm2_markdup_pair", "bm2_markdup_counts",
-           "bm2_markdup_mark", "bm2_last_markdup_stats", "bm2_markdup_memory"]
+           "bm2_markdup_mark", "bm2_last_markdup_stats", "bm2_markdup_memory", "bm2_recal_memory", "bm2_recal_set", "bm2_recal_add", "bm2_recal_tables"]
 
 _lib = None
 
@@ -729,6 +736,51 @@ class Context:
         self._check(f(self._ctx, C.byref(t)), "bm2_bqsr_tables")
         out = dict(reads=t.reads, bases=t.bases, ms=t.ms, err_kind=t.err_kind, err_index=t.err_index,
                    err_name=(t.err_name or b"").decode(), read_group=(t.read_group or b"").decode())
+        for k, shape in (("qual", (BQSR_NQ,)), ("ctx", (BQSR_NQ, BQSR_NCTX)), ("cyc", (BQSR_NQ, BQSR_NCYC))):
+            for s in ("obs", "err"):
+                out[k + "_" + s] = _host(getattr(t, k + "_" + s), int(np.prod(shape)), np.int64).reshape(shape)
+        return out
+
+    def recal_memory(self, l_pac: int, window_bytes: int, n_cov: int):
+        """bm2_recal_memory -> (bytes needed, bytes free)."""
+        need, free = C.c_int64(), C.c_int64()
+        f = lib().bm2_recal_memory
+        f.argtypes = [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p]
+        self._check(f(self._ctx, int(l_pac), int(window_bytes), int(n_cov), C.byref(need), C.byref(free)), "bm2_recal_memory")
+        return need.value, free.value
+
+    def recal_set(self, contig_off, contig_len, l_pac: int, pac, holes, covered, junction, ids, id_cov, n_cov: int):
+        """bm2_recal_set: the contigs, the packed reference ((l_pac + 3) // 4 bytes), the .amb holes ([beg, end) pairs), the known-site bitsets
+        (uint64 words), the @RG IDs with each one's covariate, and the covariate count; zeroes the counts."""
+        self._recal_keep = [np.ascontiguousarray(contig_off, np.int64), np.ascontiguousarray(contig_len, np.int32), np.ascontiguousarray(pac, np.uint8),
+                            np.ascontiguousarray(holes, np.int64).reshape(-1), np.ascontiguousarray(covered, np.uint64),
+                            np.ascontiguousarray(junction, np.uint64), np.ascontiguousarray(list(id_cov) + [0], np.int32)]
+        off, ln, pb, h, cov, jun, ic = self._recal_keep
+        names = (C.c_char_p * max(len(ids), 1))(*[i.encode() for i in ids])
+        self._recal_keep.append(names)
+        s = RecalSet(len(off), off.ctypes.data, ln.ctypes.data, int(l_pac), pb.ctypes.data, h.ctypes.data if len(h) else None, len(h) // 2,
+                     cov.ctypes.data, jun.ctypes.data, len(ids), C.cast(names, C.c_void_p) if ids else None, ic.ctypes.data, int(n_cov))
+        f = lib().bm2_recal_set
+        f.argtypes = [C.c_void_p, C.c_void_p]
+        self._check(f(self._ctx, C.byref(s)), "bm2_recal_set")
+
+    def recal_add(self, data: bytes, starts):
+        """bm2_recal_add: one window of records (uncompressed BAM at starts, any order).  A read error raises Bm2Error naming the read (the
+        tables still report it)."""
+        starts = np.ascontiguousarray(starts, np.int64)
+        buf = np.frombuffer(data, np.uint8) if len(data) else np.zeros(1, np.uint8)
+        sb = starts if len(starts) else np.zeros(1, np.int64)
+        f = lib().bm2_recal_add
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64]
+        self._check(f(self._ctx, buf.ctypes.data, len(data), sb.ctypes.data, len(starts)), "bm2_recal_add")
+
+    def recal_tables(self, cov: int):
+        """bm2_recal_tables -> bqsr_tables's dict for covariate cov (read_group empty)."""
+        t = BqsrTables()
+        f = lib().bm2_recal_tables
+        f.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
+        self._check(f(self._ctx, int(cov), C.byref(t)), "bm2_recal_tables")
+        out = dict(reads=t.reads, bases=t.bases, ms=t.ms, err_kind=t.err_kind, err_index=t.err_index, err_name=(t.err_name or b"").decode())
         for k, shape in (("qual", (BQSR_NQ,)), ("ctx", (BQSR_NQ, BQSR_NCTX)), ("cyc", (BQSR_NQ, BQSR_NCYC))):
             for s in ("obs", "err"):
                 out[k + "_" + s] = _host(getattr(t, k + "_" + s), int(np.prod(shape)), np.int64).reshape(shape)

@@ -156,6 +156,17 @@ struct bm2_ctx {
     std::vector<int32_t> mdb_partner;
     std::vector<uint8_t> mdb_carry;
     std::vector<bm2_sort_rec> mdb_srecs;
+    // bm2_recal_set / bm2_recal_add / bm2_recal_tables (recal.cu): buffers, whether a reference is set, the contigs' lengths, the reference's
+    // size and holes, the map and covariates, events, the device time and records seen since, the first read error (kind 0: none), the last tables
+    DevBuf rcl_d[10];
+    bool rcl_set = false;
+    std::vector<int32_t> rcl_contig_len;
+    int64_t rcl_l_pac = 0, rcl_n_holes = 0, rcl_map_bytes = 0, rcl_seen = 0, rcl_err_index = -1;
+    int rcl_n_ids = 0, rcl_n_cov = 0, rcl_err_kind = 0;
+    cudaEvent_t rcl_ev[2] = {nullptr, nullptr};
+    double rcl_ms = 0;
+    std::string rcl_err_name;
+    std::vector<int64_t> rcl_tables;
 
     int ensure(DevBuf &b, size_t bytes);
     int ensure_host(HostBuf &b, size_t bytes);
@@ -163,7 +174,7 @@ struct bm2_ctx {
         std::vector<DevBuf *> v = {&io_pairs, &io_ref, &io_qer, &bsw_jobs, &bsw_outs, &bsw_scratch, &dup_bits};
         append(v, pipe_d); append(v, cigar_d); append(v, sam_d); append(v, ksw_d); append(v, fq_d);
         append(v, bgzf_d); append(v, sort_d); append(v, dup_d); append(v, bqsr_d); append(v, bqa_d); append(v, wgs_d);
-        append(v, mm_d); append(v, mdb_d);
+        append(v, mm_d); append(v, mdb_d); append(v, rcl_d);
         return v;
     }
     std::vector<HostBuf *> all_host() {
@@ -177,6 +188,11 @@ struct bm2_ctx {
 // bgzf.cu: the members of the nb blocks [starts[b], starts[b+1]) of the device bytes d_in, on ctx's stream (the body of bm2_bgzf_compress),
 // gathered into *gather (nullptr: the context's own buffer) before they are copied to the host
 int bgzf_compress_device(bm2_ctx *ctx, const uint8_t *d_in, const int64_t *starts, int64_t nb, const uint8_t **out, int64_t *out_len, DevBuf *gather);
+// bqsr.cu: bqsr_count_kernel over the n records at d_base + d_starts[i] (device), enqueued on st: n_cov covariates of kBqsrCounts counters
+// each at cnt, the read-group map (n_ids entries, map_bytes; n_ids 0: no lookup, covariate 0), the first read error's word into err
+struct BqsrView;
+int bqsr_count_launch(bm2_ctx *ctx, const uint8_t *d_base, const int64_t *d_starts, int64_t n, const BqsrView &v, const void *d_map, int map_bytes,
+                      int n_ids, int n_cov, unsigned long long *cnt, unsigned long long *err, int64_t first, cudaStream_t st);
 // bqsr.cu: the covariate counts of the n records at d_base + d_starts[i] (device), enqueued on st; then, once st has finished,
 // bqsr_count_done adds the device time and returns 1 (the context's error set, naming the read) when one of these records is a read error
 int bqsr_count_device(bm2_ctx *ctx, const uint8_t *d_base, const int64_t *d_starts, int64_t n, cudaStream_t st);

@@ -6,7 +6,7 @@
 //                         bm2_sort_rec index data are what SortedWriter and BaiBuilder take
 //   bm2_last_bqsr_apply_stats  device times, counts and the first read error since the tables came
 // The kernel: one warp per record, grid-stride.  The read-group map (each @RG ID and its table index) sits in shared memory.  Lane 0 finds
-// the RG:Z value in the aux data and the lanes compare it against 32 IDs at a time; ballots over the qualities find the low-quality tails
+// the RG:Z value in the aux data and the lanes compare it against 32 IDs at a time (bqsr_rg_lookup); ballots over the qualities find the low-quality tails
 // and the qualities above 93; then the lanes take consecutive bases, each computing its context and cycle (bqsr_covariates, shared with
 // the counting kernel), reading its deltas and writing its quality in place.  The contexts read bases, not qualities, so the writes do not
 // disturb the other lanes.  The D_cyc table (94 x 1001 doubles per read group) is read from global memory through L2.
@@ -32,7 +32,6 @@ __global__ void __launch_bounds__(kWarps * 32) bqsr_apply_kernel(uint8_t *__rest
     extern __shared__ int4 s_map[];
     for (int i = threadIdx.x; i < map_bytes / 16; i += blockDim.x) s_map[i] = map[i];
     __syncthreads();
-    const uint8_t *s_bytes = (const uint8_t *) s_map;
     const int lane = threadIdx.x & 31;
     unsigned long long changed = 0, recal = 0, kept = 0;
     for (int64_t w = (int64_t) blockIdx.x * kWarps + (threadIdx.x >> 5); w < n; w += (int64_t) gridDim.x * kWarps) {
@@ -41,19 +40,8 @@ __global__ void __launch_bounds__(kWarps * 32) bqsr_apply_kernel(uint8_t *__rest
         int32_t len = 0, at = -1;
         if (lane == 0) at = bqsr_aux_rg(rec, &len);
         at = __shfl_sync(kFull, at, 0); len = __shfl_sync(kFull, len, 0);
-        int rg = -1;
-        if (at >= 0)
-            for (int j0 = 0; j0 < n_ids; j0 += 32) {                     // the first ID equal to the tag's value
-                const int j = j0 + lane;
-                bool m = false;
-                if (j < n_ids) {
-                    const int4 e = s_map[j];
-                    m = e.y == len;
-                    for (int k = 0; m && k < len; ++k) m = s_bytes[e.x + k] == rec[at + k];
-                }
-                const unsigned b = __ballot_sync(kFull, m);
-                if (b) { rg = s_map[j0 + __ffs(b) - 1].z; break; }
-            }
+        const int j = at >= 0 ? bqsr_rg_lookup((const BqsrRgEntry *) s_map, n_ids, rec, at, len) : -1;
+        const int rg = j >= 0 ? s_map[j].z : -1;
         BqsrRec r;
         bqsr_apply_prep(rec, r);
         if (rg < 0) r.status = BQSR_KEEP;

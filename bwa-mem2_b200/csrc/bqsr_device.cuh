@@ -10,6 +10,9 @@
 //             soft clips go.  The bases left, [lo, hi) of the read, are the clipped read; an empty one is not counted
 //   errors    a read without qualities (0xff), a clipped read of more than 500 bases, a quality above 93: the record is not counted and
 //             the call reports it
+//   read group  (bm2_baserecalibrator; bm2_mem has one read group and no lookup) a record that passes the filters must have an RG:Z tag whose
+//             value is an @RG ID of the headers (bqsr_rg_lookup), checked before the errors above: a record without the tag, or with a value
+//             that is no ID, is an error; the record counts into the tables of that ID's covariate.  A filtered record's tag is not read.
 //   a base    of the clipped read: aligned (M = X) at reference g, or inserted between g and g + 1.  Skipped when its base is N, its quality
 //             is below 6, or it is a known-site base (aligned: `covered` bit g; inserted: `junction` bit g).  An error when aligned and its
 //             base differs from the reference's (N inside an .amb hole)
@@ -27,17 +30,29 @@
 #define BQSR_MIN_Q 6
 #define BQSR_TAIL_Q 2
 
-enum { BQSR_COUNT = 0, BQSR_FILTERED = 1, BQSR_EMPTY = 2, BQSR_ERR_NOQUAL = 3, BQSR_ERR_CYCLES = 4, BQSR_ERR_QUAL = 5 };
+// the counters of one covariate (bqsr.cu's kernel, bm2_bqsr_tables, bm2_recal_tables): (quality, context) observations and errors, (quality,
+// cycle) observations and errors, reads, bases
+constexpr int kBqsrCxTab = 2 * BQSR_NQ * BQSR_NCTX;
+constexpr int64_t kBqsrCxObs = 0, kBqsrCxErr = BQSR_NQ * BQSR_NCTX, kBqsrCyObs = kBqsrCxTab, kBqsrCyErr = kBqsrCyObs + BQSR_NQ * BQSR_NCYC,
+                  kBqsrReads = kBqsrCyErr + BQSR_NQ * BQSR_NCYC, kBqsrBases = kBqsrReads + 1, kBqsrCounts = kBqsrBases + 1;
+// Up to this many covariates the kernel keeps their (quality, context) tables (23.5 KB each) per CTA in shared memory; above it, in global
+// memory.  Two tables and a full read-group map (kBqsrMapMax) take 79 KB, two CTAs of 8 warps per SM; two tables and a small map keep four.
+constexpr int kBqsrSharedCovMax = 2;
+constexpr int64_t kBqsrMapMax = 32768;      // bytes of a read-group map: 16 per ID and the IDs' bytes
+
+enum { BQSR_COUNT = 0, BQSR_FILTERED = 1, BQSR_EMPTY = 2, BQSR_ERR_NOQUAL = 3, BQSR_ERR_CYCLES = 4, BQSR_ERR_QUAL = 5, BQSR_ERR_NORG = 6,
+       BQSR_ERR_BADRG = 7 };
 
 // the reference and the known sites, all over the forward strand's concatenated contigs [0, l_pac)
 struct BqsrView {
-    const uint8_t *ref;                 // codes 0..3
+    const uint8_t *ref;                 // codes 0..3, one byte per base; nullptr: pac holds the reference
     const int64_t *ann_off;             // each contig's offset
     int32_t n_seqs;
     int64_t l_pac;
     const uint64_t *covered, *junction; // 1 bit per base
     const int64_t *holes;               // .amb holes as [beg, end) pairs, sorted
     int64_t n_holes;
+    const uint8_t *pac;                 // 2 bits per base, base g at pac[g >> 2] >> ((~g & 3) << 1) & 3 (the .pac layout), when ref is nullptr
 };
 
 struct BqsrRec {
@@ -136,7 +151,7 @@ BM2_HD int bqsr_ref_base(const BqsrRec &r, const BqsrView &v, int64_t g) {
     if (r.hole >= 0)
         for (int64_t h = r.hole; h < v.n_holes && v.holes[2 * h] <= g; ++h)
             if (g < v.holes[2 * h + 1]) return 4;
-    return v.ref[g];
+    return v.ref ? v.ref[g] : (v.pac[g >> 2] >> ((~g & 3) << 1)) & 3;
 }
 
 // the context (-1: none) and cycle of read base k of [lo, hi), the tails set: what both the counting and the apply side key a base by
@@ -226,6 +241,37 @@ BM2_HD int32_t bqsr_aux_rg(const uint8_t *rec, int32_t *len) {
             p += sz;
         }
     }
+    return -1;
+}
+
+// one entry of a read-group map: the map is n_ids entries, then the IDs' bytes; off is an ID's offset from the map's start, val what the
+// caller keeps per ID (a table, library or covariate index)
+struct BqsrRgEntry { int32_t off, len, val, pad; };
+
+// the index of the first map entry whose ID is the len bytes at rec + at (bqsr_aux_rg's value), -1 when none.  On the device the whole warp
+// calls it with the same arguments, and the lanes compare 32 IDs at a time.
+BM2_HD int bqsr_rg_lookup(const BqsrRgEntry *map, int n_ids, const uint8_t *rec, int32_t at, int32_t len) {
+    const uint8_t *bytes = (const uint8_t *) map;
+#if defined(__CUDA_ARCH__)
+    const int lane = threadIdx.x & 31;
+    for (int j0 = 0; j0 < n_ids; j0 += 32) {
+        const int j = j0 + lane;
+        bool m = false;
+        if (j < n_ids) {
+            const BqsrRgEntry e = map[j];
+            m = e.len == len;
+            for (int k = 0; m && k < len; ++k) m = bytes[e.off + k] == rec[at + k];
+        }
+        const unsigned b = __ballot_sync(0xFFFFFFFFu, m);
+        if (b) return j0 + __ffs(b) - 1;
+    }
+#else
+    for (int j = 0; j < n_ids; ++j) {
+        bool m = map[j].len == len;
+        for (int k = 0; m && k < len; ++k) m = bytes[map[j].off + k] == rec[at + k];
+        if (m) return j;
+    }
+#endif
     return -1;
 }
 

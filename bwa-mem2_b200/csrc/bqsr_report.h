@@ -9,7 +9,7 @@
 //                       is the same for every Q, so it is left out: the argmax does not change.
 //   report              GATKReport v1.1: Arguments (GATK 4's defaults), Quantized (qualities 0..93 mapped to themselves), RecalTable0 (the
 //                       read group), RecalTable1 (quality), RecalTable2 (quality and context, then quality and cycle), event M only, the
-//                       rows with at least one observation.  Each cell is padded to its column's widest, strings left, numbers right, two
+//                       rows with at least one observation.  Several read group covariates: each one's rows in turn, in the order given.  Each cell is padded to its column's widest, strings left, numbers right, two
 //                       spaces apart.  No timestamp.
 #pragma once
 #include "bqsr_device.cuh"
@@ -40,16 +40,18 @@ inline int bqsr_empirical_q(int64_t n, int64_t e, double prior) {
     return arg < 93 ? arg : 93;
 }
 
+// the value of a header line's tag ("ID:"), empty without it
+inline std::string bqsr_rg_tag(const std::string &line, const char *tag) {
+    const size_t at = line.find(std::string("\t") + tag);
+    if (at == std::string::npos) return std::string();
+    const size_t b = at + 4, e = line.find_first_of("\t\n", b);
+    return line.substr(b, (e == std::string::npos ? line.size() : e) - b);
+}
+
 // the read group covariate of a read group line: its PU, else its ID
 inline std::string bqsr_read_group(const std::string &rg_line) {
-    auto field = [&](const char *tag) {
-        const size_t at = rg_line.find(std::string("\t") + tag);
-        if (at == std::string::npos) return std::string();
-        const size_t b = at + 4, e = rg_line.find_first_of("\t\n", b);
-        return rg_line.substr(b, (e == std::string::npos ? rg_line.size() : e) - b);
-    };
-    const std::string pu = field("PU:");
-    return pu.empty() ? field("ID:") : pu;
+    const std::string pu = bqsr_rg_tag(rg_line, "PU:");
+    return pu.empty() ? bqsr_rg_tag(rg_line, "ID:") : pu;
 }
 
 // one GATKReport table: cols are (name, format); rows hold the cells' text
@@ -84,9 +86,15 @@ struct BqsrTable {
 
 inline std::string bqsr_fmt(const char *f, double v) { char b[64]; snprintf(b, sizeof b, f, v); return b; }
 
-// the report of the dense tables: qual [94], ctx [94 * 16], cyc [94 * 1001], observations and errors
-inline std::string bqsr_report_text(const std::string &rg, const int64_t *qo, const int64_t *qe, const int64_t *co, const int64_t *ce,
-                                    const int64_t *yo, const int64_t *ye) {
+// one covariate's dense tables: qual [94], ctx [94 * 16], cyc [94 * 1001], observations and errors
+struct BqsrCovTables {
+    std::string rg;
+    const int64_t *qo, *qe, *co, *ce, *yo, *ye;
+};
+
+// the report of several covariates (bm2_baserecalibrator, in the byte order of their strings): RecalTable0 one row per covariate,
+// RecalTable1 and RecalTable2 the rows of each covariate in turn, the Quantized table's Count summed over them
+inline std::string bqsr_report_text(const std::vector<BqsrCovTables> &covs) {
     std::string o = "#:GATKReport.v1.1:5\n";
     BqsrTable a{"Arguments", "Recalibration argument collection values used in this run", {{"Argument", "%s"}, {"Value", "%s"}}, {}};
     static const char *const args[17][2] = {
@@ -98,38 +106,50 @@ inline std::string bqsr_report_text(const std::string &rg, const int64_t *qo, co
     for (const auto &r : args) a.rows.push_back({r[0], r[1]});
     o += a.text();
     BqsrTable qz{"Quantized", "Quality quantization map", {{"QualityScore", "%d"}, {"Count", "%d"}, {"QuantizedScore", "%d"}}, {}};
-    for (int q = 0; q < BQSR_NQ; ++q) qz.rows.push_back({std::to_string(q), std::to_string((long long) qo[q]), std::to_string(q)});
+    for (int q = 0; q < BQSR_NQ; ++q) {
+        int64_t n = 0;
+        for (const BqsrCovTables &c : covs) n += c.qo[q];
+        qz.rows.push_back({std::to_string(q), std::to_string((long long) n), std::to_string(q)});
+    }
     o += qz.text();
-    int64_t N = 0, E = 0; double s = 0;
-    for (int q = 0; q < BQSR_NQ; ++q) { N += qo[q]; E += qe[q]; s += (double) qo[q] * std::pow(10.0, (double) q / -10.0); }
     BqsrTable t0{"RecalTable0", "", {{"ReadGroup", "%s"}, {"EventType", "%s"}, {"EmpiricalQuality", "%.4f"}, {"EstimatedQReported", "%.4f"},
                                      {"Observations", "%d"}, {"Errors", "%.2f"}}, {}};
-    if (N > 0) {
-        const double qr = -10.0 * std::log10(s / (double) N);
-        t0.rows.push_back({rg, "M", bqsr_fmt("%.4f", bqsr_empirical_q(N, E, qr)), bqsr_fmt("%.4f", qr), std::to_string((long long) N),
-                           bqsr_fmt("%.2f", (double) E)});
-    }
-    o += t0.text();
     BqsrTable t1{"RecalTable1", "", {{"ReadGroup", "%s"}, {"QualityScore", "%d"}, {"EventType", "%s"}, {"EmpiricalQuality", "%.4f"},
                                      {"Observations", "%d"}, {"Errors", "%.2f"}}, {}};
     BqsrTable t2{"RecalTable2", "", {{"ReadGroup", "%s"}, {"QualityScore", "%d"}, {"CovariateValue", "%s"}, {"CovariateName", "%s"},
                                      {"EventType", "%s"}, {"EmpiricalQuality", "%.4f"}, {"Observations", "%d"}, {"Errors", "%.2f"}}, {}};
     static const char L[] = "ACGT";
-    for (int q = 0; q < BQSR_NQ; ++q) {
-        if (qo[q]) t1.rows.push_back({rg, std::to_string(q), "M", bqsr_fmt("%.4f", bqsr_empirical_q(qo[q], qe[q], q)), std::to_string((long long) qo[q]),
-                                      bqsr_fmt("%.2f", (double) qe[q])});
-        for (int c = 0; c < BQSR_NCTX; ++c) {
-            const int64_t n = co[q * BQSR_NCTX + c], e = ce[q * BQSR_NCTX + c];
-            if (n) t2.rows.push_back({rg, std::to_string(q), std::string{L[c >> 2], L[c & 3]}, "Context", "M", bqsr_fmt("%.4f", bqsr_empirical_q(n, e, q)),
-                                      std::to_string((long long) n), bqsr_fmt("%.2f", (double) e)});
+    for (const BqsrCovTables &c : covs) {
+        const std::string &rg = c.rg;
+        int64_t N = 0, E = 0; double s = 0;
+        for (int q = 0; q < BQSR_NQ; ++q) { N += c.qo[q]; E += c.qe[q]; s += (double) c.qo[q] * std::pow(10.0, (double) q / -10.0); }
+        if (N > 0) {
+            const double qr = -10.0 * std::log10(s / (double) N);
+            t0.rows.push_back({rg, "M", bqsr_fmt("%.4f", bqsr_empirical_q(N, E, qr)), bqsr_fmt("%.4f", qr), std::to_string((long long) N),
+                               bqsr_fmt("%.2f", (double) E)});
         }
-        for (int y = 0; y < BQSR_NCYC; ++y) {
-            const int64_t n = yo[q * BQSR_NCYC + y], e = ye[q * BQSR_NCYC + y];
-            if (n) t2.rows.push_back({rg, std::to_string(q), std::to_string(y - BQSR_MAX_CYCLE), "Cycle", "M", bqsr_fmt("%.4f", bqsr_empirical_q(n, e, q)),
-                                      std::to_string((long long) n), bqsr_fmt("%.2f", (double) e)});
+        for (int q = 0; q < BQSR_NQ; ++q) {
+            if (c.qo[q]) t1.rows.push_back({rg, std::to_string(q), "M", bqsr_fmt("%.4f", bqsr_empirical_q(c.qo[q], c.qe[q], q)),
+                                            std::to_string((long long) c.qo[q]), bqsr_fmt("%.2f", (double) c.qe[q])});
+            for (int x = 0; x < BQSR_NCTX; ++x) {
+                const int64_t n = c.co[q * BQSR_NCTX + x], e = c.ce[q * BQSR_NCTX + x];
+                if (n) t2.rows.push_back({rg, std::to_string(q), std::string{L[x >> 2], L[x & 3]}, "Context", "M", bqsr_fmt("%.4f", bqsr_empirical_q(n, e, q)),
+                                          std::to_string((long long) n), bqsr_fmt("%.2f", (double) e)});
+            }
+            for (int y = 0; y < BQSR_NCYC; ++y) {
+                const int64_t n = c.yo[q * BQSR_NCYC + y], e = c.ye[q * BQSR_NCYC + y];
+                if (n) t2.rows.push_back({rg, std::to_string(q), std::to_string(y - BQSR_MAX_CYCLE), "Cycle", "M", bqsr_fmt("%.4f", bqsr_empirical_q(n, e, q)),
+                                          std::to_string((long long) n), bqsr_fmt("%.2f", (double) e)});
+            }
         }
     }
-    return o + t1.text() + t2.text();
+    return o + t0.text() + t1.text() + t2.text();
+}
+
+// the report of one covariate's dense tables (bm2_mem --recal-file)
+inline std::string bqsr_report_text(const std::string &rg, const int64_t *qo, const int64_t *qe, const int64_t *co, const int64_t *ce,
+                                    const int64_t *yo, const int64_t *ye) {
+    return bqsr_report_text(std::vector<BqsrCovTables>{{rg, qo, qe, co, ce, yo, ye}});
 }
 
 // ---- the apply side (bm2_applybqsr): a GATKReport v1.1 recalibration table read back into the dense tables of bqsr_device.cuh's rule ----

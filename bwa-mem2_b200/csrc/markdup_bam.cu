@@ -2,7 +2,7 @@
 // half, the merge, pairing, resolve and metrics, is markdup_bam.h).
 //   bm2_markdup_set      the merged header's read groups (each @RG ID and its library index) to the context, the per-library counters zeroed
 //   bm2_markdup_records  one merged window: one warp per record.  Lane 0 finds the RG:Z value and the lanes compare it against 32 IDs of the
-//                        shared-memory map at a time (as bqsr_apply.cu does).  Secondary / supplementary records and unmapped primaries are
+//                        shared-memory map at a time (bqsr_rg_lookup, as bqsr_apply.cu does).  Secondary / supplementary records and unmapped primaries are
 //                        counted per library (one atomic per record).  A mapped primary gets its end and score from the warp's sums
 //                        (dup_ref_len_part, dup_qual_part: markdup.cu's helpers) and, when it is half of a pair, its location from a ballot
 //                        per 32 bytes of its QNAME (the colon finder of bm2_dup_signatures_ex).
@@ -40,7 +40,6 @@ __global__ void __launch_bounds__(kWarps * 32) mdb_record_kernel(const uint8_t *
     extern __shared__ int4 s_map[];
     for (int i = threadIdx.x; i < map_bytes / 16; i += blockDim.x) s_map[i] = map[i];
     __syncthreads();
-    const uint8_t *s_bytes = (const uint8_t *) s_map;
     const int lane = threadIdx.x & 31;
     for (int64_t w = (int64_t) blockIdx.x * kWarps + (threadIdx.x >> 5); w < n; w += (int64_t) gridDim.x * kWarps) {
         const uint8_t *rec = base + starts[w];
@@ -50,18 +49,8 @@ __global__ void __launch_bounds__(kWarps * 32) mdb_record_kernel(const uint8_t *
         at = __shfl_sync(kFull, at, 0); len = __shfl_sync(kFull, len, 0);
         int rg = n_ids, lib = unknown_lib;                               // no tag: the shared read group n_ids
         if (at >= 0) {
-            rg = -1;                                                     // a value that is no @RG ID
-            for (int j0 = 0; j0 < n_ids; j0 += 32) {
-                const int j = j0 + lane;
-                bool m = false;
-                if (j < n_ids) {
-                    const int4 e = s_map[j];
-                    m = e.y == len;
-                    for (int k = 0; m && k < len; ++k) m = s_bytes[e.x + k] == rec[at + k];
-                }
-                const unsigned b = __ballot_sync(kFull, m);
-                if (b) { rg = j0 + __ffs(b) - 1; lib = s_map[rg].z; break; }
-            }
+            rg = bqsr_rg_lookup((const BqsrRgEntry *) s_map, n_ids, rec, at, len);   // -1: a value that is no @RG ID
+            if (rg >= 0) lib = s_map[rg].z;
         }
         bm2_markdup_rec o{};
         o.rg = rg; o.lib = lib; o.kind = BM2_MDB_NONE;

@@ -525,7 +525,8 @@ typedef struct bm2_bqsr_tables_t {
     int64_t reads, bases;                 /* records and bases counted                                                          */
     double ms;                            /* device time of the counting kernels (CUDA events)                                  */
     int32_t err_kind;                     /* the first read error: 0 none, 1 no qualities, 2 over 500 cycles after clipping,   */
-    int64_t err_index;                    /*   3 a quality above 93; its record's index over all records seen since the sites   */
+    int64_t err_index;                    /*   3 a quality above 93 (bm2_recal_tables also: 4 no RG tag, 5 an RG tag that is no  */
+                                          /*   ID); its record's index over all records seen since the sites                    */
     const char *err_name;                 /*   and its read name                                                                */
     const char *read_group;               /* the read group covariate given to bm2_bqsr_sites                                   */
 } bm2_bqsr_tables_t;
@@ -542,6 +543,38 @@ int  bm2_bqsr_sites(bm2_ctx *ctx, const uint64_t *covered, const uint64_t *junct
 int  bm2_bqsr_count(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int64_t *starts, int64_t n_recs);
 /* The counts since bm2_bqsr_sites (HOST arrays owned by the context, valid until its next call). */
 int  bm2_bqsr_tables(bm2_ctx *ctx, bm2_bqsr_tables_t *out);
+
+/* ---- Base quality recalibration tables of BAM files (bm2_baserecalibrator) -------------------------------------------------------------
+ * The rule of bm2_bqsr_count, with 0x400 read from the input, plus the read group: a record that passes the filters must have an RG:Z tag
+ * whose value is one of the map's IDs (checked before the read errors), and it counts into the tables of that ID's covariate.  The
+ * reference is the index's packed .pac bytes; the FM index is not needed. */
+typedef struct {
+    int32_t n_contigs;
+    const int64_t *contig_off;             /* each contig's offset in the concatenated reference                                */
+    const int32_t *contig_len;             /* and its length                                                                    */
+    int64_t l_pac;
+    const uint8_t *pac;                    /* (l_pac + 3) / 4 bytes, base i at pac[i >> 2] >> ((~i & 3) << 1) & 3               */
+    const int64_t *holes;                  /* the .amb holes as n_holes sorted [beg, end) pairs: N inside them                  */
+    int64_t n_holes;
+    const uint64_t *covered, *junction;    /* the known-site bitsets of bm2_bqsr_sites, l_pac bits each                         */
+    int32_t n_ids;                         /* the headers' @RG IDs (the first of equal IDs is the one matched; at most 32 KiB    */
+    const char *const *ids;                /*   with 16 bytes each)                                                             */
+    const int32_t *id_cov;                 /* each ID's covariate, 0 .. n_cov - 1                                               */
+    int32_t n_cov;                         /* covariates (their tables: about 1.5 MB each on the device)                        */
+} bm2_recal_set_t;
+/* Device bytes bm2_recal_set and bm2_recal_add need for a reference of l_pac bases, n_cov covariates and windows of window_bytes of records
+ * of about 300 bytes, and the bytes free on ctx's device now. */
+int  bm2_recal_memory(const bm2_ctx *ctx, int64_t l_pac, int64_t window_bytes, int32_t n_cov, int64_t *needed, int64_t *free_bytes);
+/* The reference, the known sites and the read-group map to the context, copied; zeroes the counts.  A reference larger than the free device
+ * memory is an error that gives both numbers. */
+int  bm2_recal_set(bm2_ctx *ctx, const bm2_recal_set_t *s);
+/* One window: recs (HOST, n bytes) holds n_recs records at starts, in any order.  A record that passes the filters and does not lie inside
+ * its contig is malformed: 2 is returned, naming it, and nothing is counted.  A read error (no qualities, over 500 cycles after clipping, a
+ * quality above 93, no RG tag, an RG tag that is no ID) is not counted; 2 is returned with an error naming the first such read, which
+ * bm2_recal_tables reports too (err_kind 1..5). */
+int  bm2_recal_add(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int64_t *starts, int64_t n_recs);
+/* Covariate cov's counts since bm2_recal_set (HOST arrays owned by the context, valid until its next call; read_group is empty). */
+int  bm2_recal_tables(bm2_ctx *ctx, int32_t cov, bm2_bqsr_tables_t *out);
 
 /* ---- Base quality recalibration applied (bm2_applybqsr) ------------------------------------------------------------------------------
  * The rule (csrc/bqsr_device.cuh, csrc/bqsr_report.h) restates GATK 4 ApplyBQSR's BQSRReadTransformer at its defaults: no quantization,
