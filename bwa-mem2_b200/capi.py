@@ -256,6 +256,12 @@ class MmResult(C.Structure):
                 ("add_ms", C.c_double), ("finish_ms", C.c_double)]
 
 
+# bm2_mm_gc_finish (include/bm2_b200.h)
+class MmGcResult(C.Structure):
+    _fields_ = [("windows", C.c_int64 * 101), ("reads", C.c_int64 * 101), ("bases", C.c_int64 * 101), ("errors", C.c_int64 * 101),
+                ("total_clusters", C.c_int64), ("aligned_reads", C.c_int64), ("scan_ms", C.c_double), ("add_ms", C.c_double)]
+
+
 class SortOut(C.Structure):
     _fields_ = [("z", C.c_void_p), ("z_len", C.c_int64), ("member_size", C.c_void_p), ("n_members", C.c_int64), ("carry", C.c_void_p),
                 ("carry_len", C.c_int64), ("recs", C.c_void_p), ("n_recs", C.c_int64)]
@@ -269,7 +275,7 @@ EXPORTS = ["bm2_create_sibling", "bm2_fastq_encode", "bm2_seq_encode", "bm2_fast
            "bm2_dup_signatures", "bm2_dup_resolve", "bm2_last_dup_stats", "bm2_dup_set", "bm2_dup_signatures_ex", "bm2_dup_resolve_ex",
            "bm2_bqsr_sites", "bm2_bqsr_count", "bm2_bqsr_tables", "bm2_bqsr_apply_set", "bm2_bqsr_apply", "bm2_last_bqsr_apply_stats",
            "bm2_bqsr_apply_memory", "bm2_wgs_set", "bm2_wgs_memory", "bm2_wgs_add", "bm2_wgs_finish",
-           "bm2_mm_set", "bm2_mm_memory", "bm2_mm_add", "bm2_mm_finish", "bm2_markdup_set", "bm2_markdup_records", "bm2_markdup_pair", "bm2_markdup_counts",
+           "bm2_mm_set", "bm2_mm_memory", "bm2_mm_add", "bm2_mm_finish", "bm2_mm_gc_set", "bm2_mm_gc_memory", "bm2_mm_gc_finish", "bm2_markdup_set", "bm2_markdup_records", "bm2_markdup_pair", "bm2_markdup_counts",
            "bm2_markdup_mark", "bm2_last_markdup_stats", "bm2_markdup_memory", "bm2_recal_memory", "bm2_recal_set", "bm2_recal_add", "bm2_recal_tables"]
 
 _lib = None
@@ -958,6 +964,30 @@ class Context:
                     insert_hist=_host(r.insert_hist, 3 * I, np.int64).reshape(3, I),
                     insert_big=_host(r.insert_big, r.n_big, np.uint64) if r.n_big else np.zeros(0, np.uint64), records=r.records,
                     add_ms=r.add_ms, finish_ms=r.finish_ms)
+
+    def mm_gc_set(self):
+        """bm2_mm_gc_set: after mm_set, bins the reference's windows by GC and counts GC bias in the mm_add calls that follow."""
+        f = lib().bm2_mm_gc_set
+        f.argtypes = [C.c_void_p]
+        self._check(f(self._ctx), "bm2_mm_gc_set")
+
+    def mm_gc_memory(self, window_bytes: int):
+        """bm2_mm_gc_memory -> the device bytes GC bias adds to mm_memory's figure."""
+        need = C.c_int64()
+        f = lib().bm2_mm_gc_memory
+        f.argtypes = [C.c_void_p, C.c_int64, C.c_void_p]
+        self._check(f(self._ctx, int(window_bytes), C.byref(need)), "bm2_mm_gc_memory")
+        return need.value
+
+    def mm_gc_finish(self):
+        """bm2_mm_gc_finish -> dict(windows, reads, bases, errors [101] each, total_clusters, aligned_reads, scan_ms, add_ms)."""
+        r = MmGcResult()
+        f = lib().bm2_mm_gc_finish
+        f.argtypes = [C.c_void_p, C.c_void_p]
+        self._check(f(self._ctx, C.byref(r)), "bm2_mm_gc_finish")
+        return dict(windows=np.array(r.windows, np.int64), reads=np.array(r.reads, np.int64), bases=np.array(r.bases, np.int64),
+                    errors=np.array(r.errors, np.int64), total_clusters=r.total_clusters, aligned_reads=r.aligned_reads, scan_ms=r.scan_ms,
+                    add_ms=r.add_ms)
 
     def set_sam_staged(self, on: int):
         """bm2_set_sam_staged: 1 / 2 = the rescue's local alignments as a batch (one window per warp / per thread) before the per-pair kernel, 0 = inside it."""

@@ -134,8 +134,11 @@ struct bm2_ctx {
     std::vector<int64_t> wgs_hist;
     // bm2_mm_set / bm2_mm_add / bm2_mm_finish (mm.cu): buffers, whether a reference is set, its contigs and holes, events, the records seen
     // since, the insert sizes of 2^20 or more (copied back after each window), the device times, the histograms copied back by the finish
-    DevBuf mm_d[16];
+    DevBuf mm_d[19];
     bool mm_set = false;
+    // bm2_mm_gc_set: GC bias counted by the adds that follow (bm2_mm_set turns it off), the scan's and those adds' device times
+    bool mm_gc = false;
+    double mm_gc_scan_ms = 0, mm_gc_add_ms = 0;
     int64_t mm_l_pac = 0, mm_n_holes = 0;
     int32_t mm_n_contigs = 0;
     cudaEvent_t mm_ev[2] = {nullptr, nullptr};

@@ -12,10 +12,21 @@
 //           count to per-block shared bins below kHot (global atomics above), and its insert size to dense per-orientation bins below 2^20
 //           or to an append list.  Each block flushes once with 64-bit atomics and raises the running maxima (atomicMax).
 // Only integer atomics: the sums commute, so the counts do not depend on the windows or the order of the records.
+//
+// GC bias (bm2_mm_gc_set, bm2_mm_gc_finish; the rule is mm_device.cuh's, the text mm_gcbias.h's):
+//   scan    the reference windows, once per bm2_mm_gc_set: each block takes tiles of kScanTile window starts; one thread per 32-locus word
+//           builds the tile's GC and N bitsets (kScanTile + W loci) from the packed bases and the hole bitset, the hole letters found by a
+//           binary search of the holes where a word has a hole bit (mm_gc_word), and a block scan of their popcounts gives prefix counts,
+//           so a window's counts are two prefix lookups and two masked popcounts each.  The tile walks the contigs it overlaps, clipped to
+//           their counted starts; bins go to a per-block shared histogram (one atomic per __match_any_sync group), flushed once.
+//   add     the check and count kernels instantiated with GC on: the check applies the aligned checks to every placed record and writes its
+//           MmGc (window locus, I and D lengths); the count warp classifies the 100 letters of the window with ballots and popcounts and
+//           adds the read start, bases and errors to per-block shared bins.  The instantiations with GC off are the kernels above unchanged.
 #include "bm2_common.cuh"
 #include "bm2_ctx.h"
 #include "mm_metrics.h"
 #include <algorithm>
+#include <cub/block/block_scan.cuh>
 #include <vector>
 
 namespace {
@@ -25,6 +36,9 @@ constexpr unsigned kFull = 0xFFFFFFFFu;
 constexpr int kRecBytes = 300;              // a short read's record, for bm2_mm_memory's estimate
 constexpr int kHot = 256;                   // read lengths and mismatch counts below this are binned per block in shared memory
 constexpr size_t kLenBins = (size_t) MM_MAX_LSEQ + 1, kInsBins = (size_t) MM_DENSE_INSERT;
+constexpr int kScanThreads = 256, kScanTile = 32 * (kScanThreads - 4);   // a tile's words (one per thread) cover its starts and W - 1 more loci
+// the GC bias counters: read starts, bases and errors per bin, then TOTAL_CLUSTERS and ALIGNED_READS
+enum { GC_READS = 0, GC_BASES = MM_GC_BINS, GC_ERRORS = 2 * MM_GC_BINS, GC_CLUSTERS = 3 * MM_GC_BINS, GC_ALIGNED, GC_NCOUNT };
 
 __constant__ char c_kmers[MM_N_ADAPTER_KMERS][MM_ADAPTER_LEN];
 
@@ -36,9 +50,10 @@ __global__ void mm_holes_kernel(uint32_t *bits, int64_t n_words, const int64_t *
         bits[w] = wgs_range_word(ranges, n, w);
 }
 
+template <bool GC>
 __global__ void __launch_bounds__(kWarps * 32) mm_check_kernel(const uint8_t *__restrict__ base, const int64_t *__restrict__ starts, int64_t n,
                                                                const int64_t *__restrict__ off, const int32_t *__restrict__ len, int32_t n_contigs,
-                                                               MmInfo *info, unsigned long long *sc, int64_t first) {
+                                                               MmInfo *info, unsigned long long *sc, int64_t first, MmGc *gc) {
     const int lane = threadIdx.x & 31;
     for (int64_t w = (int64_t) blockIdx.x * kWarps + (threadIdx.x >> 5); w < n; w += (int64_t) gridDim.x * kWarps) {
         const uint8_t *r = base + starts[w];
@@ -48,23 +63,32 @@ __global__ void __launch_bounds__(kWarps * 32) mm_check_kernel(const uint8_t *__
         if (inside) { wgs_cigar_part(c, lane, 32, s); mm_clip_part(c, lane, 32, t); }
         for (int k = 0; k < 3; ++k)
             for (int o = 16; o; o >>= 1) { s[k] += __shfl_xor_sync(kFull, s[k], o); t[k] += __shfl_xor_sync(kFull, t[k], o); }
+        int64_t idlen = 0;
+        if constexpr (GC) {
+            if (inside) idlen = mm_gc_idlen_part(c, lane, 32);
+            for (int o = 16; o; o >>= 1) idlen += __shfl_xor_sync(kFull, idlen, o);
+        }
         if (lane == 0) {
             MmInfo in;
-            mm_classify(r, s, t, inside, off, len, n_contigs, c_kmers, in);
+            mm_classify(r, s, t, inside, off, len, n_contigs, c_kmers, in, GC);
             info[w] = in;
             if (in.err) atomicMin(&sc[SC_ERR], (unsigned long long) (first + w) << 4 | (unsigned) in.err);
+            if constexpr (GC) gc[w] = MmGc{(in.bits & MMB_PLACED) ? mm_gc_window(r, s[1], off, len) : -1, idlen};
         }
     }
 }
 
+template <bool GC>
 __global__ void __launch_bounds__(kWarps * 32) mm_count_kernel(const uint8_t *__restrict__ base, const int64_t *__restrict__ starts, int64_t n,
                                                                const MmInfo *__restrict__ info, const uint8_t *__restrict__ pac,
                                                                const uint32_t *__restrict__ hole_bits, const int64_t *__restrict__ holes,
                                                                const char *__restrict__ hole_char, int64_t n_holes, unsigned long long *cnt,
                                                                unsigned long long *len_hist, unsigned long long *mism_hist,
                                                                unsigned long long *nocall, unsigned long long *ins, uint64_t *big,
-                                                               unsigned long long *sc) {
+                                                               unsigned long long *sc, const MmGc *__restrict__ gc, unsigned long long *gc_cnt) {
     __shared__ unsigned long long s_cnt[MM_NCAT * MM_NCOUNT];
+    __shared__ unsigned long long s_gc[GC ? GC_NCOUNT : 1];
+    if constexpr (GC) for (int k = threadIdx.x; k < GC_NCOUNT; k += blockDim.x) s_gc[k] = 0;
     __shared__ uint32_t s_len[MM_NCAT][kHot], s_mis[MM_NCAT][kHot];
     __shared__ uint32_t s_max_len, s_max_ins;
     for (int k = threadIdx.x; k < MM_NCAT * MM_NCOUNT; k += blockDim.x) s_cnt[k] = 0;
@@ -82,7 +106,7 @@ __global__ void __launch_bounds__(kWarps * 32) mm_count_kernel(const uint8_t *__
             if (mm_nibble(sq.seq, k) == 15)
                 atomicAdd(&nocall[row + (size_t) ((in.bits & MMB_REV) ? in.l_seq - 1 - k : k)], 1ull);
         uint32_t mism = 0, q20 = 0;
-        if (in.bits & MMB_ALIGNED) {
+        if (in.bits & (GC ? MMB_PLACED : MMB_ALIGNED)) {
             const DupCigar c = dup_cigar(r);
             const bool noqual = in.bits & MMB_NOQUAL;
             int64_t k = 0, g = in.g0;
@@ -95,6 +119,28 @@ __global__ void __launch_bounds__(kWarps * 32) mm_count_kernel(const uint8_t *__
             }
             mism = __reduce_add_sync(kFull, mism);
             q20 = __reduce_add_sync(kFull, q20);
+        }
+        if constexpr (GC) {
+            const MmGc gi = gc[w];
+            int bin = -1;
+            if (gi.gw >= 0) {                                            // the window's letters, 32 at a time
+                int n_gc = 0, n_n = 0;
+                for (int j = 0; j < MM_GC_W; j += 32) {
+                    const int cls = j + lane < MM_GC_W ? mm_gc_class(mm_ref_letter(pac, hole_bits, holes, hole_char, n_holes, gi.gw + j + lane)) : 0;
+                    n_gc += __popc(__ballot_sync(kFull, cls == 1));
+                    n_n += __popc(__ballot_sync(kFull, cls == 2));
+                }
+                bin = mm_gc_bin(n_gc, n_n);
+            }
+            if (lane == 0) {
+                if (in.cat != MM_SECOND) atomicAdd(&s_gc[GC_CLUSTERS], 1ull);
+                if (in.bits & MMB_PLACED) atomicAdd(&s_gc[GC_ALIGNED], 1ull);
+                if (bin >= 0) {
+                    atomicAdd(&s_gc[GC_READS + bin], 1ull);
+                    atomicAdd(&s_gc[GC_BASES + bin], (unsigned long long) in.l_seq);
+                    atomicAdd(&s_gc[GC_ERRORS + bin], (unsigned long long) mism + (unsigned long long) gi.idlen);
+                }
+            }
         }
         if (lane == 0) {
             int64_t v[MM_NCOUNT];
@@ -129,11 +175,58 @@ __global__ void __launch_bounds__(kWarps * 32) mm_count_kernel(const uint8_t *__
         if (s_max_len) atomicMax(&sc[SC_MAX_LEN], (unsigned long long) s_max_len);
         if (s_max_ins) atomicMax(&sc[SC_MAX_INS], (unsigned long long) s_max_ins);
     }
+    if constexpr (GC) for (int k = threadIdx.x; k < GC_NCOUNT; k += blockDim.x) if (s_gc[k]) atomicAdd(&gc_cnt[k], s_gc[k]);
+}
+
+// the reference windows by GC bin (mm_device.cuh's rule): tiles of kScanTile window starts, grid-stride; contigs sorted and disjoint
+__global__ void __launch_bounds__(kScanThreads) mm_gc_scan_kernel(const uint8_t *__restrict__ pac, const uint32_t *__restrict__ hole_bits,
+                                                                  const int64_t *__restrict__ holes, const char *__restrict__ hole_char, int64_t n_holes,
+                                                                  int64_t l_pac, const int64_t *__restrict__ off, const int32_t *__restrict__ len,
+                                                                  int32_t n_contigs, int64_t n_tiles, unsigned long long *windows) {
+    using Scan = cub::BlockScan<uint32_t, kScanThreads>;
+    __shared__ typename Scan::TempStorage s_scan;
+    __shared__ uint32_t s_gcw[kScanThreads], s_nw[kScanThreads], s_pre[kScanThreads], s_hist[MM_GC_BINS];
+    for (int k = threadIdx.x; k < MM_GC_BINS; k += blockDim.x) s_hist[k] = 0;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int64_t t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+        const int64_t b = t * kScanTile;                                 // a multiple of 32: word k of the tile is locus word b / 32 + k
+        uint32_t gcm, nm;
+        mm_gc_word(pac, hole_bits, holes, hole_char, n_holes, l_pac, b / 32 + threadIdx.x, gcm, nm);
+        uint32_t pre;
+        __syncthreads();                                                 // the last tile's readers are done
+        Scan(s_scan).ExclusiveSum((uint32_t) __popc(gcm) << 16 | (uint32_t) __popc(nm), pre);   // at most 8192 each
+        s_gcw[threadIdx.x] = gcm; s_nw[threadIdx.x] = nm; s_pre[threadIdx.x] = pre;
+        __syncthreads();
+        // GC letters and Ns before tile locus x: packed (GC << 16 | N)
+        auto before = [&](int x) {
+            const uint32_t m = (1u << (x & 31)) - 1;
+            return s_pre[x >> 5] + ((uint32_t) __popc(s_gcw[x >> 5] & m) << 16) + (uint32_t) __popc(s_nw[x >> 5] & m);
+        };
+        int32_t lo = 0, hi = n_contigs;                                  // the first contig ending after b
+        while (lo < hi) { const int32_t m = (lo + hi) / 2; if (off[m] + len[m] <= b) lo = m + 1; else hi = m; }
+        const int64_t e = bm2_min<int64_t>(b + kScanTile, l_pac);
+        for (int32_t c = lo; c < n_contigs && off[c] < e; ++c) {
+            const int64_t g0 = bm2_max<int64_t>(b, off[c] + 1), g1 = bm2_min<int64_t>(e, off[c] + len[c] - MM_GC_W);
+            for (int64_t k = g0 + warp * 32; k < g1; k += kScanThreads) {   // warp-uniform trips
+                int bin = -1;
+                if (k + lane < g1) {
+                    const int x = (int) (k + lane - b);
+                    const uint32_t d = before(x + MM_GC_W) - before(x);
+                    bin = mm_gc_bin((int) (d >> 16), (int) (d & 0xFFFF));
+                }
+                const unsigned peers = __match_any_sync(kFull, bin);
+                if (bin >= 0 && lane == __ffs(peers) - 1) atomicAdd(&s_hist[bin], (uint32_t) __popc(peers));
+            }
+        }
+    }
+    __syncthreads();
+    for (int k = threadIdx.x; k < MM_GC_BINS; k += blockDim.x) if (s_hist[k]) atomicAdd(&windows[k], (unsigned long long) s_hist[k]);
 }
 
 enum { MD_PAC, MD_HOLEBITS, MD_HOLES, MD_HOLECHAR, MD_OFF, MD_LEN, MD_CNT, MD_LENH, MD_MISH, MD_NOCALL, MD_INS, MD_SC, MD_BIG, MD_RECS,
-       MD_STARTS, MD_INFO, MD_END };
+       MD_STARTS, MD_INFO, MD_GC_WIN, MD_GC_CNT, MD_GC_INFO, MD_END };
 static_assert(MD_END == std::extent<decltype(bm2_ctx::mm_d)>::value, "bm2_ctx::mm_d: one buffer per slot");
+static_assert(MM_GC_BINS == BM2_MM_GC_BINS, "bm2_mm_gc_result_t's bins");
 
 const char *const kErrText[3] = {"has l_seq 0 or above 1048576", "does not lie inside a contig of the reference",
                                  "has a CIGAR that does not match its record"};
@@ -212,7 +305,7 @@ extern "C" int bm2_mm_set(bm2_ctx *ctx, const int64_t *contig_off, const int32_t
     BM2_CUDA_OK(cudaStreamSynchronize(st));
     ctx->mm_l_pac = l_pac; ctx->mm_n_holes = n_holes; ctx->mm_n_contigs = n_contigs;
     ctx->mm_seen = 0; ctx->mm_big.clear(); ctx->mm_add_ms = 0; ctx->mm_finish_ms = 0;
-    ctx->mm_set = true;
+    ctx->mm_set = true; ctx->mm_gc = false;
     return 0;
 }
 
@@ -253,8 +346,10 @@ extern "C" int bm2_mm_add(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const in
     cudaStream_t st = ctx->stream;
     DevBuf *b = ctx->mm_d;
     const size_t nr = (size_t) n_recs;
+    const bool gc = ctx->mm_gc;
     if (ctx->ensure(b[MD_RECS], (size_t) n + 16) || ctx->ensure(b[MD_STARTS], nr * 8 + 8) || ctx->ensure(b[MD_INFO], nr * sizeof(MmInfo) + 8) ||
-        ctx->ensure(b[MD_BIG], nr * 8 + 8)) return 1;
+        ctx->ensure(b[MD_BIG], nr * 8 + 8) || (gc && ctx->ensure(b[MD_GC_INFO], nr * sizeof(MmGc) + 8))) return 1;
+    MmGc *d_gc = (MmGc *) b[MD_GC_INFO].p;
     for (cudaEvent_t &ev : ctx->mm_ev) if (!ev) BM2_CUDA_OK(cudaEventCreate(&ev));
     uint8_t *d_recs = (uint8_t *) b[MD_RECS].p;
     const int64_t *d_starts = (const int64_t *) b[MD_STARTS].p;
@@ -266,8 +361,12 @@ extern "C" int bm2_mm_add(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const in
     BM2_CUDA_OK(cudaMemsetAsync(d_sc + SC_BIG_N, 0, 8, st));
     const unsigned g = (unsigned) bm2_min<int64_t>((n_recs + kWarps - 1) / kWarps, (int64_t) ctx->n_sm * 8);
     BM2_CUDA_OK(cudaEventRecord(ctx->mm_ev[0], st));
-    mm_check_kernel<<<g, kWarps * 32, 0, st>>>(d_recs, d_starts, n_recs, (const int64_t *) b[MD_OFF].p, (const int32_t *) b[MD_LEN].p, ctx->mm_n_contigs,
-                                               d_info, d_sc, ctx->mm_seen);
+    if (gc)
+        mm_check_kernel<true><<<g, kWarps * 32, 0, st>>>(d_recs, d_starts, n_recs, (const int64_t *) b[MD_OFF].p, (const int32_t *) b[MD_LEN].p,
+                                                         ctx->mm_n_contigs, d_info, d_sc, ctx->mm_seen, d_gc);
+    else
+        mm_check_kernel<false><<<g, kWarps * 32, 0, st>>>(d_recs, d_starts, n_recs, (const int64_t *) b[MD_OFF].p, (const int32_t *) b[MD_LEN].p,
+                                                          ctx->mm_n_contigs, d_info, d_sc, ctx->mm_seen, nullptr);
     BM2_CUDA_OK(cudaGetLastError());
     BM2_CUDA_OK(cudaEventRecord(ctx->mm_ev[1], st));
     unsigned long long err = 0;
@@ -276,6 +375,7 @@ extern "C" int bm2_mm_add(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const in
     float ms = 0;
     BM2_CUDA_OK(cudaEventElapsedTime(&ms, ctx->mm_ev[0], ctx->mm_ev[1]));
     ctx->mm_add_ms += ms;
+    if (gc) ctx->mm_gc_add_ms += ms;
     if (err != ~0ULL) {                                                  // a read error: nothing of this window is counted
         const int64_t idx = (int64_t) (err >> 4), i = idx - ctx->mm_seen;
         const uint8_t *r = recs + starts[i];
@@ -284,11 +384,20 @@ extern "C" int bm2_mm_add(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const in
         return 2;
     }
     BM2_CUDA_OK(cudaEventRecord(ctx->mm_ev[0], st));
-    mm_count_kernel<<<g, kWarps * 32, 0, st>>>(d_recs, d_starts, n_recs, d_info, (const uint8_t *) b[MD_PAC].p, (const uint32_t *) b[MD_HOLEBITS].p,
-                                               (const int64_t *) b[MD_HOLES].p, (const char *) b[MD_HOLECHAR].p, ctx->mm_n_holes,
-                                               (unsigned long long *) b[MD_CNT].p, (unsigned long long *) b[MD_LENH].p,
-                                               (unsigned long long *) b[MD_MISH].p, (unsigned long long *) b[MD_NOCALL].p,
-                                               (unsigned long long *) b[MD_INS].p, (uint64_t *) b[MD_BIG].p, d_sc);
+    if (gc)
+        mm_count_kernel<true><<<g, kWarps * 32, 0, st>>>(d_recs, d_starts, n_recs, d_info, (const uint8_t *) b[MD_PAC].p,
+                                                         (const uint32_t *) b[MD_HOLEBITS].p, (const int64_t *) b[MD_HOLES].p,
+                                                         (const char *) b[MD_HOLECHAR].p, ctx->mm_n_holes, (unsigned long long *) b[MD_CNT].p,
+                                                         (unsigned long long *) b[MD_LENH].p, (unsigned long long *) b[MD_MISH].p,
+                                                         (unsigned long long *) b[MD_NOCALL].p, (unsigned long long *) b[MD_INS].p,
+                                                         (uint64_t *) b[MD_BIG].p, d_sc, d_gc, (unsigned long long *) b[MD_GC_CNT].p);
+    else
+        mm_count_kernel<false><<<g, kWarps * 32, 0, st>>>(d_recs, d_starts, n_recs, d_info, (const uint8_t *) b[MD_PAC].p,
+                                                          (const uint32_t *) b[MD_HOLEBITS].p, (const int64_t *) b[MD_HOLES].p,
+                                                          (const char *) b[MD_HOLECHAR].p, ctx->mm_n_holes, (unsigned long long *) b[MD_CNT].p,
+                                                          (unsigned long long *) b[MD_LENH].p, (unsigned long long *) b[MD_MISH].p,
+                                                          (unsigned long long *) b[MD_NOCALL].p, (unsigned long long *) b[MD_INS].p,
+                                                          (uint64_t *) b[MD_BIG].p, d_sc, nullptr, nullptr);
     BM2_CUDA_OK(cudaGetLastError());
     BM2_CUDA_OK(cudaEventRecord(ctx->mm_ev[1], st));
     unsigned long long n_big = 0;
@@ -296,6 +405,7 @@ extern "C" int bm2_mm_add(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const in
     BM2_CUDA_OK(cudaStreamSynchronize(st));
     BM2_CUDA_OK(cudaEventElapsedTime(&ms, ctx->mm_ev[0], ctx->mm_ev[1]));
     ctx->mm_add_ms += ms;
+    if (gc) ctx->mm_gc_add_ms += ms;
     if (n_big) {                                                         // the window's large insert sizes, kept on the host until the finish
         const size_t at = ctx->mm_big.size();
         ctx->mm_big.resize(at + (size_t) n_big);
@@ -338,5 +448,77 @@ extern "C" int bm2_mm_finish(bm2_ctx *ctx, bm2_mm_result_t *out) {
     out->insert_big = ctx->mm_big.data(); out->n_big = (int64_t) ctx->mm_big.size();
     out->records = ctx->mm_seen;
     out->add_ms = ctx->mm_add_ms; out->finish_ms = ctx->mm_finish_ms;
+    return 0;
+}
+
+extern "C" int bm2_mm_gc_memory(const bm2_ctx *ctx, int64_t window_bytes, int64_t *needed) {
+    if (!ctx || window_bytes < 0 || !needed) return 1;
+    // the bins exactly; per record its MmGc, rounded up by 1.25 as bm2_ctx::ensure allocates.  The scan needs nothing more: it reads the hole
+    // letters from the hole list bm2_mm_set uploaded.
+    const double recs = (double) window_bytes / kRecBytes + 1;
+    *needed = (int64_t) ((double) (MM_GC_BINS + GC_NCOUNT) * 8 + 1.25 * recs * sizeof(MmGc));
+    return 0;
+}
+
+extern "C" int bm2_mm_gc_set(bm2_ctx *ctx) {
+    bm2_ctx *ctx_for_error = ctx;
+    if (!ctx) return 1;
+    if (!ctx->mm_set) { bm2_set_error(ctx, "bm2_mm_gc_set: no reference on this context (bm2_mm_set)"); return 1; }
+    BM2_CUDA_OK(cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->stream;
+    DevBuf *b = ctx->mm_d;
+    const int32_t nc = ctx->mm_n_contigs;
+    std::vector<int64_t> off((size_t) nc);
+    std::vector<int32_t> len((size_t) nc);
+    if (nc) {
+        BM2_CUDA_OK(cudaMemcpy(off.data(), b[MD_OFF].p, (size_t) nc * 8, cudaMemcpyDeviceToHost));
+        BM2_CUDA_OK(cudaMemcpy(len.data(), b[MD_LEN].p, (size_t) nc * 4, cudaMemcpyDeviceToHost));
+    }
+    for (int32_t k = 1; k < nc; ++k)
+        if (off[k] < off[k - 1] + len[k - 1]) { bm2_set_error(ctx, "bm2_mm_gc_set: the contigs must be sorted and disjoint"); return 1; }
+    const size_t win = (size_t) MM_GC_BINS * 8, cnt = (size_t) GC_NCOUNT * 8;
+    if (b[MD_GC_WIN].cap < win || b[MD_GC_CNT].cap < cnt) {
+        size_t fr = 0, tot = 0;
+        BM2_CUDA_OK(cudaMemGetInfo(&fr, &tot));
+        if (win + cnt > fr) {
+            bm2_set_error(ctx, "bm2_mm_gc_set: GC bias needs " + std::to_string(win + cnt) + " bytes of device memory, " + std::to_string(fr) + " bytes free");
+            return 1;
+        }
+    }
+    if (ensure_exact(ctx, b[MD_GC_WIN], win) || ensure_exact(ctx, b[MD_GC_CNT], cnt)) return 1;
+    for (cudaEvent_t &ev : ctx->mm_ev) if (!ev) BM2_CUDA_OK(cudaEventCreate(&ev));
+    BM2_CUDA_OK(cudaMemsetAsync(b[MD_GC_WIN].p, 0, win, st));
+    BM2_CUDA_OK(cudaMemsetAsync(b[MD_GC_CNT].p, 0, cnt, st));
+    const int64_t n_tiles = (ctx->mm_l_pac + kScanTile - 1) / kScanTile;
+    // at least one block per 4096 tiles, so that a block's 32-bit shared bins hold its windows (4096 * kScanTile < 2^32)
+    const int64_t grid = bm2_min<int64_t>(n_tiles, bm2_max<int64_t>((int64_t) ctx->n_sm * 8, (n_tiles + 4095) / 4096));
+    BM2_CUDA_OK(cudaEventRecord(ctx->mm_ev[0], st));
+    mm_gc_scan_kernel<<<(unsigned) grid, kScanThreads, 0, st>>>((const uint8_t *) b[MD_PAC].p, (const uint32_t *) b[MD_HOLEBITS].p,
+                                                                 (const int64_t *) b[MD_HOLES].p, (const char *) b[MD_HOLECHAR].p, ctx->mm_n_holes,
+                                                                 ctx->mm_l_pac, (const int64_t *) b[MD_OFF].p, (const int32_t *) b[MD_LEN].p, nc, n_tiles,
+                                                                 (unsigned long long *) b[MD_GC_WIN].p);
+    BM2_CUDA_OK(cudaGetLastError());
+    BM2_CUDA_OK(cudaEventRecord(ctx->mm_ev[1], st));
+    BM2_CUDA_OK(cudaStreamSynchronize(st));
+    float ms = 0;
+    BM2_CUDA_OK(cudaEventElapsedTime(&ms, ctx->mm_ev[0], ctx->mm_ev[1]));
+    ctx->mm_gc_scan_ms = ms; ctx->mm_gc_add_ms = 0;
+    ctx->mm_gc = true;
+    return 0;
+}
+
+extern "C" int bm2_mm_gc_finish(bm2_ctx *ctx, bm2_mm_gc_result_t *out) {
+    bm2_ctx *ctx_for_error = ctx;
+    if (!ctx || !out) { if (ctx) bm2_set_error(ctx, "bm2_mm_gc_finish: bad arguments"); return 1; }
+    if (!ctx->mm_set || !ctx->mm_gc) { bm2_set_error(ctx, "bm2_mm_gc_finish: GC bias is not on for this context (bm2_mm_gc_set)"); return 1; }
+    BM2_CUDA_OK(cudaSetDevice(ctx->device));
+    unsigned long long c[GC_NCOUNT];
+    BM2_CUDA_OK(cudaMemcpy(out->windows, ctx->mm_d[MD_GC_WIN].p, sizeof out->windows, cudaMemcpyDeviceToHost));
+    BM2_CUDA_OK(cudaMemcpy(c, ctx->mm_d[MD_GC_CNT].p, sizeof c, cudaMemcpyDeviceToHost));
+    for (int k = 0; k < MM_GC_BINS; ++k) {
+        out->reads[k] = (int64_t) c[GC_READS + k]; out->bases[k] = (int64_t) c[GC_BASES + k]; out->errors[k] = (int64_t) c[GC_ERRORS + k];
+    }
+    out->total_clusters = (int64_t) c[GC_CLUSTERS]; out->aligned_reads = (int64_t) c[GC_ALIGNED];
+    out->scan_ms = ctx->mm_gc_scan_ms; out->add_ms = ctx->mm_gc_add_ms;
     return 0;
 }

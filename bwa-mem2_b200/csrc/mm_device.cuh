@@ -19,6 +19,17 @@
 //              (htsjdk's SamPairUtil.getPairOrientation, mm_orientation)
 //   errors     a counted record with l_seq 0 or above MM_MAX_LSEQ; an aligned record whose CG:B,I runs past the record, whose refID is not a
 //              contig or whose alignment runs past its contig's end, or whose CIGAR query length is not l_seq (checked in that order)
+//
+// GC bias (CollectGcBiasMetrics at its defaults: SCAN_WINDOW_SIZE 100, MINIMUM_GENOME_FRACTION 1e-5, ALL_READS, no bisulfite, duplicates
+// kept), only when bm2_mm_gc_set turned it on; the formulas and text are mm_gcbias.h's.  Picard's loops are restated from memory:
+//   letters    mm_ref_letter's; G and C are GC, N is N, every other letter (IUPAC S included) neither; the denominator is W = 100, Ns included
+//   windows    per contig of length L, the starts 1 <= i < L - W (Picard's loop skips window 0 and the last full window); a window with more
+//              than 4 Ns is not binned, else its bin is gc * 100 / W; windows never span two contigs
+//   records    counted as above (no 0x100 or 0x800); TOTAL_CLUSTERS without 0x1 or with 0x40; placed (MMB_PLACED): without 0x4, whatever
+//              0x200 and 0x400 say -> ALIGNED_READS, and the span and CIGAR errors above apply to it as to an aligned record.  Its window is
+//              p = pos + 1 forward (Picard's 1-based alignment start used as a 0-based index) or p = pos + ref_len - W reverse; when p is a
+//              counted, binned window of the contig the record adds 1 read start, l_seq bases and its errors (the mismatches over M / = / X,
+//              plus the I and D lengths) to that bin.  Windows at p = L - W or beyond enter no bin (Picard would read bin 0 or fail there).
 #pragma once
 #include "hd.h"
 #include "bam_sort_device.cuh"
@@ -34,7 +45,7 @@ static_assert(MM_NCOUNT == BM2_MM_NCOUNT && MM_NCAT == BM2_MM_NCAT, "bm2_mm_resu
 enum { MM_FR, MM_RF, MM_TANDEM, MM_NORIENT };
 // a record's bits
 enum { MMB_COUNTED = 1, MMB_PF = 2, MMB_NOISE = 4, MMB_ADAPTER = 8, MMB_ALIGNED = 16, MMB_IN_PAIRS = 32, MMB_IMPROPER = 64, MMB_FORWARD = 128,
-       MMB_HQ = 256, MMB_CHIM = 512, MMB_INSERT = 1024, MMB_REV = 2048, MMB_NOQUAL = 4096 };
+       MMB_HQ = 256, MMB_CHIM = 512, MMB_INSERT = 1024, MMB_REV = 2048, MMB_NOQUAL = 4096, MMB_PLACED = 8192 };
 enum { MM_ERR_LSEQ = 1, MM_ERR_SPAN = 2, MM_ERR_CIGAR = 3 };
 
 constexpr int MM_MIN_MAPQ = 20, MM_MIN_BASEQ = 20;
@@ -42,6 +53,7 @@ constexpr int64_t MM_CHIMERA_INSERT = 100000;          // MAX_INSERT_SIZE
 constexpr int32_t MM_MAX_LSEQ = 1 << 20;               // a chosen bound: the per-cycle and per-length arrays stay dense
 constexpr int64_t MM_DENSE_INSERT = 1 << 20;           // insert sizes below this go to dense bins, larger ones to a list
 constexpr int MM_ADAPTER_LEN = 16, MM_N_ADAPTER_KMERS = 12;
+constexpr int MM_GC_W = 100, MM_GC_BINS = 101, MM_GC_MAX_N = 4;  // SCAN_WINDOW_SIZE, the bins 0..100, the most Ns of a binned window
 
 // a record's classification, from the check kernel to the count kernel
 struct MmInfo {
@@ -129,9 +141,10 @@ BM2_HD int32_t mm_sc3(const DupCigar &c, bool rev) {
 }
 
 // the record's classification from its fixed fields, the CIGAR sums s (wgs_cigar_part: aligned, reference, query) and t (mm_clip_part),
-// both summed over all lanes, and whether a CG:B,I CIGAR lies inside the record
+// both summed over all lanes, and whether a CG:B,I CIGAR lies inside the record.  gc (GC bias on): the checks of an aligned record apply to
+// every placed one, which gets MMB_PLACED and g0.
 BM2_HD void mm_classify(const uint8_t *r, const int64_t s[3], const int64_t t[3], bool cigar_inside, const int64_t *contig_off,
-                        const int32_t *contig_len, int32_t n_contigs, const char (*kmers)[MM_ADAPTER_LEN], MmInfo &in) {
+                        const int32_t *contig_len, int32_t n_contigs, const char (*kmers)[MM_ADAPTER_LEN], MmInfo &in, bool gc = false) {
     const BamFixed f = bam_fixed(r);
     in.g0 = 0; in.insert = 0; in.bits = 0; in.err = 0; in.cat = 0; in.aligned = in.softclip = in.hardclip = in.sc3 = in.indels = in.orient = 0;
     in.l_seq = bam_le32(r + 20);
@@ -142,14 +155,15 @@ BM2_HD void mm_classify(const uint8_t *r, const int64_t s[3], const int64_t t[3]
     const uint8_t *seq = r + 36 + f.l_read_name + 4 * (int64_t) f.n_cigar;
     if (seq[(in.l_seq + 1) / 2] == 0xFF) b |= MMB_NOQUAL;
     if (f.flag & 0x10) b |= MMB_REV;
-    const bool pf = !(f.flag & 0x200), aligned = pf && !(f.flag & 4);
-    if (aligned) {
+    const bool pf = !(f.flag & 0x200), aligned = pf && !(f.flag & 4), placed = gc ? !(f.flag & 4) : aligned;
+    if (placed) {
         if (!cigar_inside) { in.err = MM_ERR_CIGAR; return; }
         if (f.rid < 0 || f.rid >= n_contigs || f.pos < 0 || (int64_t) f.pos + s[1] > (int64_t) contig_len[f.rid]) { in.err = MM_ERR_SPAN; return; }
         if (s[2] != in.l_seq) { in.err = MM_ERR_CIGAR; return; }
     }
     const int32_t mrid = bam_le32(r + 24), mpos = bam_le32(r + 28), tlen = bam_le32(r + 32);
     const int64_t ref_len = cigar_inside ? s[1] : 0;
+    if (gc && placed) { b |= MMB_PLACED; in.g0 = contig_off[f.rid] + f.pos; }
     if (pf) {
         b |= MMB_PF;
         if (mm_int_tag_is_one(mm_tag(r, 'X', 'N'))) b |= MMB_NOISE;
@@ -212,4 +226,69 @@ BM2_HD void mm_base(const WgsSeq &sq, bool noqual, int64_t k, int64_t g, const u
                     const char *hole_char, int64_t n_holes, uint32_t &mism, uint32_t &q20) {
     mism += mm_read_letter(mm_nibble(sq.seq, k)) != mm_ref_letter(pac, hole_bits, holes, hole_char, n_holes, g);
     q20 += !noqual && sq.qual[k] >= MM_MIN_BASEQ;
+}
+
+// ---- GC bias ----
+
+// a record's GC bias placement, from the check kernel to the count kernel (GC bias on only)
+struct MmGc {
+    int64_t gw;              // the first locus of the record's window when it is a counted window of the contig (1 <= p < L - W), else -1
+    int64_t idlen;           // the summed I and D lengths
+};
+
+// the summed I and D lengths lane `lane` of `lanes` adds over the CIGAR
+BM2_HD int64_t mm_gc_idlen_part(const DupCigar &c, int lane, int lanes) {
+    int64_t s = 0;
+    for (int64_t k = lane; k < c.n; k += lanes) {
+        const uint32_t op = dup_op(c, k), t = op & 15;
+        if (t == 1 || t == 2) s += op >> 4;
+    }
+    return s;
+}
+
+// the first locus of a placed record's window (ref_len: its CIGAR's reference length), or -1 when the window is not one the reference scan
+// counts; whether the window has more than 4 Ns is left to the caller
+BM2_HD int64_t mm_gc_window(const uint8_t *r, int64_t ref_len, const int64_t *contig_off, const int32_t *contig_len) {
+    const BamFixed f = bam_fixed(r);
+    const int64_t p = (f.flag & 0x10) ? (int64_t) f.pos + ref_len - MM_GC_W : (int64_t) f.pos + 1;
+    return p >= 1 && p < (int64_t) contig_len[f.rid] - MM_GC_W ? contig_off[f.rid] + p : -1;
+}
+
+// a reference letter's class: 1 GC, 2 N, 0 neither
+BM2_HD int mm_gc_class(char c) { return c == 'G' || c == 'C' ? 1 : c == 'N' ? 2 : 0; }
+
+// the bin of a window with gc GC letters and n Ns, or -1 when it is not binned
+BM2_HD int mm_gc_bin(int gc, int n) { return n > MM_GC_MAX_N ? -1 : gc * 100 / MM_GC_W; }
+
+// the GC and N bitsets of locus word w (loci 32w .. 32w + 31, bit k for locus 32w + k; no bit at or past l_pac): ACGT[pac code] outside the
+// holes, the hole's letter (upper case) inside, found by a binary search of the holes as wgs_range_word does
+BM2_HD void mm_gc_word(const uint8_t *pac, const uint32_t *hole_bits, const int64_t *holes, const char *hole_char, int64_t n_holes, int64_t l_pac,
+                       int64_t w, uint32_t &gcm, uint32_t &nm) {
+    gcm = nm = 0;
+    const int64_t b = w * 32;
+    if (b >= l_pac) return;
+    const int64_t pb = (l_pac + 3) / 4;
+    uint64_t v = 0;
+    if (8 * w + 8 <= pb) v = *(const uint64_t *) (pac + 8 * w);
+    else for (int64_t j = 8 * w; j < pb; ++j) v |= (uint64_t) pac[j] << (8 * (j - 8 * w));
+    for (int k = 0; k < 32; ++k) {
+        const uint32_t code = (uint32_t) (v >> (8 * (k >> 2) + 2 * (3 - (k & 3)))) & 3;
+        gcm |= ((code ^ (code >> 1)) & 1) << k;                         // C (1) and G (2)
+    }
+    const uint32_t hb = hole_bits[w];
+    if (hb) {
+        gcm &= ~hb;
+        int64_t lo = 0, hi = n_holes;                                    // the first hole ending after b
+        while (lo < hi) { const int64_t m = (lo + hi) / 2; if (holes[2 * m + 1] <= b) lo = m + 1; else hi = m; }
+        for (int64_t h = lo; h < n_holes && holes[2 * h] < b + 32; ++h) {
+            const int64_t x = bm2_max(holes[2 * h], b) - b, y = bm2_min(holes[2 * h + 1], b + 32) - b;
+            const uint32_t m = (y - x >= 32 ? ~0u : ((1u << (y - x)) - 1)) << x;
+            char c = hole_char[h];
+            c = c >= 'a' && c <= 'z' ? (char) (c - 32) : c;
+            const int cls = mm_gc_class(c);
+            if (cls == 1) gcm |= m;
+            if (cls == 2) nm |= m;
+        }
+    }
+    if (b + 32 > l_pac) { const uint32_t keep = (1u << (l_pac - b)) - 1; gcm &= keep; nm &= keep; }
 }

@@ -728,6 +728,27 @@ int  bm2_mm_memory(const bm2_ctx *ctx, int64_t l_pac, int64_t window_bytes, int6
 int  bm2_mm_add(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int64_t *starts, int64_t n_recs);
 /* The counters and histograms since bm2_mm_set, copied back up to their largest keys.  It may be called again. */
 int  bm2_mm_finish(bm2_ctx *ctx, bm2_mm_result_t *out);
+/* GC bias (Picard CollectGcBiasMetrics at its defaults, csrc/mm_device.cuh's rule, csrc/mm_gcbias.h's formulas; byte equality with Picard is
+ * not claimed).  bm2_mm_gc_set, after bm2_mm_set, bins the reference's 100-base windows by GC (windows 1 <= i < L - 100 of each contig, those
+ * with more than 4 Ns left out) and turns GC counting on for the bm2_mm_add calls that follow, until the next bm2_mm_set.  With it on, every
+ * counted record without 0x4 gets the checks of an aligned record (a read error otherwise), and a record whose window is binned adds a read
+ * start, its l_seq and its errors (mismatches plus I and D lengths) to the window's bin.  The contigs must be sorted and disjoint.  Device
+ * memory it cannot get is an error that gives the bytes needed and free. */
+#define BM2_MM_GC_BINS 101
+typedef struct {
+    int64_t windows[BM2_MM_GC_BINS];       /* reference windows by GC                                                                */
+    int64_t reads[BM2_MM_GC_BINS];         /* read starts by the GC of their window                                                  */
+    int64_t bases[BM2_MM_GC_BINS];         /* their l_seq, summed                                                                    */
+    int64_t errors[BM2_MM_GC_BINS];        /* their mismatches, I and D lengths, summed                                              */
+    int64_t total_clusters;                /* counted records without 0x1 or with 0x40                                               */
+    int64_t aligned_reads;                 /* counted records without 0x4                                                            */
+    double scan_ms, add_ms;                /* device time of the reference scan, and of the bm2_mm_add kernels since bm2_mm_gc_set   */
+} bm2_mm_gc_result_t;
+int  bm2_mm_gc_set(bm2_ctx *ctx);
+/* Device bytes GC bias adds to bm2_mm_memory's figure for windows of window_bytes. */
+int  bm2_mm_gc_memory(const bm2_ctx *ctx, int64_t window_bytes, int64_t *needed);
+/* The GC bias counts since bm2_mm_gc_set.  It may be called again. */
+int  bm2_mm_gc_finish(bm2_ctx *ctx, bm2_mm_gc_result_t *out);
 
 /* Staged mate rescue inside bm2_sam_pe (same records, other kernels): the windows mem_matesw (src/bwamem_pair.cpp:150-283) can ask for are
  * listed for all pairs of a wave from the regions before any rescue, aligned as one batch with one window per warp (the job shape of
