@@ -276,7 +276,8 @@ EXPORTS = ["bm2_create_sibling", "bm2_fastq_encode", "bm2_seq_encode", "bm2_fast
            "bm2_bqsr_sites", "bm2_bqsr_count", "bm2_bqsr_tables", "bm2_bqsr_apply_set", "bm2_bqsr_apply", "bm2_last_bqsr_apply_stats",
            "bm2_bqsr_apply_memory", "bm2_wgs_set", "bm2_wgs_memory", "bm2_wgs_add", "bm2_wgs_finish",
            "bm2_mm_set", "bm2_mm_memory", "bm2_mm_add", "bm2_mm_finish", "bm2_mm_gc_set", "bm2_mm_gc_memory", "bm2_mm_gc_finish", "bm2_markdup_set", "bm2_markdup_records", "bm2_markdup_pair", "bm2_markdup_counts",
-           "bm2_markdup_mark", "bm2_last_markdup_stats", "bm2_markdup_memory", "bm2_recal_memory", "bm2_recal_set", "bm2_recal_add", "bm2_recal_tables"]
+           "bm2_markdup_mark", "bm2_last_markdup_stats", "bm2_markdup_memory", "bm2_recal_memory", "bm2_recal_set", "bm2_recal_add", "bm2_recal_tables",
+           "bm2_bam2fq_records", "bm2_bam2fq_format", "bm2_last_bam2fq_stats", "bm2_bam2fq_memory"]
 
 _lib = None
 
@@ -940,6 +941,50 @@ class Context:
         f = lib().bm2_last_markdup_stats
         f.argtypes = [C.c_void_p, C.c_void_p]
         self._check(f(self._ctx, v), "bm2_last_markdup_stats")
+        return tuple(v)
+
+    def bam2fq_records(self, data: bytes, starts, suffixes: bool):
+        """bm2_bam2fq_records: one window of records (uncompressed BAM at starts, contiguous) -> structured array of bm2_bam2fq_rec
+        (hash, text_len, kind).  The window stays on the device for bam2fq_format.  A read error raises Bm2Error naming the read."""
+        starts = np.ascontiguousarray(starts, np.int64)
+        buf = np.frombuffer(data, np.uint8) if len(data) else np.zeros(1, np.uint8)
+        sb = starts if len(starts) else np.zeros(1, np.int64)
+        out = C.c_void_p()
+        f = lib().bm2_bam2fq_records
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p]
+        self._check(f(self._ctx, buf.ctypes.data, len(data), sb.ctypes.data, len(starts), int(bool(suffixes)), C.byref(out)), "bm2_bam2fq_records")
+        dt = np.dtype([("hash", "<u8"), ("text_len", "<i8"), ("kind", "<i4"), ("pad", "<i4")])
+        if not len(starts):
+            return np.zeros(0, dt)
+        return np.frombuffer((C.c_uint8 * (len(starts) * dt.itemsize)).from_address(out.value), dt).copy()
+
+    def bam2fq_format(self, order, extra_recs, suffixes: bool, carry: bytes = b"", compress: bool = False, last: bool = True):
+        """bm2_bam2fq_format: order lists record i of the last bam2fq_records window as i and record k of extra_recs (a list of record
+        bytes) as ~k -> (data, tail, text_len): the text, or with compress the BGZF members and the unfinished block."""
+        lst = np.ascontiguousarray(list(order) + [0], np.int64)
+        xb = b"".join(extra_recs)
+        xbuf = np.frombuffer(xb + b"\0", np.uint8)
+        xs = np.ascontiguousarray(np.cumsum([0] + [len(r) for r in extra_recs])[:-1].tolist() + [0], np.int64)
+        cb = np.frombuffer(carry + b"\0", np.uint8)
+
+        class Out(C.Structure):
+            _fields_ = [("data", C.c_void_p), ("len", C.c_int64), ("tail", C.c_void_p), ("tail_len", C.c_int64), ("text_len", C.c_int64)]
+        o = Out()
+        f = lib().bm2_bam2fq_format
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int64, C.c_int32,
+                      C.c_int32, C.c_void_p]
+        self._check(f(self._ctx, lst.ctypes.data, len(lst) - 1, xbuf.ctypes.data, len(xb), xs.ctypes.data, len(extra_recs), int(bool(suffixes)),
+                      cb.ctypes.data, len(carry), int(bool(compress)), int(bool(last)), C.byref(o)), "bm2_bam2fq_format")
+        data = C.string_at(o.data, o.len) if o.len else b""
+        tail = C.string_at(o.tail, o.tail_len) if o.tail_len else b""
+        return data, tail, int(o.text_len)
+
+    def bam2fq_stats(self):
+        """bm2_last_bam2fq_stats -> (record_ms, format_ms, bgzf_ms)."""
+        v = (C.c_double * 3)()
+        f = lib().bm2_last_bam2fq_stats
+        f.argtypes = [C.c_void_p, C.c_void_p]
+        self._check(f(self._ctx, v), "bm2_last_bam2fq_stats")
         return tuple(v)
 
     def mm_add(self, data: bytes, starts):

@@ -170,6 +170,15 @@ struct bm2_ctx {
     double rcl_ms = 0;
     std::string rcl_err_name;
     std::vector<int64_t> rcl_tables;
+    // bm2_bam2fq_records / bm2_bam2fq_format (bam2fq.cu): buffers (the window stays for the format calls), the window's record count,
+    // events, the device times, the last calls' outputs
+    DevBuf b2f_d[11];
+    HostBuf b2f_h[2];
+    int64_t b2f_n_recs = 0;
+    cudaEvent_t b2f_ev[4] = {nullptr, nullptr, nullptr, nullptr};
+    double b2f_record_ms = 0, b2f_format_ms = 0, b2f_bgzf_ms = 0;
+    std::vector<bm2_bam2fq_rec> b2f_recs;
+    std::vector<uint8_t> b2f_tail;
 
     int ensure(DevBuf &b, size_t bytes);
     int ensure_host(HostBuf &b, size_t bytes);
@@ -177,12 +186,12 @@ struct bm2_ctx {
         std::vector<DevBuf *> v = {&io_pairs, &io_ref, &io_qer, &bsw_jobs, &bsw_outs, &bsw_scratch, &dup_bits};
         append(v, pipe_d); append(v, cigar_d); append(v, sam_d); append(v, ksw_d); append(v, fq_d);
         append(v, bgzf_d); append(v, sort_d); append(v, dup_d); append(v, bqsr_d); append(v, bqa_d); append(v, wgs_d);
-        append(v, mm_d); append(v, mdb_d); append(v, rcl_d);
+        append(v, mm_d); append(v, mdb_d); append(v, rcl_d); append(v, b2f_d);
         return v;
     }
     std::vector<HostBuf *> all_host() {
         std::vector<HostBuf *> v;
-        append(v, pipe_h); append(v, cigar_h); append(v, sam_h); append(v, fq_h); append(v, bgzf_h); append(v, sort_h); append(v, bqa_h); append(v, mdb_h);
+        append(v, pipe_h); append(v, cigar_h); append(v, sam_h); append(v, fq_h); append(v, bgzf_h); append(v, sort_h); append(v, bqa_h); append(v, mdb_h); append(v, b2f_h);
         return v;
     }
     template <class B, size_t N> static void append(std::vector<B *> &v, B (&t)[N]) { for (B &x : t) v.push_back(&x); }
@@ -206,3 +215,6 @@ int bqsr_count_done(bm2_ctx *ctx, const uint8_t *d_base, const int64_t *h_starts
 // out gets the members, carry_v and recs_v (the records' bm2_sort_rec, copied from recs)
 int bam_compress_stream(bm2_ctx *ctx, const uint8_t *d_stream, int64_t carry_len, const int64_t *offs, int64_t n_recs, int64_t total, int last,
                         bm2_sort_rec *recs, DevBuf *gather, std::vector<uint8_t> &carry_v, std::vector<bm2_sort_rec> &recs_v, bm2_sort_out *out);
+// markdup_bam.cu: 0 when the n_recs records at starts (HOST) are whole, each where the one before ends, the last ending at n; otherwise the
+// context's error names fn and the record, and 1 is returned
+int bam_check_records(bm2_ctx *ctx, const char *fn, const uint8_t *recs, int64_t n, const int64_t *starts, int64_t n_recs);

@@ -199,6 +199,7 @@ extern "C" void bm2_destroy(bm2_ctx *ctx) {
     for (cudaEvent_t ev : ctx->bqa_ev) if (ev) cudaEventDestroy(ev);
     for (cudaEvent_t ev : ctx->mm_ev) if (ev) cudaEventDestroy(ev);
     for (cudaEvent_t ev : ctx->mdb_ev) if (ev) cudaEventDestroy(ev);
+    for (cudaEvent_t ev : ctx->b2f_ev) if (ev) cudaEventDestroy(ev);
     bm2_free_index(ctx);
     for (DevBuf *b : ctx->all_dev()) if (b->p) cudaFree(b->p);
     for (HostBuf *b : ctx->all_host()) if (b->p) cudaFreeHost(b->p);

@@ -128,8 +128,10 @@ static_assert(MB_END == std::extent<decltype(bm2_ctx::mdb_d)>::value, "bm2_ctx::
 static_assert(MH_END == std::extent<decltype(bm2_ctx::mdb_h)>::value, "bm2_ctx::mdb_h: one buffer per slot");
 static_assert(sizeof(bm2_markdup_rec) == 48 && sizeof(bm2_markdup_half) == 24, "bm2_markdup_rec, bm2_markdup_half: no padding, as the Python bindings read them");
 
+}  // namespace
+
 // the records at starts are whole, each where the one before ends, the last ending at n
-int check_records(bm2_ctx *ctx, const char *fn, const uint8_t *recs, int64_t n, const int64_t *starts, int64_t n_recs) {
+int bam_check_records(bm2_ctx *ctx, const char *fn, const uint8_t *recs, int64_t n, const int64_t *starts, int64_t n_recs) {
     for (int64_t i = 0, at = 0; i <= n_recs; ++i) {
         if (i == n_recs) { if (at != n) { bm2_set_error(ctx, std::string(fn) + ": the records do not end where the buffer ends"); return 1; } break; }
         const int64_t s = starts[i];
@@ -145,8 +147,6 @@ int check_records(bm2_ctx *ctx, const char *fn, const uint8_t *recs, int64_t n, 
     }
     return 0;
 }
-
-}  // namespace
 
 extern "C" int bm2_markdup_set(bm2_ctx *ctx, int32_t n_ids, const char *const *ids, const int32_t *libs, int32_t n_lib, int32_t unknown_lib) {
     bm2_ctx *ctx_for_error = ctx;
@@ -188,7 +188,7 @@ extern "C" int bm2_markdup_records(bm2_ctx *ctx, const uint8_t *recs, int64_t n,
         return 1;
     }
     if (!ctx->mdb_set) { bm2_set_error(ctx, "bm2_markdup_records: no read groups on this context (bm2_markdup_set)"); return 1; }
-    if (check_records(ctx, "bm2_markdup_records", recs, n, starts, n_recs)) return 1;
+    if (bam_check_records(ctx, "bm2_markdup_records", recs, n, starts, n_recs)) return 1;
     BM2_CUDA_OK(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
     DevBuf *b = ctx->mdb_d;
@@ -290,7 +290,7 @@ extern "C" int bm2_markdup_mark(bm2_ctx *ctx, const uint8_t *recs, int64_t n, co
         return 1;
     }
     if (!ctx->mdb_set) { bm2_set_error(ctx, "bm2_markdup_mark: no read groups on this context (bm2_markdup_set)"); return 1; }
-    if (check_records(ctx, "bm2_markdup_mark", recs, n, starts, n_recs)) return 1;
+    if (bam_check_records(ctx, "bm2_markdup_mark", recs, n, starts, n_recs)) return 1;
     memset(out, 0, sizeof *out);
     BM2_CUDA_OK(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;

@@ -750,6 +750,36 @@ int  bm2_mm_gc_memory(const bm2_ctx *ctx, int64_t window_bytes, int64_t *needed)
 /* The GC bias counts since bm2_mm_gc_set.  It may be called again. */
 int  bm2_mm_gc_finish(bm2_ctx *ctx, bm2_mm_gc_result_t *out);
 
+/* ---- BAM back to FASTQ (bm2_bam2fq) -----------------------------------------------------------------------------------------------------
+ * The rule (csrc/bam2fq_device.cuh, the host half csrc/bam2fq.h) follows `samtools fastq` at its defaults where it can; byte equality with
+ * samtools is not claimed.  The GPU classifies and checks each record and writes the FASTQ text; the mates are joined by bm2_markdup_pair
+ * with one read group, and the host keeps the order of the output. */
+enum { BM2_B2F_SKIP = 0, BM2_B2F_READ1 = 1, BM2_B2F_READ2 = 2, BM2_B2F_OTHER = 3 };
+/* One record: hash, the 64-bit FNV-1a hash of its QNAME (a READ1 or READ2 only); text_len, the bytes of its text (0 when skipped); kind. */
+typedef struct { uint64_t hash; int64_t text_len; int32_t kind, pad; } bm2_bam2fq_rec;   /* 24 bytes */
+/* One call's output (HOST, owned by the context, valid until its next call): data, the text, or with compression the BGZF members of the
+ * blocks completed; tail, the bytes of the unfinished block (compression without last only); text_len, the text bytes this call formatted. */
+typedef struct { const uint8_t *data; int64_t len; const uint8_t *tail; int64_t tail_len, text_len; } bm2_bam2fq_out;
+typedef struct { double record_ms, format_ms, bgzf_ms; } bm2_bam2fq_stats_t;
+/* One window of whole records (HOST, contiguous, each where the one before ends), one warp per record: *out (HOST, n_recs, owned by the
+ * context, valid until its next call) gets each record's bm2_bam2fq_rec, with /1 and /2 counted in text_len when suffixes is set.  A kept
+ * record with l_seq 0 or a quality above 93 is a read error: the first by index is named in the error and 2 is returned, with nothing of
+ * the window kept.  Otherwise the window stays on the device for the bm2_bam2fq_format calls that follow. */
+int  bm2_bam2fq_records(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int64_t *starts, int64_t n_recs, int32_t suffixes,
+                        const bm2_bam2fq_rec **out);
+/* The text of one output stream: list[i] >= 0 is record list[i] of the last bm2_bam2fq_records window, list[i] < 0 record ~list[i] of
+ * extra (HOST, n_extra records at extra_starts, such as halves carried from earlier windows).  The lengths come from a device scan and one
+ * warp writes each record.  With compress, carry (the tail of the stream's previous call) and the text are cut into blocks of exactly 65280
+ * bytes; the full blocks are compressed on the GPU and the rest is the tail, or with last its member too.  Without compress, data is the
+ * text. */
+int  bm2_bam2fq_format(bm2_ctx *ctx, const int64_t *list, int64_t n_list, const uint8_t *extra, int64_t extra_len, const int64_t *extra_starts,
+                       int64_t n_extra, int32_t suffixes, const uint8_t *carry, int64_t carry_len, int32_t compress, int32_t last, bm2_bam2fq_out *out);
+/* Device ms (CUDA events) since the context was made: the record kernel, the scan and format kernels, BGZF. */
+int  bm2_last_bam2fq_stats(const bm2_ctx *ctx, bm2_bam2fq_stats_t *out);
+/* Device bytes bm2_bam2fq_records, bm2_markdup_pair and bm2_bam2fq_format need for windows of window_bytes of records of about 300 bytes,
+ * and the bytes free on ctx's device now. */
+int  bm2_bam2fq_memory(const bm2_ctx *ctx, int64_t window_bytes, int64_t *needed, int64_t *free_bytes);
+
 /* Staged mate rescue inside bm2_sam_pe (same records, other kernels): the windows mem_matesw (src/bwamem_pair.cpp:150-283) can ask for are
  * listed for all pairs of a wave from the regions before any rescue, aligned as one batch with one window per warp (the job shape of
  * bm2_ksw_align2; the reference batches the same alignments across pairs in its kswv path, src/bwamem_pair.cpp:930-1248, src/kswv.cpp),
