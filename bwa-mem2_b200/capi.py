@@ -277,7 +277,8 @@ EXPORTS = ["bm2_create_sibling", "bm2_fastq_encode", "bm2_seq_encode", "bm2_fast
            "bm2_bqsr_apply_memory", "bm2_wgs_set", "bm2_wgs_memory", "bm2_wgs_add", "bm2_wgs_finish",
            "bm2_mm_set", "bm2_mm_memory", "bm2_mm_add", "bm2_mm_finish", "bm2_mm_gc_set", "bm2_mm_gc_memory", "bm2_mm_gc_finish", "bm2_markdup_set", "bm2_markdup_records", "bm2_markdup_pair", "bm2_markdup_counts",
            "bm2_markdup_mark", "bm2_last_markdup_stats", "bm2_markdup_memory", "bm2_recal_memory", "bm2_recal_set", "bm2_recal_add", "bm2_recal_tables",
-           "bm2_bam2fq_records", "bm2_bam2fq_format", "bm2_last_bam2fq_stats", "bm2_bam2fq_memory"]
+           "bm2_bam2fq_records", "bm2_bam2fq_format", "bm2_last_bam2fq_stats", "bm2_bam2fq_memory",
+           "bm2_bam_qname_sort_compress", "bm2_bam_qname_sort_memory"]
 
 _lib = None
 
@@ -611,6 +612,34 @@ class Context:
         sizes = _host(o.member_size, o.n_members, np.int32) if o.n_members else np.zeros(0, np.int32)
         return dict(z=C.string_at(o.z, o.z_len) if o.z_len else b"", member_size=sizes, carry=C.string_at(o.carry, o.carry_len) if o.carry_len else b"",
                     recs=recs, ms=dict(keys=ms[0], sort=ms[1], gather=ms[2], bgzf=ms[3]))
+
+    def bam_qname_sort_compress(self, data: bytes, starts, carry: bytes = b"", last: bool = True):
+        """bm2_bam_qname_sort_compress: bam_sort_compress in read-name order (samtools sort -n: the names by samtools' strnum_cmp, then
+        flag & 0xc0, then input order) -> bam_sort_compress's dict (ms: device ms of keys, merge sort, gather, BGZF)."""
+        starts = np.ascontiguousarray(starts, np.int64)
+        buf = np.frombuffer(data, np.uint8) if len(data) else np.zeros(1, np.uint8)
+        cb = np.frombuffer(carry, np.uint8) if len(carry) else np.zeros(1, np.uint8)
+        o = SortOut()
+        f = lib().bm2_bam_qname_sort_compress
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int, C.c_void_p]
+        self._check(f(self._ctx, buf.ctypes.data, len(data), starts.ctypes.data, len(starts), cb.ctypes.data, len(carry), int(last), C.byref(o)),
+                    "bm2_bam_qname_sort_compress")
+        ms = (C.c_double * 4)()
+        lib().bm2_last_sort_stats.argtypes = [C.c_void_p, C.c_void_p]
+        lib().bm2_last_sort_stats(self._ctx, ms)
+        recs = np.ctypeslib.as_array(C.cast(o.recs, C.POINTER(C.c_uint8)), shape=(o.n_recs * SORT_REC_DT.itemsize,)).view(SORT_REC_DT).copy() \
+            if o.n_recs else np.zeros(0, SORT_REC_DT)
+        sizes = _host(o.member_size, o.n_members, np.int32) if o.n_members else np.zeros(0, np.int32)
+        return dict(z=C.string_at(o.z, o.z_len) if o.z_len else b"", member_size=sizes, carry=C.string_at(o.carry, o.carry_len) if o.carry_len else b"",
+                    recs=recs, ms=dict(keys=ms[0], sort=ms[1], gather=ms[2], bgzf=ms[3]))
+
+    def bam_qname_sort_memory(self, run_bytes: int):
+        """bm2_bam_qname_sort_memory -> (bytes needed, bytes free)."""
+        need, free = C.c_int64(), C.c_int64()
+        f = lib().bm2_bam_qname_sort_memory
+        f.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+        self._check(f(self._ctx, int(run_bytes), C.byref(need), C.byref(free)), "bm2_bam_qname_sort_memory")
+        return need.value, free.value
 
     def bam_sort_compress_ex(self, data: bytes, starts, tids, carry: bytes = b"", last: bool = True):
         """bm2_bam_sort_compress_ex: bam_sort_compress with each record's template id (int64[]) carried through the sort; records of the

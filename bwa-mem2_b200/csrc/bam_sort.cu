@@ -9,6 +9,11 @@
 //   gather      one warp per record, 16-byte copies when source and destination agree modulo 16
 //   BGZF        the blocks are cut on the host (bam_sort_layout) from the scan, and bm2_bgzf_compress's kernels compress them straight from the
 //               sorted device buffer; the unfinished last block goes back as the carry (bam_compress_stream, which bm2_bqsr_apply shares)
+// bm2_bam_qname_sort_compress (bm2_sort -n) is the same code with only the keys and sort stages changed:
+//   keys        the same key kernel (the index data and lengths), then one thread per record writes its 8-byte entry: the offset of its QNAME in
+//               the uploaded buffer and its flag & 0xc0 (bam_qname_entry); the names are not copied
+//   sort        cub::DeviceMergeSort::SortKeys over the 32-bit ordinals with bam_qname_cmp (bam_sort_device.cuh) as the comparison: names,
+//               then flag bits, then ordinal, a total order, so ties keep input order
 // bm2_bam_sort_compress_ex is the same code with one template id per record carried through the permutation; with a duplicate bitset on the
 // context (bm2_dup_set, markdup.cu) the key kernel sets 0x400 in the index data of the records of duplicate templates and the gather writes it
 // into the copied record.  With counting armed (bm2_bqsr_sites, bqsr.cu), the sorted records are counted for the recalibration tables after
@@ -17,6 +22,7 @@
 #include "bm2_ctx.h"
 #include "bam_sort_device.cuh"
 #include "markdup_device.cuh"
+#include <cub/device/device_merge_sort.cuh>
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 #include <vector>
@@ -91,6 +97,29 @@ __global__ void sort_gather_kernel(const uint8_t *__restrict__ in, const int64_t
     }
 }
 
+// name order: one thread per record, its entry and its ordinal
+__global__ void qname_key_kernel(const uint8_t *__restrict__ in, const int64_t *__restrict__ starts, int64_t n, uint64_t *ent, uint32_t *ord) {
+    const int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    ent[i] = bam_qname_entry(in + starts[i], starts[i]);
+    ord[i] = (uint32_t) i;
+}
+
+// the name order of two ordinals, through their entries into the uploaded records
+struct QnameLess {
+    const uint8_t *in; const uint64_t *ent;
+    __device__ bool operator()(uint32_t a, uint32_t b) const {
+        const uint64_t x = ent[a], y = ent[b];
+        return bam_qname_cmp(in + (x >> 8), (uint32_t) (x & 0xc0), a, in + (y >> 8), (uint32_t) (y & 0xc0), b) < 0;
+    }
+};
+
+size_t qname_sort_temp(int64_t n, cudaStream_t st, cudaError_t *e) {
+    size_t t = 0;
+    *e = cub::DeviceMergeSort::SortKeys(nullptr, t, (uint32_t *) nullptr, n, QnameLess{nullptr, nullptr}, st);
+    return t;
+}
+
 enum { SD_IN, SD_STARTS, SD_INFO, SD_LEN, SD_KEYS0, SD_KEYS1, SD_VALS0, SD_VALS1, SD_LENS, SD_OFFS, SD_TEMP, SD_OUT, SD_SINFO, SD_MAX, SD_TIDS,
        SD_STIDS, SD_END };
 enum { SH_OFFS, SH_INFO, SH_END };
@@ -101,26 +130,28 @@ int bits_of(uint64_t v) { int b = 0; while (v >> b) ++b; return b; }
 
 }  // namespace
 
-// bm2_bam_sort_compress and bm2_bam_sort_compress_ex: tids (may be NULL) carried into ctx->sort_tids; marking when tids and a bitset are there
+// bm2_bam_sort_compress and bm2_bam_sort_compress_ex: tids (may be NULL) carried into ctx->sort_tids; marking when tids and a bitset are there.
+// by_name: bm2_bam_qname_sort_compress (no tids)
 static int sort_compress(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int64_t *starts, int64_t n_recs, const int64_t *tids, const uint8_t *carry,
-                         int64_t carry_len, int last, bm2_sort_out *out) {
+                         int64_t carry_len, int last, bm2_sort_out *out, bool by_name = false) {
     bm2_ctx *ctx_for_error = ctx;
+    const std::string what = by_name ? "bm2_bam_qname_sort_compress" : "bm2_bam_sort_compress";
     if (!ctx || !out || n < 0 || (n && !recs) || n_recs < 0 || (n_recs && !starts) || carry_len < 0 || carry_len >= BGZF_BLOCK ||
         (carry_len && !carry)) {
-        if (ctx) bm2_set_error(ctx, "bm2_bam_sort_compress: bad arguments");
+        if (ctx) bm2_set_error(ctx, what + ": bad arguments");
         return 1;
     }
     const bool mark = tids && ctx->dup_n_bits > 0;
-    if (n_recs >= (1LL << 31) - 1) { bm2_set_error(ctx, "bm2_bam_sort_compress: 2^31-1 records or more in one call"); return 1; }
+    if (n_recs >= (1LL << 31) - 1) { bm2_set_error(ctx, what + ": 2^31-1 records or more in one call"); return 1; }
     for (int64_t i = 0; i < n_recs; ++i) {                       // each record whole inside the buffer, in order, not overlapping the next
         const int64_t s = starts[i];
         if (s < 0 || s + 36 > n || (i && s < starts[i - 1] + 4 + (int64_t) bam_le32(recs + starts[i - 1]))) {
-            bm2_set_error(ctx, "bm2_bam_sort_compress: record " + std::to_string(i) + " does not lie within the buffer after the one before");
+            bm2_set_error(ctx, what + ": record " + std::to_string(i) + " does not lie within the buffer after the one before");
             return 1;
         }
         const int64_t m = 4 + (int64_t) bam_le32(recs + s);
         const int32_t rid = bam_le32(recs + s + 4);
-        if (m < 36 || s + m > n || rid < -1) { bm2_set_error(ctx, "bm2_bam_sort_compress: record " + std::to_string(i) + " is malformed"); return 1; }
+        if (m < 36 || s + m > n || rid < -1) { bm2_set_error(ctx, what + ": record " + std::to_string(i) + " is malformed"); return 1; }
     }
     memset(out, 0, sizeof *out);
     for (double &x : ctx->sort_ms) x = 0;
@@ -129,9 +160,15 @@ static int sort_compress(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int
     DevBuf *b = ctx->sort_d;
     const int64_t nr = n_recs;
     size_t temp = 0;
-    {
+    if (by_name) {
+        cudaError_t e;
+        temp = qname_sort_temp(bm2_max<int64_t>(nr, 1), st, &e);
+        BM2_CUDA_OK(e);
+    } else {
         cub::DoubleBuffer<uint64_t> k((uint64_t *) nullptr, nullptr); cub::DoubleBuffer<uint32_t> v((uint32_t *) nullptr, nullptr);
         BM2_CUDA_OK(cub::DeviceRadixSort::SortPairs(nullptr, temp, k, v, (int) bm2_max<int64_t>(nr, 1), 0, 64, st));
+    }
+    {
         size_t t2 = 0;
         BM2_CUDA_OK(cub::DeviceScan::ExclusiveSum(nullptr, t2, (int64_t *) nullptr, (int64_t *) nullptr, (int) nr + 1, st));
         temp = bm2_max(temp, t2);
@@ -163,19 +200,29 @@ static int sort_compress(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int
                                            (int64_t *) b[SD_LEN].p, (unsigned *) b[SD_MAX].p, d_tids,
                                            mark ? (const uint64_t *) ctx->dup_bits.p : nullptr, ctx->dup_n_bits);
         BM2_CUDA_OK(cudaGetLastError());
+        if (by_name) {                                          // the entries in the key buffer, the ordinals in the value buffer
+            qname_key_kernel<<<g, 256, 0, st>>>((const uint8_t *) b[SD_IN].p, (const int64_t *) b[SD_STARTS].p, nr, (uint64_t *) b[SD_KEYS0].p,
+                                                (uint32_t *) b[SD_VALS0].p);
+            BM2_CUDA_OK(cudaGetLastError());
+        }
         BM2_CUDA_OK(cudaEventRecord(ctx->sort_ev[1], st));
-        unsigned mx[2] = { 0, 0 };
-        BM2_CUDA_OK(cudaMemcpyAsync(mx, b[SD_MAX].p, 8, cudaMemcpyDeviceToHost, st));
-        BM2_CUDA_OK(cudaStreamSynchronize(st));
-        const int pos_bits = bits_of(mx[1]), end_bit = bm2_max(1, bits_of(mx[0]) + pos_bits + 1);   // ranks 0..mx[0] (mx[0]: refID -1)
-        sort_pack_kernel<<<g, 256, 0, st>>>((const bm2_sort_rec *) b[SD_INFO].p, nr, mx[0], pos_bits, (uint64_t *) b[SD_KEYS0].p,
-                                            (uint32_t *) b[SD_VALS0].p);
-        BM2_CUDA_OK(cudaGetLastError());
-        cub::DoubleBuffer<uint64_t> kb((uint64_t *) b[SD_KEYS0].p, (uint64_t *) b[SD_KEYS1].p);
-        cub::DoubleBuffer<uint32_t> vb((uint32_t *) b[SD_VALS0].p, (uint32_t *) b[SD_VALS1].p);
         size_t tb = b[SD_TEMP].cap;
-        BM2_CUDA_OK(cub::DeviceRadixSort::SortPairs(b[SD_TEMP].p, tb, kb, vb, (int) nr, 0, end_bit, st));
-        ord = vb.Current();
+        if (by_name) {
+            BM2_CUDA_OK(cub::DeviceMergeSort::SortKeys(b[SD_TEMP].p, tb, (uint32_t *) b[SD_VALS0].p, nr,
+                                                       QnameLess{(const uint8_t *) b[SD_IN].p, (const uint64_t *) b[SD_KEYS0].p}, st));
+        } else {
+            unsigned mx[2] = { 0, 0 };
+            BM2_CUDA_OK(cudaMemcpyAsync(mx, b[SD_MAX].p, 8, cudaMemcpyDeviceToHost, st));
+            BM2_CUDA_OK(cudaStreamSynchronize(st));
+            const int pos_bits = bits_of(mx[1]), end_bit = bm2_max(1, bits_of(mx[0]) + pos_bits + 1);   // ranks 0..mx[0] (mx[0]: refID -1)
+            sort_pack_kernel<<<g, 256, 0, st>>>((const bm2_sort_rec *) b[SD_INFO].p, nr, mx[0], pos_bits, (uint64_t *) b[SD_KEYS0].p,
+                                                (uint32_t *) b[SD_VALS0].p);
+            BM2_CUDA_OK(cudaGetLastError());
+            cub::DoubleBuffer<uint64_t> kb((uint64_t *) b[SD_KEYS0].p, (uint64_t *) b[SD_KEYS1].p);
+            cub::DoubleBuffer<uint32_t> vb((uint32_t *) b[SD_VALS0].p, (uint32_t *) b[SD_VALS1].p);
+            BM2_CUDA_OK(cub::DeviceRadixSort::SortPairs(b[SD_TEMP].p, tb, kb, vb, (int) nr, 0, end_bit, st));
+            ord = vb.Current();
+        }
         BM2_CUDA_OK(cudaEventRecord(ctx->sort_ev[2], st));
         sort_permute_kernel<<<g1, 256, 0, st>>>(ord, nr, (const int64_t *) b[SD_LEN].p, (const bm2_sort_rec *) b[SD_INFO].p, (int64_t *) b[SD_LENS].p,
                                                 (bm2_sort_rec *) b[SD_SINFO].p, d_tids, d_stids);
@@ -236,6 +283,11 @@ extern "C" int bm2_bam_sort_compress_ex(bm2_ctx *ctx, const uint8_t *recs, int64
     return 0;
 }
 
+extern "C" int bm2_bam_qname_sort_compress(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int64_t *starts, int64_t n_recs, const uint8_t *carry,
+                                           int64_t carry_len, int last, bm2_sort_out *out) {
+    return sort_compress(ctx, recs, n, starts, n_recs, nullptr, carry, carry_len, last, out, true);
+}
+
 extern "C" int bm2_last_sort_stats(const bm2_ctx *ctx, double ms[4]) {
     if (!ctx || !ms) return 1;
     for (int k = 0; k < 4; ++k) ms[k] = ctx->sort_ms[k];
@@ -258,5 +310,17 @@ extern "C" int bm2_bam_sort_memory_ex(const bm2_ctx *ctx, int64_t run_bytes, int
     BM2_CUDA_OK(cudaSetDevice(ctx->device));
     BM2_CUDA_OK(cudaMemGetInfo(&fr, &tot));
     *needed = (int64_t) bytes; *free_bytes = (int64_t) fr;
+    return 0;
+}
+
+extern "C" int bm2_bam_qname_sort_memory(const bm2_ctx *ctx, int64_t run_bytes, int64_t *needed, int64_t *free_bytes) {
+    if (bm2_bam_sort_memory(ctx, run_bytes, needed, free_bytes)) return 1;
+    bm2_ctx *ctx_for_error = (bm2_ctx *) ctx;
+    // bm2_bam_sort_memory's buffers (the 8-byte entries in its key buffer, the 4-byte ordinals in its value buffer) plus cub's merge-sort
+    // temporary storage for as many records, rounded up by 1.25 as bm2_ctx::ensure allocates
+    cudaError_t e;
+    const size_t t = qname_sort_temp((int64_t) ((double) run_bytes / kRecBytes) + 1, nullptr, &e);
+    BM2_CUDA_OK(e);
+    *needed += (int64_t) (1.25 * (double) t);
     return 0;
 }

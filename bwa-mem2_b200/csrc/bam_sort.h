@@ -9,7 +9,7 @@
 //           over the runs not yet fully loaded, r* the first such run whose last key is T; every loaded record with key < T, and those with key == T of runs up to r*, are settled.  They are
 //           concatenated in run order and sorted with the same device call (stable, so ties keep run order and then the order within the
 //           run, which is input order), passing the carry: the BGZF blocks are cut over the whole sorted stream.  r*'s last record is
-//           always settled, so every window makes progress.
+//           always settled, so every window makes progress.  With cmp set (bm2_sort -n), cmp orders the records in place of the key.
 //   BAI     (SAMv1 §5.2) from each record's (refID, pos, end, bin, flag) and virtual offset: per bin its chunks, a chunk joined to the one
 //           before when that one ends where it starts; the 16 kbp linear index, empty windows filled from the one before; pseudo-bin 37450
 //           with the reference's offset span and its mapped / unmapped counts; n_no_coor.
@@ -32,7 +32,7 @@
 //           that only the final pass (the one-run sort, or the merge windows) counts, with the records' final flags; the runs spilled
 //           before are never counted.
 //
-// The device calls are parameters, so that tests/host_emul/bam_sort_emul.cpp and markdup_emul.cpp run all of this with the GPU swapped for a
+// The device calls are parameters, so that tests/host_emul/bam_sort_emul.cpp, bamsort_emul.cpp and markdup_emul.cpp run all of this with the GPU swapped for a
 // CPU restatement.
 #pragma once
 #include "bam_sort_device.cuh"
@@ -65,6 +65,8 @@ using DupCallEx = std::function<int(const bm2_dup_loc_entry *e, int64_t n, int r
                                     int64_t *n_dups, int64_t *n_optical, double *device_s)>;
 // the duplicate bitset to the sort context (bm2_dup_set)
 using DupSetCall = std::function<int(const uint64_t *bits, int64_t n_bits)>;
+// the three-way order of two records (block_size first) that a SortCall sorts by: < 0, 0 or > 0
+using RecCmp = std::function<int(const uint8_t *a, const uint8_t *b)>;
 // reports an error and does not return
 using SortFail = std::function<void(const std::string &)>;
 
@@ -191,6 +193,7 @@ struct BamSortSink {
     DupCall dup; DupSetCall dup_set;             // --markdup when dup is set (sort_ex must be set then)
     DupCallEx dup_ex;                            // --markdup-metrics: the pair space through this one, with add_sigs_ex
     std::function<void()> before_final;          // --recal-file: called once the duplicates are known, before the one-run sort or the merge
+    RecCmp cmp;                                  // the order sort sorts by (without input order), for the merge; unset: the coordinate key
     int64_t run_bytes = (int64_t) 2 << 30;
     int64_t sig_bytes = (int64_t) 256 << 20;     // entries held on the host (--sort-mem / 8)
     int64_t n_reads = 0;                         // the duplicate bitset's bits: set before finish
@@ -472,6 +475,11 @@ struct BamSortSink {
     };
 
     static uint64_t key_at(const uint8_t *r) { const BamFixed f = bam_fixed(r); return bam_coord_key(f.rid, f.pos, f.flag); }
+    int rec_cmp(const uint8_t *a, const uint8_t *b) const {
+        if (cmp) return cmp(a, b);
+        const uint64_t x = key_at(a), y = key_at(b);
+        return x < y ? -1 : x > y ? 1 : 0;
+    }
 
     void merge(SortedWriter &w) {
         const double t0 = std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count();
@@ -523,19 +531,19 @@ struct BamSortSink {
                 }
             }
             // T and r* over the runs not fully loaded
-            bool open = false; uint64_t T = 0; size_t rs = 0;
+            bool open = false; const uint8_t *T = nullptr; size_t rs = 0;
             for (size_t r = 0; r < nr; ++r) {
                 if (c[r].next >= runs[r].members.size()) continue;
-                const uint64_t k = key_at(c[r].buf.data() + c[r].recs.back());
-                if (!open || k < T) { T = k; rs = r; open = true; }
+                const uint8_t *k = c[r].buf.data() + c[r].recs.back();
+                if (!open || rec_cmp(k, T) < 0) { T = k; rs = r; open = true; }
             }
             win.clear(); win_starts.clear(); win_tids.clear();
             for (size_t r = 0; r < nr; ++r) {
                 Cursor &x = c[r];
                 size_t k = 0;
                 while (k < x.recs.size()) {
-                    const uint64_t kk = key_at(x.buf.data() + x.recs[k]);
-                    if (open && (kk > T || (kk == T && r > rs))) break;
+                    const int o = open ? rec_cmp(x.buf.data() + x.recs[k], T) : -1;
+                    if (o > 0 || (o == 0 && r > rs)) break;
                     ++k;
                 }
                 if (!k) continue;

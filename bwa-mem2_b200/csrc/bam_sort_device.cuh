@@ -1,6 +1,6 @@
 // bam_sort_device.cuh — the per-record logic of bm2_bam_sort_compress (bam_sort.cu): a BAM record's fixed fields (SAMv1 §4.2), its
-// coordinate key and its reference end, and (host only) where the sorted records fall in the BGZF blocks.  BM2_HD functions, so that the
-// host emulation tests/host_emul/bam_sort_emul.cpp compiles the same source.
+// coordinate key and its reference end, the read-name order of bm2_bam_qname_sort_compress, and (host only) where the sorted records fall in
+// the BGZF blocks.  BM2_HD functions, so that the host emulations tests/host_emul/bam_sort_emul.cpp and bamsort_emul.cpp compile the same source.
 //
 //   key   ((uint32) refID << 32) | ((uint32) (pos + 1) << 1) | (flag & 16 ? 1 : 0): samtools' coordinate key.  A placed unmapped mate sorts at
 //         its mate's position (its refID and pos are the mate's); refID -1 sorts last.
@@ -68,6 +68,53 @@ BM2_HD bm2_sort_rec bam_sort_rec(const uint8_t *r) {
     s.block = 0; s.offset = 0; s._pad = 0;
     return s;
 }
+
+// ---- name order (bm2_bam_qname_sort_compress, bm2_sort -n): samtools sort -n ----
+// The names are compared by strnum_cmp of samtools' bam_sort.c (the 1.9-era form, recalled, not checked against samtools), bytes unsigned,
+// both names NUL-terminated: outside digits, the first differing byte decides; where both sides are on a digit, the zeros and then the equal
+// digits are skipped on each side, and then a longer digit run is greater (the first differing digit decides at equal lengths), a side still on
+// a digit is greater, and a side that has consumed fewer bytes is greater.  A name that ends first is less.  Digit runs are never parsed into
+// integers, so runs of any length compare by their length.  The order is total with the flag bits and the ordinal after the names: the host
+// merge (bam_sort.h, without the ordinal), the device sort and the host emulation all call bam_qname_cmp.
+BM2_HD bool bam_is_digit(uint8_t c) { return c >= '0' && c <= '9'; }
+
+BM2_HD int bam_strnum_cmp(const uint8_t *a, const uint8_t *b) {
+    const uint8_t *pa = a, *pb = b;
+    while (*pa && *pb) {
+        if (bam_is_digit(*pa) && bam_is_digit(*pb)) {
+            while (*pa == '0') ++pa;
+            while (*pb == '0') ++pb;
+            while (bam_is_digit(*pa) && bam_is_digit(*pb) && *pa == *pb) ++pa, ++pb;
+            if (bam_is_digit(*pa) && bam_is_digit(*pb)) {
+                int64_t i = 0;
+                while (bam_is_digit(pa[i]) && bam_is_digit(pb[i])) ++i;
+                return bam_is_digit(pa[i]) ? 1 : bam_is_digit(pb[i]) ? -1 : (int) *pa - (int) *pb;
+            }
+            if (bam_is_digit(*pa)) return 1;
+            if (bam_is_digit(*pb)) return -1;
+            if (pa - a != pb - b) return pa - a < pb - b ? 1 : -1;
+        } else {
+            if (*pa != *pb) return (int) *pa - (int) *pb;
+            ++pa; ++pb;
+        }
+    }
+    return *pa ? 1 : *pb ? -1 : 0;
+}
+
+// -1, 0 or 1: the names a and b (NUL-terminated), then flag & 0xc0 ascending, then the ordinals
+BM2_HD int bam_qname_cmp(const uint8_t *a, uint32_t fa, int64_t oa, const uint8_t *b, uint32_t fb, int64_t ob) {
+    const int c = bam_strnum_cmp(a, b);
+    if (c) return c < 0 ? -1 : 1;
+    fa &= 0xc0; fb &= 0xc0;
+    if (fa != fb) return fa < fb ? -1 : 1;
+    return oa < ob ? -1 : oa > ob ? 1 : 0;
+}
+
+// bam_qname_cmp of two records (block_size first) without the ordinal: the sink's merge order for bm2_sort -n
+BM2_HD int bam_qname_rec_cmp(const uint8_t *a, const uint8_t *b) { return bam_qname_cmp(a + 36, bam_le16(a + 18), 0, b + 36, bam_le16(b + 18), 0); }
+
+// the name-order entry of the record at r = buffer + start: the offset of its QNAME in the buffer << 8 | flag & 0xc0
+BM2_HD uint64_t bam_qname_entry(const uint8_t *r, int64_t start) { return (uint64_t) (start + 36) << 8 | (bam_le16(r + 18) & 0xc0); }
 
 // ---- host only: the blocks of the stream carry + sorted records, and each record's block and offset ----
 // carry_len bytes of the previous call's unfinished block come first (one "record" for the cut rule: only their length matters); then the

@@ -42,6 +42,7 @@
 #include "../csrc/seq_grammar.cuh"
 #include "../csrc/read_input.h"
 #include "../csrc/bam_sort.h"
+#include "../csrc/sort_header.h"
 #include "../csrc/markdup_metrics.h"
 #include "../csrc/bqsr_report.h"
 #include "../csrc/known_sites.h"
@@ -399,44 +400,6 @@ void int_pair(const char *arg, int *a, int *b) {
     if (*p != 0 && ispunct((unsigned char) *p) && isdigit((unsigned char) p[1])) *b = (int) strtol(p + 1, &p, 10);
 }
 
-// "SIZE" of --sort-mem: a positive decimal integer, optionally followed by one of K M G (binary multiples, either case)
-bool parse_size(const char *s, long long *v) {
-    char *e;
-    if (!isdigit((unsigned char) *s)) return false;
-    errno = 0;
-    const unsigned long long x = strtoull(s, &e, 10);
-    int shift = 0;
-    if (*e == 'k' || *e == 'K') shift = 10, ++e;
-    else if (*e == 'm' || *e == 'M') shift = 20, ++e;
-    else if (*e == 'g' || *e == 'G') shift = 30, ++e;
-    if (*e || errno || x == 0 || x > (unsigned long long) (INT64_MAX >> shift)) return false;
-    *v = (long long) (x << shift);
-    return true;
-}
-
-// --sort: the header's @HD line first, with SO:coordinate; an @HD line from -H keeps its other fields
-std::string coordinate_header(const std::string &h) {
-    std::string hd, rest;
-    for (size_t b = 0; b < h.size();) {
-        size_t e = h.find('\n', b); if (e == std::string::npos) e = h.size();
-        const std::string line = h.substr(b, e - b);
-        if (hd.empty() && (line == "@HD" || line.compare(0, 4, "@HD\t") == 0)) {
-            hd = "@HD";
-            bool so = false;
-            for (size_t p = 3; p < line.size();) {
-                size_t q = line.find('\t', p + 1); if (q == std::string::npos) q = line.size();
-                const std::string f = line.substr(p + 1, q - p - 1);
-                if (f.compare(0, 3, "SO:") == 0) { if (!so) hd += "\tSO:coordinate"; so = true; }
-                else hd += "\t" + f;
-                p = q;
-            }
-            if (!so) hd += "\tSO:coordinate";
-        } else rest += line + "\n";
-        b = e + 1;
-    }
-    return (hd.empty() ? std::string("@HD\tVN:1.6\tSO:coordinate") : hd) + "\n" + rest;
-}
-
 // "N" of --optical-distance: a decimal integer in [0, 2^31 - 1]
 bool parse_distance(const char *s, long long *v) {
     if (!*s || strlen(s) > 10) return false;
@@ -697,7 +660,7 @@ int main(int argc, char **argv) {
             for (size_t i = 0; i < names.size(); ++i)
                 header += "@SQ\tSN:" + names[i] + "\tLN:" + std::to_string(lens[i]) + (idx->ann_is_alt && idx->ann_is_alt[i] ? "\tAH:*\n" : "\n");
         if (have_hdr) header += hdr_line + "\n";
-        if (sort) header = coordinate_header(header);
+        if (sort) header = header_with_sort_order(header, "coordinate");
     }
     if (dump) {
         const bm2_mem_opt_t &o = opt;

@@ -449,6 +449,14 @@ int  bm2_last_sort_stats(const bm2_ctx *ctx, double ms[4]);
 int  bm2_bam_sort_memory(const bm2_ctx *ctx, int64_t run_bytes, int64_t *needed, int64_t *free_bytes);
 /* The same with with_tids != 0: plus the template ids bm2_bam_sort_compress_ex carries (8 bytes per record in, 8 sorted). */
 int  bm2_bam_sort_memory_ex(const bm2_ctx *ctx, int64_t run_bytes, int with_tids, int64_t *needed, int64_t *free_bytes);
+/* bm2_bam_sort_compress in read-name order (bm2_sort -n), the natural order of `samtools sort -n`: the QNAMEs compared by samtools'
+ * strnum_cmp (digit runs by value, never parsed: csrc/bam_sort_device.cuh), then flag & 0xc0 ascending, then input order.  Same arguments,
+ * outputs and bm2_last_sort_stats stages (ms[1]: the merge sort).  Each record's QNAME must end with its NUL inside the record. */
+int  bm2_bam_qname_sort_compress(bm2_ctx *ctx, const uint8_t *recs, int64_t n, const int64_t *starts, int64_t n_recs, const uint8_t *carry,
+                                 int64_t carry_len, int last, bm2_sort_out *out);
+/* Device bytes one bm2_bam_qname_sort_compress call on run_bytes of records of about 300 bytes needs (bm2_bam_sort_memory's, plus cub's
+ * merge-sort temporary storage), and the bytes free on ctx's device now. */
+int  bm2_bam_qname_sort_memory(const bm2_ctx *ctx, int64_t run_bytes, int64_t *needed, int64_t *free_bytes);
 
 /* ---- Duplicate marking (bm2_mem --markdup) ------------------------------------------------------------------------------------------------
  * The rule (csrc/markdup_device.cuh) follows Picard MarkDuplicates's defaults, SUM_OF_BASE_QUALITIES; optical duplicates are marked like any
